@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- GPT4RoI region-token prefill throughput on B200 (BASELINE.json metric).
+"""bench.py -- GPT4RoI region-token prefill throughput on one H100 per rank (BASELINE.json metric).
 
   python bench.py --gpus N --steps K --warmup W            (N>1: launched under torchrun, one rank/GPU)
   python bench.py --impl reference ...                     (the reference's CPU path, bounded sample)
@@ -12,6 +12,9 @@ Beside the headline the line carries, as extras measured in the same run (each u
 changes `value`): the RoIAlign microbench at the BASELINE size (configs[4], `roialign_roofline`), configs[2]'s
 16-RoI variant (`config2_16roi`), the stage-2 / stage-1 training step of configs[3] at the rank count of the run
 (`train_step`: DDP over NCCL, exposed all-reduce time), and the decode loop (`decode`, N=1 only).
+
+--dump-outputs DIR writes what the timed path returned in its last step (a fixed, seeded sample of the full
+[B, L, V] logits, see dump_outputs()) as DIR/<name>.npy, so that two builds can be compared output for output.
 """
 import argparse
 import json
@@ -36,8 +39,8 @@ def peaks():
     try:
         p = json.load(open(os.path.join(ROOT, 'MEASURED_PEAKS.json')))
         return p, 'measured'
-    except Exception:
-        return dict(hbm_gbs=6650.0, bf16_tflops=1590.0, bf16_tflops_sustained=1400.0), 'fallback'
+    except Exception:   # NVIDIA's H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense bf16
+        return dict(hbm_gbs=3350.0, bf16_tflops=989.0, bf16_tflops_sustained=989.0), 'H100 SXM data sheet'
 
 
 class ClockSampler:
@@ -155,7 +158,7 @@ def pick_cpu_threads():
 def cpu_reference_sample(repeats=3):
     """One headline sample (336 px, 8 RoIs, L = 706) on the host cores, fp32.
       * SPI module: IN FULL -- the reference's own modules (gpt4roi/models/layers.py under tests/golden/ref_shims.py)
-        when /root/reference exists, else their pinned restatement oracle/spi_oracle.py; RoIAlign = the reference's
+        when the reference tree is available ($GPT4ROI_REFERENCE), else their pinned restatement oracle/spi_oracle.py; RoIAlign = the reference's
         own cpu/roi_align.cpp compiled in place (oracle/_ref) when present, else the C port;
       * mm_projector, lm_head: in full;  ViT: 1 of 24 encoder layers x24, LLaMA: 1 of 32 decoder layers x32
         (transformers' own layers; the stacks are 24 / 32 identical layers, the whole 7B fp32 forward would need
@@ -212,7 +215,8 @@ def cpu_reference_sample(repeats=3):
     spi_fn, saved = None, None
     if ext is not None:
         kind = 'reference'
-    if os.path.isdir('/root/reference') and not tiny:
+    from oracle import build_ref
+    if build_ref.reference_present() and not tiny:
         try:   # the reference's OWN MLVLROIQueryModule (unmodified; 336: the three literals lifted, SURVEY 8(c))
             from tests.golden import ref_shims
             mod = ref_shims.build_roi_query_module(S)
@@ -295,50 +299,52 @@ def roialign_microbench(dev, pk, how, n_maps=256, rois_per_map=100):
     rois = torch.from_numpy(np.concatenate(rows).astype(np.float32)).to(dev)
     K = rois.shape[0]
     scales = [float(np.float32(1.0 / s)) for s in (14 / 8, 14 / 4, 14 / 2, 14)]
-    flush = torch.zeros(256 * 1024 * 1024 // 4, device=dev)   # 256 MiB > 126 MB L2, rewritten between iterations
+    flush = torch.zeros(256 * 1024 * 1024 // 4, device=dev)   # 256 MiB > 50 MB L2, rewritten between iterations
 
     def run(dtype, ph):
-        maps = [torch.randn(n_maps, h, h, C, device=dev, dtype=dtype) for h in sizes]
-        out = torch.empty((4, K, ph, ph, C), device=dev, dtype=dtype)
+        # the output of every RoI must fit beside the maps: with fewer maps than n_maps (the fp32 14x14 variant would need
+        # 82 GB of output alone) the launch covers the first n_used maps and their RoIs
+        esz = torch.tensor([], dtype=dtype).element_size()
+        free = torch.cuda.mem_get_info(dev)[0] - 2 * 1024 ** 3
+        per_map = (sum(h * h for h in sizes) * C + 4 * rois_per_map * ph * ph * C) * esz
+        n_used = min(n_maps, int(free // per_map))
+        k_used = n_used * rois_per_map
+        maps = [torch.randn(n_used, h, h, C, device=dev, dtype=dtype) for h in sizes]
+        r = rois[:k_used]
+        out = torch.empty((4, k_used, ph, ph, C), device=dev, dtype=dtype)
         for _ in range(3):
-            g.roi_align_mlvl(maps, rois, ph, scales, 2, out=out)
+            g.roi_align_mlvl(maps, r, ph, scales, 2, out=out)
         torch.cuda.synchronize(dev)
         ts = []
         for _ in range(5):
             flush.add_(1)
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             e0.record()
-            g.roi_align_mlvl(maps, rois, ph, scales, 2, out=out)
+            g.roi_align_mlvl(maps, r, ph, scales, 2, out=out)
             e1.record()
             torch.cuda.synchronize(dev)
             ts.append(e0.elapsed_time(e1))
         ms = sorted(ts)[len(ts) // 2]
-        alg = sum(m.numel() for m in maps) * maps[0].element_size() + out.numel() * out.element_size() + K * 20
+        alg = sum(m.numel() for m in maps) * maps[0].element_size() + out.numel() * out.element_size() + k_used * 20
         del maps, out
         torch.cuda.empty_cache()
-        return ms, alg
-    ms, alg = run(torch.float32, 7)
+        return ms, alg, n_used
+    ms, alg, n_used = run(torch.float32, 7)
     ach = alg / 1e9 / (ms / 1e3)
     others = {}
     for name, dt, ph in (('fp32_14x14', torch.float32, 14), ('bf16_7x7', torch.bfloat16, 7), ('bf16_14x14', torch.bfloat16, 14)):
         try:
-            m2, a2 = run(dt, ph)
-            others[name] = dict(ms=m2, achieved=a2 / 1e9 / (m2 / 1e3), frac=a2 / 1e9 / (m2 / 1e3) / pk['hbm_gbs'])
+            m2, a2, n2 = run(dt, ph)
+            others[name] = dict(ms=m2, achieved=a2 / 1e9 / (m2 / 1e3), frac=a2 / 1e9 / (m2 / 1e3) / pk['hbm_gbs'], maps=n2)
         except Exception as e:
             others[name] = dict(skipped=str(e)[:120])
-    traffic, tsrc = None, None
-    try:
-        tj = json.load(open(os.path.join(ROOT, 'profiles', 'r2_roialign_traffic.json')))
-        traffic, tsrc = tj['traffic_bytes_per_launch'], tj['source']
-    except Exception:
-        pass
     del flush
     torch.cuda.empty_cache()
     return dict(bound='hbm', kernel='roi_align_fwd_nhwc_mlvl_dedup', achieved=ach, peak=pk['hbm_gbs'], unit='GB/s',
                 frac=ach / pk['hbm_gbs'], peak_kind=how, ms=ms, algorithmic_GB=alg / 1e9,
                 config='%d maps x %d RoIs, 7x7, 4 levels x 1024 ch (128,64,32,16), fp32 NHWC, L2 flushed between launches'
-                       % (n_maps, rois_per_map),
-                traffic=traffic, traffic_source=tsrc, variants=others)
+                       % (n_used, rois_per_map),
+                variants=others)
 
 
 def run_reference(args):
@@ -456,7 +462,16 @@ def train_extra(dev, world, rank, steps=4, warmup=2, batch=4, stage1=True):
         variants.append(('stage2_sharded_optimizer', dict(trainable=('embed', 'proj', 'spi', 'llama', 'head'), shard_optimizer=True)))
     if stage1:
         variants.append(('stage1_only_spi', dict(trainable=('spi',), spi_decay_all=0.01)))
+    hbm_gb = torch.cuda.get_device_properties(dev).total_memory / 1e9
     for name, kw in variants:
+        # per-GPU state of the 7.04 B trainable parameters (DESIGN.md section 7, the sum of its parts, ~126 GB on one rank):
+        # bf16 weights + gradients + activations ~42 GB, fp32 masters + AdamW moments 84.5 GB (1/world of that with the
+        # sharded optimizer).  ONLY_SPI: 34 GB, the peak measured on an H100 80GB
+        need_gb = 34.0 if name == 'stage1_only_spi' else 42.0 + 84.5 / (world if kw.get('shard_optimizer') else 1)
+        if need_gb > 0.95 * hbm_gb:
+            out[name] = dict(skipped='needs ~%.0f GB per GPU, the device has %.0f GB; run with more ranks (the sharded '
+                                     'optimizer divides the optimizer state by the rank count)' % (need_gb, hbm_gb))
+            continue
         torch.cuda.empty_cache()
         torch.cuda.reset_peak_memory_stats(dev)
         sd, vit_sd = random_state_dicts(cfg, dev, seed=0)           # same weights on every rank
@@ -485,6 +500,21 @@ def train_extra(dev, world, rank, steps=4, warmup=2, batch=4, stage1=True):
     out['config'] = ('configs[3]: 336 px, 8 RoIs/img, 128 text tokens (L=706), 7B, bf16 compute, fp32 masters + AdamW, '
                      'grad-norm clip 1.0, cosine LR, DDP x%d (one flat bf16 bucket per decoder layer over NCCL)' % world)
     return out
+
+
+def dump_outputs(out_dir, logits, n_rows=256):
+    """The timed path returns the full [B, L, V] logits (361 MB in bf16).  Written as float32: a fixed, seeded sample
+    of n_rows (batch, position) rows with the whole vocabulary (logits_rows.npy, [n_rows, V]; the flat row indices in
+    logits_row_index.npy) and the arg-max token of every position (argmax.npy, [B, L]) -- 33 MB in all."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    B, L, V = logits.shape
+    rows = torch.randperm(B * L, generator=torch.Generator().manual_seed(1234))[:n_rows].sort().values
+    flat = logits.reshape(B * L, V)
+    np.save(os.path.join(out_dir, 'logits_rows.npy'), flat[rows.to(flat.device)].float().cpu().numpy())
+    np.save(os.path.join(out_dir, 'logits_row_index.npy'), rows.numpy().astype(np.float64))
+    np.save(os.path.join(out_dir, 'argmax.npy'), logits.argmax(-1).float().cpu().numpy())
 
 
 def run_ours(args):
@@ -552,6 +582,8 @@ def run_ours(args):
     barrier()
     ms_total = max_over_ranks(e0.elapsed_time(e1))
     clocks = sampler.stop() if sampler else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, graph.out)
     ms_step = ms_total / args.steps
     value = world * B / (ms_step / 1e3)
 
@@ -592,7 +624,7 @@ def run_ours(args):
     del h_out, d_snap
     torch.cuda.empty_cache()
 
-    # ---- roofline of the dominant kernel (tcgen05 GEMM / implicit-GEMM conv): one instrumented
+    # ---- roofline of the dominant kernel (wgmma GEMM / implicit-GEMM conv): one instrumented
     #      eager step with CUDA events around every launch on the launching stream ------------
     dense.PROFILE = []
     plan = eng.plan_boxes(boxes)
@@ -602,17 +634,9 @@ def run_ours(args):
     gemm_ms = sum(s.elapsed_time(e) for _, _, s, e in prof)
     gemm_flops = sum(f for _, f, _, _ in prof)
     achieved = gemm_flops / 1e12 / (gemm_ms / 1e3)
-    traffic, traffic_src = None, None
-    for name in ('r2_gemm_traffic.json', 'r1_gemm_traffic.json'):
-        try:  # dram__bytes_read+write per launch from the committed ncu --set full capture of this kernel
-            tj = json.load(open(os.path.join(ROOT, 'profiles', name)))
-            traffic, traffic_src = tj['traffic_bytes_per_launch_avg'], tj['source']
-            break
-        except Exception:
-            pass
-    roof = dict(bound='tensor', kernel='gemm_bf16_tcgen05', achieved=achieved, peak=pk['bf16_tflops_sustained'],
-                unit='TFLOP/s', frac=achieved / pk['bf16_tflops_sustained'], traffic=traffic, traffic_source=traffic_src,
-                peak_kind=how + ' (sustained cuBLAS bf16; kernel timed inside a long step)',
+    roof = dict(bound='tensor', kernel='gemm_bf16_wgmma', achieved=achieved, peak=pk['bf16_tflops_sustained'],
+                unit='TFLOP/s', frac=achieved / pk['bf16_tflops_sustained'],
+                peak_kind=how + ' (bf16; kernel timed inside a long step)',
                 launches=len(prof), flops_per_launch_avg=gemm_flops / max(len(prof), 1),
                 avg_launch_ms=gemm_ms / max(len(prof), 1), share_of_step=gemm_ms / ms_step,
                 note='events around each launch in one eager instrumented step after the timed region')
@@ -671,7 +695,7 @@ def run_ours(args):
                                      'CLIP-ViT-L/14 + SPI + LLaMA-7B (%d layers) + lm_head, full logits' %
                                      (B, K, T, L, cfg.n_layers),
                             global_batch=world * B, seq_len=L, parallelism='replicas x%d (batch split, no collective)' % world,
-                            l2='weights (14.6 GB) >> 126 MB L2: inputs larger than L2, no explicit flush',
+                            l2='weights (14.6 GB) >> 50 MB L2: inputs larger than L2, no explicit flush',
                             cuda_graph=True, flops_per_sample=FLOPS_PER_SAMPLE),
                 clocks=clocks, gpu_launches=launches_per_step * args.steps,
                 e2e=dict(value=world * B / (e2e_ms / 1e3), unit='samples/s', h2d_bytes_per_step=h2d,
@@ -700,6 +724,8 @@ def main():
     ap.add_argument('--no-extras', action='store_true', help='headline only (no config2 / decode / train_step extras)')
     ap.add_argument('--no-train', action='store_true')
     ap.add_argument('--ncu', action='store_true', help='one eager forward inside a cudaProfiler window')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='write the last timed step\'s outputs (seeded sample of the logits) as DIR/<name>.npy')
     args = ap.parse_args()
     if args.impl == 'reference':
         run_reference(args)

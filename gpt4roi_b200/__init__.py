@@ -1,4 +1,4 @@
-"""gpt4roi_b200 -- B200 (sm_100a) implementation of GPT4RoI's region-token forward path.
+"""gpt4roi_b200 -- H100 (sm_90a) implementation of GPT4RoI's region-token forward path.
 
 Host code is Python/PyTorch (device memory, streams, torch.distributed plumbing); the
 compute is hand-written CUDA behind the C ABI in include/gpt4roi_b200.h

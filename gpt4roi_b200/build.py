@@ -1,7 +1,7 @@
-"""Build libgpt4roi_b200.so (sm_100a only) in-tree with nvcc.
+"""Build libgpt4roi_b200.so (sm_90a only) in-tree with nvcc.
 
 `python -m gpt4roi_b200.build [--force] [--verbose]`.  nvcc cross-compiles without a
-GPU; the .so is git-ignored but travels to the GPU box with gpurun.
+GPU; the .so and the object files are build products and stay out of git.
 """
 import concurrent.futures
 import os
@@ -14,7 +14,7 @@ CSRC = os.path.join(PKG, 'csrc')
 OBJ = os.path.join(PKG, 'build')
 LIB = os.path.join(PKG, 'libgpt4roi_b200.so')
 
-ARCH = ['-gencode', 'arch=compute_100a,code=sm_100a']
+ARCH = ['-gencode', 'arch=compute_90a,code=sm_90a']
 COMMON = ['-O3', '-std=c++17', '-lineinfo', '-Xcompiler', '-fPIC', '--expt-relaxed-constexpr',
           '-Xptxas', '-v']
 # per-file extra flags.  roi_align.cu: no FMA contraction (bit-exact bin/weight arithmetic).
@@ -23,7 +23,7 @@ EXTRA = {
 }
 # The inference kernels are built twice: bf16 as written, and an fp16 twin (-DG4R_ACT_HALF, csrc/act_type.cuh) for the
 # demo's dtype (gpt4roi/app.py:74-98: model.half()).  Both land in the one shared library.
-FP16_TWINS = ('gemm_tcgen05.cu', 'attention_tcgen05.cu', 'attention.cu', 'elementwise.cu', 'gemm_skinny.cu', 'decode.cu')
+FP16_TWINS = ('gemm_wgmma.cu', 'attention_wgmma.cu', 'attention.cu', 'elementwise.cu', 'gemm_skinny.cu', 'decode.cu')
 
 
 def nvcc():

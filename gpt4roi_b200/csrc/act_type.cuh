@@ -2,12 +2,12 @@
 //
 // The demo serves the model in fp16 (gpt4roi/app.py:74-98,271: `model.half()`, `images.half()`, `bboxes.half()`), the
 // training scripts and everything else in bf16 (train_stage*.sh --bf16 True).  The six inference sources
-// (gemm_tcgen05.cu, attention_tcgen05.cu, attention.cu, elementwise.cu, gemm_skinny.cu, decode.cu) are therefore built
+// (gemm_wgmma.cu, attention_wgmma.cu, attention.cu, elementwise.cu, gemm_skinny.cu, decode.cu) are therefore built
 // twice: as written (bf16), and with -DG4R_ACT_HALF, where this header -- included AFTER common.cuh / ptx.cuh --
 // retargets the type, its conversion intrinsics, the tensor-core operand format and the exported names to fp16:
 //   * every kernel keeps fp32 accumulation and the same rounding points ("round to the storage type" is now fp16);
-//   * tcgen05 kind::f16 takes either format, selected by the instruction descriptor (a_format / b_format 0 = F16,
-//     1 = BF16); mma.sync switches its .bf16 operand qualifier to .f16; TMA tensor maps carry the matching data type;
+//   * wgmma and mma.sync switch their .bf16 operand qualifier to .f16 (G4R_ACT_PTX); TMA tensor maps carry the
+//     matching data type;
 //   * the C entry points get an _f16 name (`g4r_gemm_bf16` -> `g4r_gemm_f16`, `g4r_rmsnorm_ex` -> `g4r_rmsnorm_ex_f16`)
 //     with identical signatures (include/gpt4roi_b200.h), and the C++ symbols move to namespace g4r_h;
 //   * entry points only the training step uses are not built for fp16 (G4R_BF16_ONLY).
@@ -24,7 +24,6 @@
 #define __float2bfloat16_rn __float2half_rn
 #define __floats2bfloat162_rn __floats2half2_rn
 #define __bfloat1622float2 __half22float2
-#define make_idesc_bf16_f32 make_idesc_f16_f32
 #define CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 CU_TENSOR_MAP_DATA_TYPE_FLOAT16
 
 #define g4r_gemm_bf16 g4r_gemm_f16

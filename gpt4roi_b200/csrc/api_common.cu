@@ -20,10 +20,10 @@ int cuda_fail(cudaError_t e, const char* what) {
 int num_sms() {
   static int cached[64] = {0};
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
   if (cached[dev] == 0) {
     int n = 0;
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
     cached[dev] = n;
   }
   return cached[dev];
@@ -70,4 +70,4 @@ extern "C" int g4r_set_sm_reserve(int n_sms) {
 
 extern "C" const char* g4r_last_error(void) { return g4r::g_err; }
 extern "C" int g4r_version(void) { return 1000; }
-extern "C" int g4r_built_arch(void) { return 100; }
+extern "C" int g4r_built_arch(void) { return 90; }

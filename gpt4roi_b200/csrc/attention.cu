@@ -6,7 +6,7 @@
 //
 // Round-1 implementation note (DESIGN.md "attention"): attention is ~1.5 % of the path's FLOPs
 // (SURVEY.md App. B), so this first version uses warp-level mma.sync.m16n8k16 tiles (legacy tensor
-// path, HMMA) with cp.async double buffering; the tcgen05/TMEM version is scheduled after the GEMMs.
+// path, HMMA) with cp.async double buffering; the wgmma version (attention_wgmma.cu) is the default.
 // Numerics: QK^T accumulates in fp32 and the scaled scores stay fp32 through the softmax (the
 // reference rounds them to bf16 twice -- after the matmul and after *scale -- which only adds
 // noise); P is cast to bf16 before the PV product like the reference, the output is rounded once.

@@ -1,4 +1,4 @@
-// common.cuh -- shared helpers for the sm_100a kernels of libgpt4roi_b200.so
+// common.cuh -- shared helpers for the sm_90a kernels of libgpt4roi_b200.so
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>

@@ -1,4 +1,4 @@
-// elementwise.cu -- the HBM-bound glue of the region-token path (sm_100a): normalisations,
+// elementwise.cu -- the HBM-bound glue of the region-token path (sm_90a): normalisations,
 // rotary embedding, patchify, bilinear resampling / channel shuffle, GroupNorm finalisation and
 // the small box-position MLP.  bf16 in / bf16 out, fp32 math, 128-bit accesses.
 //

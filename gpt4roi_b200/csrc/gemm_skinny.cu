@@ -2,13 +2,13 @@
 // generate(), SURVEY.md 8(f1): one new token per sample, gpt4roi/models/spi_llava.py:47-48 skips the
 // vision branch so the step is the 7B LLaMA stack at M = batch).
 //
-// D[M, N] = A[M, K] . W[N, K]^T with the epilogues of gemm_tcgen05.cu (bias, residual, SwiGLU,
-// fused RoPE).  At M <= 16 a 128-row tcgen05 tile wastes the tensor pipe and, worse, gives one CTA
+// D[M, N] = A[M, K] . W[N, K]^T with the epilogues of gemm_wgmma.cu (bias, residual, SwiGLU,
+// fused RoPE).  At M <= 16 a 128-row wgmma tile wastes the tensor pipe and, worse, gives one CTA
 // per 256 weight rows: too few CTAs to keep HBM busy (measured 1.7 TB/s).  This kernel is HBM-bound
 // by construction: every weight byte is read exactly once with 16-byte streaming loads
 // (ld.global.nc.L1::no_allocate), hundreds of CTAs each cover 16/32 weight rows over the whole K, and
 // the warps of a CTA split K.  The arithmetic rides on mma.sync m16n8k16 with the weight rows as the
-// 16-row operand and the (<= 8) activation rows as the 8-column operand -- tcgen05 has no shape this
+// 16-row operand and the (<= 8) activation rows as the 8-column operand -- wgmma has no shape this
 // small (M >= 64) and the kernel is nowhere near compute-bound (2*M flop per weight byte pair).
 //
 // k-permutation trick: the MMA contracts over "logical" k and does not care which physical k each
@@ -18,8 +18,7 @@
 //
 // Optional split-K over a thread-block cluster (G4R_SKINNY_CTAS=<target CTA count>): the KS CTAs of a
 // cluster (gridDim.y) share one weight-row tile and interleave its k-blocks; partial sums meet in rank 0
-// through distributed shared memory.  Measured slower than KS=1 on B200 (profiles/r1_decode_kernels.md),
-// so it is off by default; bytes in flight per SM come from 16-warp CTAs on the narrow-N shapes instead.
+// through distributed shared memory.  Off by default (the extra reduction did not pay for itself); bytes in flight per SM come from 16-warp CTAs on the narrow-N shapes instead.
 // Deterministic: partial sums of the warps and of the cluster ranks are added in fixed order.
 #include "common.cuh"
 #include <cooperative_groups.h>
@@ -265,7 +264,7 @@ gemm_skinny_bf16(const SkinnyParams p) {
       const float v1 = total(r, m), v2 = total(16 + r, m);
       __nv_bfloat16* o = p.D + (long long)m * p.ldd;
       if (n1 < p.rope_cols) {
-        // rounding points as in the tcgen05 epilogue / transformers modeling_llama.py:138-168
+        // rounding points as in the wgmma GEMM epilogue / transformers modeling_llama.py:138-168
         const int pos = (p.rope_pos_dev ? *p.rope_pos_dev : p.rope_pos0) + m % p.rope_L;
         const int d = n1 & 127;
         const __nv_bfloat16* ct = p.rope_cos + (long long)pos * 128;
@@ -353,7 +352,7 @@ static bool wide_prefers_8_warps(int tiles) {
   return waste(w8) < 0.95 * waste(w4);
 }
 
-// Called by gemm_impl (gemm_tcgen05.cu) when the shape qualifies; returns -1 when it does not.
+// Called by gemm_impl (gemm_wgmma.cu) when the shape qualifies; returns -1 when it does not.
 int gemm_skinny_dispatch(const void* A, long long lda, const void* B, long long ldb, void* D, long long ldd, int M,
                          int N, int K, const void* bias, int bias_f32, const void* residual, long long ldr, int act,
                          const void* rope_cos, const void* rope_sin, int rope_cols, int rope_L, int rope_pos0,
@@ -381,8 +380,8 @@ int gemm_skinny_dispatch(const void* A, long long lda, const void* B, long long 
   }
   const unsigned grid = (unsigned)((N + 15) / 16);
   // 16-row tiles give few CTAs (N/16 = 256 for the 4096-row projections).  M <= 8: 8 warps with two k-blocks in flight
-  // each (128 registers -> 2 CTAs per SM, so all 256 CTAs are resident at once and request half the matrix up front):
-  // o_proj 11.4 -> 8.4 us, down_proj 21.5 -> 17.8 us (B200, profiles/r2_decode_pdl_depth.md).  M <= 16: 16 warps.
+  // each (128 registers -> 2 CTAs per SM, so all 256 CTAs are resident at once and request half the matrix up front).
+  // M <= 16: 16 warps.
   return M <= 8 ? launch_skinny<1, 1, 8, false, false, 2>(p, grid, st) : launch_skinny<1, 2, 16, false>(p, grid, st);
 }
 

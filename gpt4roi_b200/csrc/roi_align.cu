@@ -1,4 +1,4 @@
-// roi_align.cu -- RoIAlign forward/backward for sm_100a (HBM-bound gather / scatter-add).
+// roi_align.cu -- RoIAlign forward/backward for sm_90a (HBM-bound gather / scatter-add).
 //
 // THIS TRANSLATION UNIT IS COMPILED WITH -fmad=false: the bin / sample / weight
 // arithmetic below is written with the reference's association and must not be
@@ -6,13 +6,13 @@
 // to the reference CPU kernel (mmcv-1.4.7/mmcv/ops/csrc/pytorch/cpu/roi_align.cpp)
 // -- checked by tests/test_roi_align_gpu.py against the CPU checker.
 //
-// Replaces (reference, relative to /root/reference/mmcv-1.4.7/mmcv/ops/csrc):
+// Replaces (reference, relative to mmcv-1.4.7/mmcv/ops/csrc of the reference checkout):
 //   common/cuda/roi_align_cuda_kernel.cuh:17-108   roi_align_forward_cuda_kernel
 //   common/cuda/roi_align_cuda_kernel.cuh:111-210  roi_align_backward_cuda_kernel
 //   common/cuda/common_cuda_helper.hpp:28-119      bilinear_interpolate(_gradient)
 //   pytorch/cuda/roi_align_cuda.cu:5-57            launchers
 //
-// Design (B200): the reference runs one thread per output scalar and recomputes the
+// Design: the reference runs one thread per output scalar and recomputes the
 // RoI geometry in every thread.  Here the geometry is separable: a sample's y depends
 // on (ph,iy) only and its x on (pw,ix) only, so a CTA computes PH*gh + PW*gw axis
 // entries {lo,hi,frac,1-frac,valid} once into shared memory and every thread reuses
@@ -315,14 +315,14 @@ __device__ __forceinline__ void store_vec(Tout* p, const float (&v)[N]) {
   }
 }
 
-// ---- packed fp32x2 arithmetic (Blackwell FMUL2 / FFMA2: two IEEE fp32 lanes per instruction) ----------
-// The forward is bound by the fma pipe, not by HBM: the reference association
+// ---- channel-pair fp32 arithmetic ----------------------------------------------------------------------
+// The reference association
 //   val = ((w1*v1 + w2*v2) + w3*v3) + w4*v4;  acc += val          (roi_align.cpp:70-78 / cuda_kernel.cuh:63-66)
 // is 8 dependent-rounding fp32 ops per channel-sample and must not be contracted into FMAs to stay
-// bit-exact with the reference CPU kernel.  Two channels per instruction halves the pipe time.
-// ptxas contracts mul.rn.f32x2 + add.rn.f32x2 into FFMA2 even under --fmad=false (seen in SASS), so the
-// unfused add is spelled fma(a, one, b) with `one` == 1.0f supplied at run time: a*1 is exact, the single
-// rounding is that of a + b, and there is no multiply left to contract.
+// bit-exact with the reference CPU kernel.  The kernels carry channels in pairs (one 64-bit register pair);
+// sm_90 has no packed fp32 instructions, so each helper issues one explicitly rounded scalar op per lane,
+// which ptxas never contracts.  The unfused add is spelled fma(a, one, b) with `one` == 1.0f supplied at run
+// time: a*1 is exact, the single rounding is that of a + b, and there is no multiply left to contract.
 using f32x2 = unsigned long long;
 __device__ __forceinline__ f32x2 pack2(float a, float b) {
   f32x2 r;
@@ -333,19 +333,24 @@ __device__ __forceinline__ void unpack2(f32x2 v, float& a, float& b) {
   asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(v));
 }
 __device__ __forceinline__ f32x2 mul2(f32x2 a, f32x2 b) {
-  f32x2 r;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
+  float a0, a1, b0, b1, r0, r1;
+  unpack2(a, a0, a1);
+  unpack2(b, b0, b1);
+  asm("mul.rn.f32 %0, %1, %2;" : "=f"(r0) : "f"(a0), "f"(b0));
+  asm("mul.rn.f32 %0, %1, %2;" : "=f"(r1) : "f"(a1), "f"(b1));
+  return pack2(r0, r1);
 }
 __device__ __forceinline__ f32x2 fma2(f32x2 a, f32x2 b, f32x2 c) {
-  f32x2 r;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-  return r;
+  float a0, a1, b0, b1, c0, c1, r0, r1;
+  unpack2(a, a0, a1);
+  unpack2(b, b0, b1);
+  unpack2(c, c0, c1);
+  asm("fma.rn.f32 %0, %1, %2, %3;" : "=f"(r0) : "f"(a0), "f"(b0), "f"(c0));
+  asm("fma.rn.f32 %0, %1, %2, %3;" : "=f"(r1) : "f"(a1), "f"(b1), "f"(c1));
+  return pack2(r0, r1);
 }
 __device__ __forceinline__ f32x2 add2_unfused(f32x2 a, f32x2 b, f32x2 one) {
-  f32x2 r;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(one), "l"(b));
-  return r;
+  return fma2(a, one, b);
 }
 
 // 16-byte read-only global load with an explicit state space (the hoisted row pointers pass through an
@@ -1024,13 +1029,10 @@ static int launch_fwd_mlvl(MlvlParams& p, bool affine, cudaStream_t st) {
     nv_env = e ? atoi(e) : 0;
   }
   // 2 vectors per thread only for fp32 maps (8 channels/thread); 16-bit maps already carry 8 per vector
-  // measured on B200 (profiles/r1_roialign_microbench_v3.jsonl): 2 vectors/thread is 25 % SLOWER (fewer
-  // threads per bin => less latency hiding), so it stays opt-in (G4R_ROI_NV=2)
+  // 2 vectors/thread means fewer threads per bin => less latency hiding, so it stays opt-in (G4R_ROI_NV=2)
   const bool nv2 = sizeof(Tin) == 4 && p.C % (2 * VEC) == 0 && p.C / (2 * VEC) >= 32 && nv_env == 2;
-  // The row-walk kernel (fewer L1 wavefronts, but on-demand loads at 3 CTAs/SM) measured 9.7 ms against the
-  // table kernel's 7.6 ms on the BASELINE microbench (profiles/r1_roialign_microbench_v5.jsonl); an in-bin
-  // tap-dedup variant of the table kernel measured 10.7 ms.  Both lose to plain occupancy, so the walk kernel
-  // is opt-in (G4R_ROI_WALK=1) and the dedup variant was dropped.
+  // The row-walk kernel (fewer L1 wavefronts, but on-demand loads at 3 CTAs/SM) trades occupancy for fewer
+  // wavefronts, so it is opt-in (G4R_ROI_WALK=1).
   static int walk_env = -1;
   if (walk_env < 0) {
     const char* e = getenv("G4R_ROI_WALK");

@@ -1,4 +1,4 @@
-// splice.cu -- embedding gather + image-span splice + <bbox> region-token scatter (sm_100a).
+// splice.cu -- embedding gather + image-span splice + <bbox> region-token scatter (sm_90a).
 //
 // Replaces the per-sample python loop of gpt4roi/models/spi_llava.py:99-196 (and the
 // embed_tokens lookup at :44-45): ~10 small launches, three full-row copies and several

@@ -1,7 +1,7 @@
 // train.cu -- the non-GEMM kernels of the stage-2 training step (SURVEY.md 8(a) row 14:
 // gpt4roi/train/train.py:698-712 drives HF Trainer over SPILlavaMPTForCausalLM; the loss is
 // llava/model/llava.py:238-249: shift logits/labels, CrossEntropyLoss() = mean over labels != -100).
-// Backward GEMMs are g4r_gemm_bf16_t (gemm_tcgen05.cu).  Everything here is HBM-bound elementwise /
+// Backward GEMMs are g4r_gemm_bf16_t (gemm_wgmma.cu).  Everything here is HBM-bound elementwise /
 // row-reduction work: 16-byte vector loads, fp32 math, fixed-order reductions (no atomics, bitwise
 // reproducible), bf16 storage like the reference's bf16 autocast.
 #include "common.cuh"

@@ -1,7 +1,7 @@
-"""Dense contractions (nn.Linear / nn.Conv2d replacements) on the tcgen05 kernels.
+"""Dense contractions (nn.Linear / nn.Conv2d replacements) on the wgmma kernels.
 
 Thin torch-tensor front-ends of `g4r_gemm_bf16` / `g4r_conv_nhwc_bf16`
-(csrc/gemm_tcgen05.cu).  bf16 operands (or fp16 throughout: the `_f16` twins, for the demo's dtype), fp32
+(csrc/gemm_wgmma.cu).  bf16 operands (or fp16 throughout: the `_f16` twins, for the demo's dtype), fp32
 accumulation; no library GEMM is called.
 """
 import torch

@@ -1,5 +1,5 @@
 """Region-token prefill engine: CLIP-ViT-L/14 -> MLVL fuse -> multi-level RoIAlign -> region
-projector -> splice -> LLaMA prefill -> lm_head, every op a hand-written sm_100a kernel behind
+projector -> splice -> LLaMA prefill -> lm_head, every op a hand-written sm_90a kernel behind
 the C ABI.  PyTorch supplies device memory, streams and CUDA-graph capture only.
 
 Reference call stack reproduced (SURVEY.md 3.3):
@@ -38,8 +38,8 @@ class EngineConfig:
         twins of every kernel (csrc/act_type.cuh), same fp32 accumulation and rounding points.
         llama_stream: dtype of the LLaMA residual stream in the prefill -- 'bf16' (default: what the reference has
         when the model was cast to bf16, the BASELINE "7B bf16 prefill" mode) or 'fp32' (what the reference has
-        whenever its parameters are fp32 under autocast; 25 % closer to the fp32 anchor at 32 layers, 2.4 % slower:
-        tests/test_parity_7b_gpu.py, profiles/r2_bench_stream_ab.json).  Env G4R_LLAMA_STREAM overrides the default."""
+        whenever its parameters are fp32 under autocast; closer to the fp32 anchor at 32 layers, somewhat slower:
+        tests/test_parity_7b_gpu.py).  Env G4R_LLAMA_STREAM overrides the default."""
         import os
         if llama_stream is None:
             llama_stream = os.environ.get('G4R_LLAMA_STREAM', 'bf16')
@@ -420,9 +420,8 @@ def _decode_step_chain(self, token_ids, cache, pos_dev):
     scale = c.head_dim ** -0.5
     fused = c.head_dim == 128 and (2 * c.hidden) % 256 == 0
     # KV-cache append folded into the q|k|v GEMM's RoPE epilogue (7 launches per layer instead of 8).  Folding the two
-    # RMSNorms into the GEMMs as well (G4R_DECODE_FUSED=2: 5 launches) measured SLOWER on B200 -- 4.57 vs 3.58 ms/token:
-    # the per-fragment normalisation sits between the weight-streaming loads of a kernel that lives on memory-level
-    # parallelism (profiles/r2_decode_fusion.md) -- so it stays opt-in.  G4R_DECODE_FUSED=0: the round-1 sequence.
+    # RMSNorms into the GEMMs as well (G4R_DECODE_FUSED=2: 5 launches) puts the per-fragment normalisation between the
+    # weight-streaming loads of a kernel that lives on memory-level parallelism, so it stays opt-in.  G4R_DECODE_FUSED=0: the round-1 sequence.
     fuse_step = fused and B <= 16 and c.hidden % 256 == 0 and _DECODE_FUSED > 0
     for li, w in enumerate(self.layers):
         if fuse_step:

@@ -74,7 +74,7 @@ class BatchPreprocessor:
         self.S, self.dev, self.out_dtype, self.to_rgb = int(S), torch.device(device), out_dtype, bool(to_rgb)
         if self.dev.type != 'cuda':
             raise RuntimeError('gpt4roi_b200.input_pipeline: device %s -- implementation for device %s not found '
-                               '(CUDA sm_100a only; no CPU fallback)' % (self.dev, self.dev.type))
+                               '(CUDA sm_90a only; no CPU fallback)' % (self.dev, self.dev.type))
         import ctypes
         self._mean = (ctypes.c_float * 3)(*[float(np.float32(m)) for m in mean])   # float32, as mmdet's Normalize stores them
         self._std = (ctypes.c_float * 3)(*[float(np.float32(s)) for s in std])

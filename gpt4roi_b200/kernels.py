@@ -79,7 +79,7 @@ def rope_inplace(qkv, cos, sin, L, n_heads_qk, head_dim):
     return qkv
 
 
-ATTN_IMPL = __import__('os').environ.get('G4R_ATTN', 'tc')  # 'tc' = tcgen05 kernel, 'mma' = mma.sync kernel
+ATTN_IMPL = __import__('os').environ.get('G4R_ATTN', 'tc')  # 'tc' = wgmma kernel, 'mma' = mma.sync kernel
 
 
 def attention(qkv, B, L, n_heads, head_dim, causal, scale, out=None, seqlens=None, impl=None):

@@ -156,7 +156,7 @@ def load():
     if not os.path.isfile(LIB_PATH):
         raise ImportError(
             'gpt4roi_b200: %s is missing. Build it with `python -m gpt4roi_b200.build` '
-            '(needs nvcc; cross-compiles for sm_100a without a GPU). There is no CPU or '
+            '(needs nvcc; cross-compiles for sm_90a without a GPU). There is no CPU or '
             'PyTorch fallback for this path.' % LIB_PATH)
     lib = ctypes.CDLL(LIB_PATH)
     for name, (res, args) in SIGNATURES.items():
@@ -204,7 +204,7 @@ def require_cuda_same_device(named):
             if not t.is_cuda:
                 raise RuntimeError(
                     'gpt4roi_b200: %s is on %s -- implementation for device %s not found '
-                    '(this library is CUDA sm_100a only; no CPU fallback)' % (name, t.device, t.device.type))
+                    '(this library is CUDA sm_90a only; no CPU fallback)' % (name, t.device, t.device.type))
         elif t.device != first.device:
             raise RuntimeError('gpt4roi_b200: arg %d (%s) is on %s but arg 0 is on %s'
                                % (idx, name, t.device, first.device))

@@ -1,5 +1,5 @@
 """`mmcv._ext` drop-in: lets the reference's own `mmcv.ops.roi_align` / `RoIAlign`
-(mmcv-1.4.7/mmcv/ops/roi_align.py) run UNCHANGED on the sm_100a kernels.
+(mmcv-1.4.7/mmcv/ops/roi_align.py) run UNCHANGED on the sm_90a kernels.
 
 `mmcv/utils/ext_loader.py:12-16` only does `importlib.import_module('mmcv._ext')` and
 `assert hasattr(ext, fun)`.  The reference tree is read-only and mmcv is not pip
@@ -34,7 +34,7 @@ class _ExtModule(types.ModuleType):
 
 def make_module():
     m = _ExtModule('mmcv._ext')
-    m.__doc__ = 'gpt4roi_b200 drop-in for mmcv._ext (sm_100a RoIAlign)'
+    m.__doc__ = 'gpt4roi_b200 drop-in for mmcv._ext (sm_90a RoIAlign)'
     m.roi_align_forward = _ra.roi_align_forward
     m.roi_align_backward = _ra.roi_align_backward
     m.__gpt4roi_b200__ = True

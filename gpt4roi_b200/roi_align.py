@@ -1,7 +1,7 @@
 """Operator seam: `roi_align`, `RoIAlign`, `RoIAlignFunction` and the `mmcv._ext` entry points.
 
 Host-side mirror of the reference operator API (same names, argument meaning and error
-behaviour), backed by the sm_100a kernels behind the C ABI:
+behaviour), backed by the sm_90a kernels behind the C ABI:
 
     mmcv-1.4.7/mmcv/ops/roi_align.py:14-128   RoIAlignFunction (autograd)
     mmcv-1.4.7/mmcv/ops/roi_align.py:131      roi_align
@@ -138,7 +138,7 @@ class RoIAlign(nn.Module):
     """RoI align pooling layer -- same constructor and forward as mmcv.ops.RoIAlign
     (mmcv/ops/roi_align.py:134-224), including the deprecated `out_size` / `sample_num`
     keyword aliases (:171-177).  `use_torchvision=True` is refused: this module is the
-    sm_100a path and has no alternate back-end.
+    sm_90a path and has no alternate back-end.
     """
 
     def __init__(self, output_size=None, spatial_scale=1.0, sampling_ratio=0, pool_mode='avg',
@@ -153,7 +153,7 @@ class RoIAlign(nn.Module):
         if output_size is None:
             raise TypeError("missing required argument 'output_size'")
         if use_torchvision:
-            raise NotImplementedError('gpt4roi_b200.RoIAlign has a single (sm_100a) back-end')
+            raise NotImplementedError('gpt4roi_b200.RoIAlign has a single (sm_90a) back-end')
         self.output_size = _pair(output_size)
         self.spatial_scale = float(spatial_scale)
         self.sampling_ratio = int(sampling_ratio)

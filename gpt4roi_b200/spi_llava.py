@@ -1,4 +1,4 @@
-"""Model seam: drop-in mirrors of the reference's model classes, running on the sm_100a engine.
+"""Model seam: drop-in mirrors of the reference's model classes, running on the sm_90a engine.
 
 Same class names, constructor arguments, forward keyword arguments, attributes and -- above all --
 parameter names/shapes as the reference, so its checkpoints load unchanged and its train / serve
@@ -128,7 +128,7 @@ class MLVLFuseModule(nn.Module):
         activated NCHW maps.  Inference only; gradients flow through MLVLROIQueryModule.forward."""
         from . import kernels
         if self.num_levels != 4 or self.num_fuse != 5 or self.embed_dims != 1024:
-            raise NotImplementedError('the sm_100a SPI kernels are built for the GPT4RoI configuration (4 levels, 5 rounds, 1024 ch)')
+            raise NotImplementedError('the sm_90a SPI kernels are built for the GPT4RoI configuration (4 levels, 5 rounds, 1024 ch)')
         dev = inputs[0].device
         G = inputs[-1].shape[-1]
         eng = _spi_engine(self, 'mlvl_fuse.', {}, G, dev)
@@ -612,7 +612,7 @@ class SPILlavaMPTForCausalLM(LlamaForCausalLM, _EngineHost):
     @torch.no_grad()
     def generate(self, input_ids=None, images=None, bboxes=None, max_new_tokens=32, do_sample=False,
                  temperature=1.0, stopping_criteria=None, eos_token_id=None, use_hf_loop=False, **kwargs):
-        """Region-token prefill + KV-cache decode on the sm_100a engine.  Accepts the arguments the demo
+        """Region-token prefill + KV-cache decode on the sm_90a engine.  Accepts the arguments the demo
         passes (gpt4roi/app.py:293-300); boxes may be given here or bound the way app.py does
         (`self.forward = partial(self.forward, bboxes=...)`, :286-291).  Returns ids [B, L+new] like HF.
         use_hf_loop=True runs transformers' own GenerationMixin.generate over this model's forward /

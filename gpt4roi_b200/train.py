@@ -3,7 +3,7 @@
 The reference's stage-2 step (gpt4roi/train/train.py:698-712: HF Trainer over SPILlavaMPTForCausalLM under
 bf16 autocast, DDP gradient all-reduce, AdamW with the parameter groups of llava_trainer.py:59-144) spends
 6.48 B of its 7.04 B trainable parameters in the 32 LLaMA decoder layers.  This module is that part, built on
-the sm_100a kernels only:
+the sm_90a kernels only:
 
     inputs_embeds (from the region-token prefill front end: engine.PrefillEngine splice)
       -> 32 x [RMSNorm -> fused QKV GEMM + RoPE -> causal attention (saves LSE) -> o_proj + residual
@@ -160,7 +160,7 @@ def layer_numel(cfg):
 
 
 class LlamaTrainStack:
-    """LLaMA decoder stack with explicit forward / backward / AdamW on the sm_100a kernels.
+    """LLaMA decoder stack with explicit forward / backward / AdamW on the sm_90a kernels.
 
     Storage: per decoder layer ONE flat bf16 weight buffer (the four matrices are views of it) and, where this object
     owns the optimizer, flat fp32 master / moment buffers -- the whole vector, or this rank's 1/world slice of it
@@ -777,7 +777,7 @@ class SpiTrain:
     """Forward (with saved activations) and complete backward of the SPI module -- MLVLROIQueryModule
     (gpt4roi/models/layers.py:198-236): pyramid upsampling, MLVLFuseModule (4 input 1x1 convs + 5 shared
     ConvModule(3x3, GN(64), ReLU) rounds with the channel shuffle between levels), MlvlRoIExtractor (4 RoIAligns,
-    4 pconvs, flatten_linear, box position MLP, updims) -- on the sm_100a kernels, no autograd.
+    4 pconvs, flatten_linear, box position MLP, updims) -- on the sm_90a kernels, no autograd.
     Inputs: the CLIP hidden states (frozen tower) and the boxes; output: one region token per box.
     `backward(d_region)` returns gradients under the reference's parameter names and layouts (fp32 or bf16)."""
 
@@ -912,7 +912,7 @@ class Stage2Trainer:
     """One optimisation step of GPT4RoI training (scripts train_stage{1,2}.sh -> gpt4roi/train/train.py:698-712 ->
     HF Trainer.training_step): forward, backward, DDP gradient all-reduce, global grad-norm clip
     (max_grad_norm 1.0, the HF default the scripts do not override), warm-up + cosine learning rate
-    (train_stage2.sh:47-53) and torch.optim.AdamW semantics -- all on the sm_100a kernels; no autograd.
+    (train_stage2.sh:47-53) and torch.optim.AdamW semantics -- all on the sm_90a kernels; no autograd.
     Stage 2 trains every parameter except the frozen CLIP tower (embed_tokens, mm_projector, the SPI module, the
     32 LLaMA layers, final norm, lm_head); `trainable` selects the reference's other sets
     (ONLY_SPI / PROJ, `trainable_from_env`).  Loss: llava/model/llava.py:238-249.
@@ -962,8 +962,7 @@ class Stage2Trainer:
         # SMs kept free of the persistent GEMM kernels while a gradient collective runs beside the backward
         # (lib.set_sm_reserve); pair it with NCCL_MAX_CTAS=<same> set before the process group is created
         import os
-        # measured on 2 x B200 (profiles/r2_ddp_sm_reserve_sweep_2gpu.jsonl): reserving SMs does not shorten the step
-        # (260.3 ms with 0, 268 with 8, 263 with 16), so the default is 0
+        # the default is 0: whether reserving SMs shortens the step depends on the interconnect; measure before setting it
         self.sm_reserve = int(os.environ.get('G4R_DDP_SM_RESERVE', '0')) if sm_reserve is None else int(sm_reserve)
         fcfg = copy.copy(cfg)
         fcfg.n_layers = 0                                   # the front-end engine holds no decoder layers

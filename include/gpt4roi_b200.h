@@ -1,5 +1,5 @@
 /*
- * gpt4roi_b200.h -- C ABI of libgpt4roi_b200.so (sm_100a).
+ * gpt4roi_b200.h -- C ABI of libgpt4roi_b200.so (sm_90a).
  *
  * Drop-in boundary for the GPT4RoI region-token forward path.  Every entry
  * point takes raw DEVICE pointers, plain sizes and a cudaStream_t (as void*),
@@ -8,7 +8,7 @@
  * synchronises the stream unless stated.  No torch types cross this boundary.
  *
  * Each declaration cites the reference interface it replaces; paths are
- * relative to /root/reference.
+ * relative to the reference checkout (jshilong/GPT4RoI).
  */
 #ifndef GPT4ROI_B200_H_
 #define GPT4ROI_B200_H_
@@ -39,8 +39,8 @@ enum {
 const char* g4r_last_error(void);
 /* Library/ABI version (major*1000+minor) and the SM arch it was built for. */
 int g4r_version(void);
-int g4r_built_arch(void); /* 100 for sm_100a */
-/* Keep n_sms SMs free of the persistent (one CTA per SM) tcgen05 GEMM kernels -- room for the CTAs of a collective
+int g4r_built_arch(void); /* 90 for sm_90a */
+/* Keep n_sms SMs free of the persistent (one CTA per SM) wgmma GEMM kernels -- room for the CTAs of a collective
  * that runs beside the backward (the DDP gradient all-reduce of gpt4roi/train/train.py:698-712).  Returns the
  * previous reserve.  Process-wide; 0 (default) = the GEMMs use every SM. */
 int g4r_set_sm_reserve(int n_sms);
@@ -169,12 +169,12 @@ int g4r_splice_region_tokens(const int64_t* input_ids, const void* embed_table,
                              int64_t im_end_token, int64_t bbox_token,
                              void* stream);
 
-/* ---- dense contractions on tcgen05 tensor cores ---------------------------- */
+/* ---- dense contractions on the wgmma tensor cores -------------------------- */
 enum { G4R_ACT_NONE = 0, G4R_ACT_RELU = 1, G4R_ACT_QUICK_GELU = 2, G4R_ACT_SWIGLU = 3 };
 
 /*
  * D[M,N] = epilogue(A[M,K] . B[N,K]^T): bf16 operands (both K-major, i.e. B is an
- * nn.Linear weight [out,in]), fp32 accumulation in TMEM, TMA-fed, persistent.
+ * nn.Linear weight [out,in]), fp32 accumulation in registers, TMA-fed, persistent.
  * Replaces the cuBLAS calls behind torch.nn.Linear at
  *   gpt4roi/models/layers.py:260-270,326-329  (pos_embedd, flatten_linear, updims)
  *   llava/model/llava.py:52,76 / gpt4roi/models/spi_llava.py:89-97 (mm_projector)
@@ -287,8 +287,8 @@ int g4r_attention_bf16(const void* q, const void* k, const void* v, void* out,
                        void* stream);
 
 /*
- * Same contract on the tcgen05 tensor cores (TMA-fed, S and O accumulators in TMEM, V consumed as an
- * MN-major operand); requires the packed layout bs == L*ld.  csrc/attention_tcgen05.cu.
+ * Same contract on the wgmma tensor cores (TMA-fed, S and O accumulators in registers, V consumed as an
+ * MN-major operand); requires the packed layout bs == L*ld.  csrc/attention_wgmma.cu.
  */
 int g4r_attention_tc_bf16(const void* q, const void* k, const void* v, void* out,
                           long long ld, long long bs, long long ldo, long long bso,
@@ -385,7 +385,7 @@ int g4r_swiglu_bwd_bf16(const void* gu, long long ldg, const void* df, long long
 int g4r_attention_fwd_lse_bf16(const void* q, const void* k, const void* v, void* out, long long ld,
                                long long bs, long long ldo, long long bso, int B, int H, int L,
                                int head_dim, int causal, float scale, float* lse, void* stream);
-/* Same contract on the tcgen05 / TMEM attention kernel (q, k, v must be one packed [B*L, width] buffer, bs == L*ld):
+/* Same contract on the wgmma attention kernel (q, k, v must be one packed [B*L, width] buffer, bs == L*ld):
  * the training forward's default since round 2. */
 int g4r_attention_tc_lse_bf16(const void* q, const void* k, const void* v, void* out, long long ld, long long bs,
                               long long ldo, long long bso, int B, int H, int L, int head_dim, int causal, float scale,
@@ -499,8 +499,8 @@ int g4r_grad_clip_coef(const float* slabs, long long n_slabs, float pre_scale, f
  * Every entry point below has the signature, argument meaning and error behaviour of its `_bf16` namesake above,
  * with "bf16" read as "fp16" for every 16-bit tensor (activations, weights, norm / bias vectors, RoPE tables, KV
  * cache); fp32 arguments (statistics, scale / shift, split-K slabs, fp32 residual streams) are unchanged, and the
- * arithmetic is the same (fp32 accumulation, the same rounding points, tcgen05 kind::f16 with the F16 operand
- * format).  Built from the same sources with -DG4R_ACT_HALF (gpt4roi_b200/csrc/act_type.cuh).  RoIAlign and the
+ * arithmetic is the same (fp32 accumulation, the same rounding points, wgmma with .f16 instead of .bf16
+ * operands).  Built from the same sources with -DG4R_ACT_HALF (gpt4roi_b200/csrc/act_type.cuh).  RoIAlign and the
  * splice take a dtype argument / are 2-byte copies and need no twin; the training step is bf16 only
  * (train_stage*.sh --bf16 True). */
 int g4r_gemm_f16(const void* A, long long lda, const void* B, long long ldb,

@@ -6,7 +6,7 @@
  * cpu_baseline leg as the parity checker.  Nothing under gpt4roi_b200/ may
  * import, link or call it.
  *
- * Reference followed (paths relative to /root/reference/mmcv-1.4.7/mmcv/ops/csrc):
+ * Reference followed (paths relative to mmcv-1.4.7/mmcv/ops/csrc of the reference checkout):
  *   pytorch/cpu/roi_align.cpp:23-108    pre_calc_for_bilinear_interpolate
  *   pytorch/cpu/roi_align.cpp:110-214   ROIAlignForward<T>
  *   pytorch/cpu/roi_align.cpp:216-262   bilinear_interpolate_gradient
@@ -25,7 +25,7 @@
  * Differences from the reference that are deliberate:
  *   - layout/stride generalisation: the sample table is computed once per RoI
  *     exactly like PreCalc, but the input may be NCHW (reference layout) or
- *     NHWC (the layout the B200 kernels also accept) -- the VALUES are the same.
+ *     NHWC (the layout the GPU kernels also accept) -- the VALUES are the same.
  *   - the "aligned && negative RoI size" AT_ASSERTM (cpu/roi_align.cpp:137-139)
  *     is reported as return code 2 instead of throwing.
  */

@@ -1,7 +1,7 @@
 """Generate the committed golden fixtures under tests/golden/ FROM THE REFERENCE ITSELF.
 
-Run in the build container (needs /root/reference; the GPU box never runs this):
-    python tests/golden/make_golden.py
+Needs a checkout of the reference (jshilong/GPT4RoI) named by $GPT4ROI_REFERENCE; no GPU:
+    GPT4ROI_REFERENCE=<checkout> python tests/golden/make_golden.py [--model | --train | --input | --live | --wrapper]
 
 Fixtures:
   mmcv_roi_align_kat.json   the reference's own known-answer vectors, read from
@@ -9,8 +9,13 @@ Fixtures:
                             (3 cases: input, rois -> forward output and input-gradient;
                             pool 2x2, scale 1.0, sampling 2, avg, aligned)
   roi_align_ref_cases.npz   seeded random + adversarial cases run through the reference's
-                            CPU kernel compiled unmodified (oracle/_ref, see oracle/build_ref.py):
-                            forward (avg/max, argmax) and backward, fp32, NCHW.
+  roi_align_ref_cases_grad.npz  CPU kernel compiled unmodified (oracle/_ref, see oracle/build_ref.py):
+                            forward (avg/max, argmax) and backward, fp32, NCHW; inputs are replayed
+                            from the seed (tests/helpers.py:load_ref_cases).
+  roi_align_live_ref.npz    (--live) the same kernel on the seeded inputs of
+                            tests/test_oracle_cpu.py::test_oracle_matches_live_reference_build.
+  mmcv_wrapper_calls.json   (--wrapper) the symbols the reference's unmodified mmcv.ops asks of mmcv._ext
+                            and the calls its RoIAlign wrapper makes, recorded over the gpt4roi_b200 drop-in.
 """
 import importlib.util
 import json
@@ -25,7 +30,7 @@ ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, ROOT)
 from oracle import build_ref  # noqa: E402
 
-REF = os.environ.get('GPT4ROI_REFERENCE', '/root/reference')
+REF = os.environ.get('GPT4ROI_REFERENCE', '')
 
 
 def kat():
@@ -120,8 +125,13 @@ def ref_cases():
                          pool_mode='max' if pm == 0 else 'avg', aligned=aligned,
                          spatial_scale=scale, K=K))
     out['meta'] = np.frombuffer(json.dumps(meta).encode(), dtype=np.uint8)
+    # inputs and output gradients are replayed from the seed by tests/helpers.py:load_ref_cases; the two largest
+    # input gradients go to a second file so that each stays below 1 MB
+    out = {k: v for k, v in out.items() if not k.endswith(('.input', '.grad_output'))}
+    big = ('l0_224.grad_input', 'l1_224.grad_input')
+    np.savez_compressed(os.path.join(HERE, 'roi_align_ref_cases_grad.npz'), **{k: out.pop(k) for k in big})
     np.savez_compressed(os.path.join(HERE, 'roi_align_ref_cases.npz'), **out)
-    print('wrote roi_align_ref_cases.npz (%d cases)' % len(meta))
+    print('wrote roi_align_ref_cases*.npz (%d cases)' % len(meta))
 
 
 if __name__ == '__main__' and len(sys.argv) == 1:
@@ -251,8 +261,10 @@ def full_model_golden():
     L = ids.shape[1]
     probe = torch.unique(torch.cat([torch.arange(0, L, L // 12), torch.tensor([1, 2, cfg.num_patches + 2, L - 1]),
                                     torch.where(ids[0] == cfg.bbox_token)[0]]))
+    # a fixed sample of 4096 vocabulary columns keeps the file below 1 MB; argmax covers the whole vocabulary
+    vocab = np.sort(np.random.default_rng(0).choice(logits.shape[-1], 4096, replace=False))
     np.savez_compressed(os.path.join(HERE, 'full_model_ref_224.npz'),
-                        probe=probe.numpy(), logits=logits[:, probe].numpy(),
+                        probe=probe.numpy(), vocab=vocab, logits=logits[:, probe][:, :, vocab].numpy(),
                         argmax=logits.argmax(-1).numpy(), lmean=np.array([float(logits.double().mean()), float(logits.double().std())]),
                         ids_checksum=np.array([int(ids.sum())]),
                         w_checksum=np.array([float(sd['lm_head.weight'].double().sum())]))
@@ -266,7 +278,7 @@ if __name__ == '__main__' and '--model' in sys.argv:
 # ---------------------------------------------------------------------------------------
 # Training-step golden: the reference's OWN forward WITH labels + loss.backward() (the body of the HF Trainer step,
 # gpt4roi/train/train.py:698-712) on the same unmodified modules as the full-model golden, fp32 on CPU, CLIP tower
-# frozen as in stage 2.  Weights are rounded to bf16-representable values so that the sm_100a trainer starts from
+# frozen as in stage 2.  Weights are rounded to bf16-representable values so that the sm_90a trainer starts from
 # identical parameters.  Stored: the loss and the gradients of a probe set of parameters (small tensors in full,
 # the first rows of the large ones).  Pins gpt4roi_b200.train.Stage2Trainer to the reference's autograd.
 # ---------------------------------------------------------------------------------------
@@ -429,3 +441,93 @@ def input_pipeline_golden():
 
 if __name__ == '__main__' and '--input' in sys.argv:
     input_pipeline_golden()
+
+
+# ---------------------------------------------------------------------------------------------
+# --live: the reference CPU kernel's answers for the seeded inputs of
+# tests/test_oracle_cpu.py::test_oracle_matches_live_reference_build -> roi_align_live_ref.npz
+# ---------------------------------------------------------------------------------------------
+LIVE_CASES = [(48, 14, 2, 'avg', 7.0), (24, 7, 0, 'avg', 14.0), (16, 3, 2, 'max', 14.0)]
+
+
+def live_ref_golden():
+    from tests.helpers import make_rois
+    ext = build_ref.load()
+    assert ext is not None, 'reference tree not available'
+    rng = np.random.default_rng(7)
+    store = {}
+    for i, (H, PH, sr, mode, stride) in enumerate(LIVE_CASES):
+        x = rng.standard_normal((2, 5, H, H)).astype(np.float32)
+        rois = make_rois(rng, 2, 6, H * stride, adversarial=True)
+        scale = float(np.float32(1 / stride))
+        xt, rt = torch.from_numpy(x), torch.from_numpy(rois)
+        pm = 0 if mode == 'max' else 1
+        o = xt.new_zeros(rois.shape[0], 5, PH, PH)
+        ay = xt.new_zeros(o.shape) if pm == 0 else xt.new_zeros(0)
+        ax = xt.new_zeros(o.shape) if pm == 0 else xt.new_zeros(0)
+        ext.roi_align_forward(xt, rt, o, ay, ax, aligned_height=PH, aligned_width=PH,
+                              spatial_scale=scale, sampling_ratio=sr, pool_mode=pm, aligned=True)
+        store['%d.output' % i] = o.numpy()
+        if pm == 0:
+            store['%d.argmax_y' % i], store['%d.argmax_x' % i] = ay.numpy(), ax.numpy()
+    np.savez_compressed(os.path.join(HERE, 'roi_align_live_ref.npz'), **store)
+    print('wrote roi_align_live_ref.npz (%d cases)' % len(LIVE_CASES))
+
+
+if __name__ == '__main__' and '--live' in sys.argv:
+    live_ref_golden()
+
+
+# ---------------------------------------------------------------------------------------------
+# --wrapper: what the reference's UNMODIFIED mmcv.ops asks of `mmcv._ext` while importing, and the exact calls its
+# RoIAlign wrapper (mmcv-1.4.7/mmcv/ops/roi_align.py) makes, recorded over the gpt4roi_b200 drop-in on CPU tensors
+# -> mmcv_wrapper_calls.json (replayed by tests/test_abi_cpu.py without the reference tree)
+# ---------------------------------------------------------------------------------------------
+def _describe(v):
+    if isinstance(v, torch.Tensor):
+        return dict(tensor=list(v.shape), dtype=str(v.dtype).replace('torch.', ''))
+    return dict(value=v)
+
+
+def wrapper_golden():
+    import types
+    sys.path.insert(0, HERE)
+    import ref_shims
+    ref_shims.install(use_b200=True)
+    ours = sys.modules['mmcv._ext']
+    asked, calls = [], []
+
+    class Recorder(types.ModuleType):
+        def __getattr__(self, name):
+            if name.startswith('__'):
+                raise AttributeError(name)
+            if name not in asked:
+                asked.append(name)
+            fn = getattr(ours, name)
+
+            def record(*args, **kwargs):
+                calls.append(dict(fn=name, args=[_describe(a) for a in args],
+                                  kwargs={k: _describe(v) for k, v in kwargs.items()}))
+                return fn(*args, **kwargs)
+            return record
+    sys.modules['mmcv._ext'] = Recorder('mmcv._ext')
+    import mmcv.ops  # noqa: F401  (every ext_loader.load_ext of mmcv/ops/__init__.py asserts hasattr)
+    R = sys.modules['mmcv.ops.roi_align']
+    assert os.path.realpath(R.__file__).startswith(os.path.realpath(REF) + os.sep), R.__file__
+    x, rois = torch.zeros(1, 4, 8, 8), torch.tensor([[0., 0., 0., 4., 4.]])
+    outcomes = []
+    for call in (lambda: R.RoIAlign((7, 7), 0.5, 2)(x, rois),
+                 lambda: R.roi_align(x, rois, (3, 5), 0.25, 0, 'max', False)):
+        try:
+            call()
+            outcomes.append('computed on the CPU')
+        except RuntimeError as e:
+            outcomes.append('RuntimeError: %s' % e)
+    store = dict(mmcv_version=sys.modules['mmcv'].__version__, asked=asked, calls=calls, outcomes=outcomes)
+    with open(os.path.join(HERE, 'mmcv_wrapper_calls.json'), 'w') as f:
+        json.dump(store, f, indent=1)
+    print('wrote mmcv_wrapper_calls.json (%d symbols, %d calls)' % (len(asked), len(calls)))
+
+
+if __name__ == '__main__' and '--wrapper' in sys.argv:
+    wrapper_golden()

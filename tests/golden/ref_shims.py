@@ -1,7 +1,7 @@
 """Import shims that let the reference's OWN python modules run unmodified in the build
 container (SURVEY.md Appendix A, variant 6b).  TEST INFRASTRUCTURE: used only by
-tests/golden/make_golden.py and the optional live-reference tests; never on the GPU box
-(/root/reference does not exist there).
+tests/golden/make_golden.py and the optional live-reference tests, where the reference
+tree is available ($GPT4ROI_REFERENCE).
 
   * leaf stubs for third-party packages that are not installed (addict, yapf, terminaltables,
     pycocotools, matplotlib) -- none of them is touched on the hot path;
@@ -16,7 +16,7 @@ import os
 import sys
 import types
 
-REF = os.environ.get('GPT4ROI_REFERENCE', '/root/reference')
+REF = os.environ.get('GPT4ROI_REFERENCE', '')
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 

@@ -13,9 +13,25 @@ def load_kat():
         return json.load(f)
 
 
+REF_CASES_SEED = 20260923
+
+
 def load_ref_cases():
-    z = np.load(os.path.join(GOLDEN, 'roi_align_ref_cases.npz'))
+    """The reference RoIAlign cases of make_golden.py: its outputs, argmaxes and input gradients are stored
+    (roi_align_ref_cases*.npz); the inputs and output gradients are replayed from the same seeded generator, in the
+    order make_golden.py drew them."""
+    z = {}
+    for fn in ('roi_align_ref_cases.npz', 'roi_align_ref_cases_grad.npz'):
+        with np.load(os.path.join(GOLDEN, fn)) as f:
+            z.update({k: f[k] for k in f.files})
     meta = json.loads(bytes(z['meta']).decode())
+    rng = np.random.default_rng(REF_CASES_SEED)
+    for m in meta:
+        n = m['name']
+        z[n + '.input'] = rng.standard_normal((m['N'], m['C'], m['H'], m['W'])).astype(np.float32)
+        rng.uniform(0, 1, (12, 2, 2))            # the 12 random boxes (stored in .rois)
+        rng.integers(0, m['N'], (m['K'], 1))     # their image indices (stored in .rois)
+        z[n + '.grad_output'] = rng.standard_normal((m['K'], m['C'], m['PH'], m['PW'])).astype(np.float32)
     return z, meta
 
 
@@ -61,7 +77,7 @@ def golden_stream_mismatch():
     import pytest
     import torch
     msg = ('seeded CPU RNG stream differs from the one the golden fixtures were generated with (torch %s); regenerate them '
-           'with tests/golden/make_golden.py where /root/reference exists' % torch.__version__)
+           'with tests/golden/make_golden.py where the reference tree is available' % torch.__version__)
     if os.environ.get('G4R_ALLOW_GOLDEN_SKIP') == '1':
         pytest.skip(msg)
     pytest.fail(msg)

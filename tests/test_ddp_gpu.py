@@ -2,7 +2,7 @@
 a DDP step on a batch split over two GPUs must equal the single-GPU step on the concatenated batch -- same loss,
 same (averaged) gradients, same clip norm, same weights after AdamW within bf16 tolerance.
 
-Needs >= 2 GPUs (skipped otherwise; run with `gpurun --gpus 2 -- python -m pytest tests/test_ddp_gpu.py -m gpu`).
+Needs >= 2 GPUs (skipped otherwise; run on a multi-GPU machine with `python -m pytest tests/test_ddp_gpu.py -m gpu`).
 The CPU/gloo counterpart of the reducer plumbing is tests/test_dist_cpu.py."""
 import os
 import tempfile

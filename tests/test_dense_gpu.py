@@ -1,4 +1,4 @@
-"""GPU numerics tests for the tcgen05 GEMM / implicit-GEMM conv (floating point: tolerance
+"""GPU numerics tests for the wgmma GEMM / implicit-GEMM conv (floating point: tolerance
 tests against a plain PyTorch fp32 reference of the same op on the same bf16 inputs)."""
 import pytest
 import torch
@@ -118,7 +118,7 @@ def test_skinny_gemm_plain_matches_fp32_and_tile_path(M, N, K):
     b = (torch.randn(N, K, device=DEV) * 0.5).bfloat16()
     got = dense.linear(a, b)
     _close(got, a.float() @ b.float().t())
-    # against the 128-row tcgen05 tile kernel on a padded copy (M=17 rows disables the skinny route)
+    # against the 128-row wgmma tile kernel on a padded copy (M=17 rows disables the skinny route)
     a17 = torch.cat([a, torch.zeros(17 - M, K, device=DEV, dtype=torch.bfloat16)])
     tile = dense.linear(a17, b)[:M]
     assert (got.float() - tile.float()).abs().max() <= 2e-2 * tile.float().abs().max()

@@ -1,4 +1,4 @@
-"""GPU end-to-end parity of the sm_100a engine against the oracle (oracle/model_oracle.py: the
+"""GPU end-to-end parity of the sm_90a engine against the oracle (oracle/model_oracle.py: the
 reference's composition over transformers' CLIP/LLaMA + the SPI torch restatement pinned to the
 reference by tests/golden/spi_module_ref.npz).
 
@@ -156,8 +156,8 @@ def test_engine_vs_reference_forward_golden_224():
     cfg, sd, vit_sd, ids, images, boxes, z = full_model_case()
     eng = PrefillEngine(cfg, sd, vit_sd, DEV)
     got = eng.forward(ids.to(DEV), images.to(DEV, torch.bfloat16), boxes).float().cpu()
-    probe = torch.from_numpy(z['probe'])
-    e = rel(got[:, probe], torch.from_numpy(z['logits']))
+    probe, vocab = torch.from_numpy(z['probe']), torch.from_numpy(z['vocab'])
+    e = rel(got[:, probe][:, :, vocab], torch.from_numpy(z['logits']))
     print('engine vs reference-forward golden (224): rel-L2 %.3e' % e)
     assert e < 2.5e-2
     assert (got.argmax(-1).numpy() == z['argmax']).mean() > 0.9

@@ -3,7 +3,7 @@ passes `images.half()` / `bboxes.half()` (gpt4roi/app.py:74-98,271,296).  Every 
 (`*_f16` entry points, csrc/act_type.cuh: same sources, fp16 storage and tensor-core operand format, fp32
 accumulation, the same rounding points).  Checked here through the C ABI:
 
-  * kernel level -- GEMM (+ epilogues), conv, norms, tcgen05 attention, the decode GEMM / attention -- against fp32
+  * kernel level -- GEMM (+ epilogues), conv, norms, wgmma attention, the decode GEMM / attention -- against fp32
     torch references on fp16-representable inputs; tolerances are the bf16 tests' divided by 4 (fp16 carries three more
     mantissa bits), stated inline;
   * engine level -- region-token prefill vs the fp32 oracle on fp16-representable weights: closer than the bf16 engine
@@ -32,7 +32,7 @@ def _close(got, want, rtol=4e-3, atol=4e-3):
 
 @pytest.mark.parametrize('M,N,K', [(128, 128, 64), (200, 384, 320), (706, 4096, 4096), (5648, 1024, 1024), (8, 4096, 4096)])
 def test_gemm_f16_plain_and_epilogues(M, N, K):
-    """D = act(A W^T + bias) + residual on the tcgen05 tile kernels (1-CTA / 2-CTA) and, for M <= 16, the skinny
+    """D = act(A W^T + bias) + residual on the wgmma tile kernel and, for M <= 16, the skinny
     kernel: fp16 operands, fp32 accumulate, one rounding to fp16."""
     torch.manual_seed(M + N + K)
     a = (torch.randn(M, K, device=DEV) * 0.5).to(H)

@@ -1,12 +1,14 @@
 """CPU tests: pin the oracle (oracle/roi_align_oracle.c) against the reference's own
 known-answer vectors, the committed golden fixtures (outputs of the reference kernel
 compiled from its sources) and -- when oracle/_ref is present -- the live reference."""
+import os
+
 import numpy as np
 import pytest
 
 from oracle import build_ref
 from oracle import roi_align_oracle as O
-from tests.helpers import load_kat, load_ref_cases, make_rois
+from tests.helpers import GOLDEN, load_kat, load_ref_cases, make_rois
 
 
 @pytest.mark.parametrize('dtype', [np.float32, np.float64])
@@ -71,17 +73,22 @@ def test_oracle_empty_rois():
 
 
 def test_oracle_matches_live_reference_build():
-    """oracle/_ref = the reference's cpu/roi_align.cpp compiled unmodified (when available)."""
-    ext = build_ref.load()
-    if ext is None:
-        pytest.skip('oracle/_ref not built and /root/reference absent')
+    """The reference's cpu/roi_align.cpp compiled unmodified: its stored answers for these seeded inputs
+    (tests/golden/roi_align_live_ref.npz, make_golden.py --live), and the live build too where oracle/_ref exists."""
     import torch
+    ext = build_ref.load()
+    z = np.load(os.path.join(GOLDEN, 'roi_align_live_ref.npz'))
     rng = np.random.default_rng(7)
-    for (H, PH, sr, mode, stride) in [(48, 14, 2, 'avg', 7.0), (24, 7, 0, 'avg', 14.0), (16, 3, 2, 'max', 14.0)]:
+    for i, (H, PH, sr, mode, stride) in enumerate([(48, 14, 2, 'avg', 7.0), (24, 7, 0, 'avg', 14.0), (16, 3, 2, 'max', 14.0)]):
         x = rng.standard_normal((2, 5, H, H)).astype(np.float32)
         rois = make_rois(rng, 2, 6, H * stride, adversarial=True)
         scale = float(np.float32(1 / stride))
         out, ay, ax = O.roi_align_forward(x, rois, PH, scale, sr, mode, True)
+        assert np.array_equal(out, z['%d.output' % i])
+        if mode == 'max':
+            assert np.array_equal(ay, z['%d.argmax_y' % i]) and np.array_equal(ax, z['%d.argmax_x' % i])
+        if ext is None:
+            continue
         xt, rt = torch.from_numpy(x), torch.from_numpy(rois)
         o = xt.new_zeros(out.shape)
         pm = 0 if mode == 'max' else 1

@@ -54,8 +54,8 @@ def test_mmcv_ext_module_as_the_reference_wrapper_calls_it():
     """The `mmcv._ext` drop-in module (gpt4roi_b200.mmcv_ext, what `install()` registers), called exactly the way the
     reference's own wrapper calls it -- mmcv-1.4.7/mmcv/ops/roi_align.py:83-96 (forward: `new_zeros` output / argmax
     buffers, five positional tensors, six keyword scalars) and :113-123 (backward) -- on the mmcv known-answer cases and on
-    a pyramid-sized fp32 case against the oracle (bit-exact forward).  tests/test_abi_cpu.py runs the reference's actual
-    wrapper over the same module in the build container (no reference tree on the GPU box)."""
+    a pyramid-sized fp32 case against the oracle (bit-exact forward).  tests/test_abi_cpu.py replays the calls recorded from
+    the reference's actual wrapper over the same module."""
     from gpt4roi_b200 import mmcv_ext
     ext = mmcv_ext.make_module()
     kat = load_kat()
@@ -195,7 +195,18 @@ def test_mlvl_backward_vs_oracle():
     for l, s in enumerate(shapes):
         want = O.roi_align_backward(go[l], rois, s, SCALES[l], 2, 'avg', True, in_layout=O.NHWC,
                                     out_layout=O.NHWC)
-        np.testing.assert_allclose(grads[l].cpu().numpy(), want, rtol=1e-4, atol=2e-5)
+        # The kernel scatters with fp32 atomics (as the reference kernel does), so each pixel's terms are summed in
+        # whatever order the hardware issues them.  Two fp32 summation orders can differ by up to a few units of
+        # 2^-24 * sum(|term|), where the result cancels.  Because the weights are >= 0, sum(|term|) is the oracle's
+        # backward of |grad_out|.  Needed on an H100: with the bound 2e-5 + 1e-4 * |want| alone, one run failed on 1 of
+        # 16384 elements (|err| 2.53e-5 at |want| ~ 0.049, i.e. 0.5 % over); sum(|term|) reaches ~340 on the pixels fed
+        # by the degenerate adversarial boxes, where one fp32 ulp is already 3e-5.
+        mag = O.roi_align_backward(np.abs(go[l]), rois, s, SCALES[l], 2, 'avg', True, in_layout=O.NHWC,
+                                   out_layout=O.NHWC)
+        got = grads[l].cpu().numpy()
+        err = np.abs(got - want)
+        bound = 2e-5 + 1e-4 * np.abs(want) + 16 * 2.0 ** -24 * mag
+        assert (err <= bound).all(), (l, float(err.max()), int((err > bound).sum()))
 
 
 def test_mlvl_fused_groupnorm_relu_taps():

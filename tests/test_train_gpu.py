@@ -331,7 +331,7 @@ def test_right_padded_batch_needs_no_mask_in_causal_training():
 def test_stage2_step_matches_reference_autograd_golden():
     """tests/golden/train_step_ref_224.npz = loss and probe gradients of the reference's OWN
     SPILlavaMPTForCausalLM.forward(labels=...) + loss.backward() (unmodified modules under tests/golden/ref_shims.py,
-    fp32, CPU, CLIP frozen; generated by `make_golden.py --train`).  The sm_100a trainer starts from the same
+    fp32, CPU, CLIP frozen; generated by `make_golden.py --train`).  The sm_90a trainer starts from the same
     bf16-representable weights.  Tolerances (rel-L2 vs the fp32 golden): loss 3e-3; LLaMA / lm_head / projector /
     SPI-head tensors 3e-2; pconvs 8e-2; fuse / input convs and their GroupNorms 1.5e-1 (x2.5 for the 2-channel row probes
     of conv weights) -- the depth-dependent bf16

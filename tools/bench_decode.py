@@ -8,7 +8,7 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-from bench import synthetic_inputs  # noqa: E402
+from bench import peaks, synthetic_inputs  # noqa: E402
 from gpt4roi_b200.engine import EngineConfig, GraphedDecode, KVCache, PrefillEngine, random_state_dicts  # noqa: E402
 
 
@@ -45,7 +45,7 @@ def main():
         dec = e[1].elapsed_time(e[2])
         print(json.dumps(dict(batch=B, prompt_len=L, new_tokens=n_new, prefill_ms=pre, decode_ms_per_token=dec / n_new,
                               decode_tokens_per_s=B * n_new / (dec / 1e3),
-                              weight_stream_floor_ms=13.5e9 / 6.579e12 * 1e3,
+                              weight_stream_floor_ms=13.5e9 / (peaks()[0]['hbm_gbs'] * 1e9) * 1e3,
                               mode='cuda_graph' if graphed else 'eager_launches')), flush=True)
 
 

@@ -1,6 +1,6 @@
 """RoIAlign microbench (BASELINE config 5): N_maps x 100 RoIs, 4 levels x 1024 ch.
 Prints one JSON object per variant; run on the GPU box:  python tools/bench_roialign.py [--maps 256]
-Compares the sm_100a kernels with the reference CUDA kernel compiled unmodified for sm_100a
+Compares the sm_90a kernels with the reference CUDA kernel compiled unmodified for sm_90a
 (oracle/_ref/_mmcv_ref_cuda_ext.so, 4 launches on NCHW fp32) and torchvision's CUDA roi_align."""
 import argparse
 import json
@@ -17,10 +17,9 @@ from tests.helpers import PYRAMID, SCALES, make_rois  # noqa: E402
 
 
 def peak_hbm():
-    try:
-        return json.load(open(os.path.join(ROOT, 'MEASURED_PEAKS.json')))['hbm_gbs'], 'measured'
-    except Exception:
-        return 6650.0, 'fallback'
+    from bench import peaks   # MEASURED_PEAKS.json when present, else the H100 SXM data sheet
+    p, how = peaks()
+    return p['hbm_gbs'], how
 
 
 def time_fn(fn, iters, flush=None):
@@ -87,7 +86,7 @@ def main():
 
     if a.variants in ('nhwc', 'headline'):
         return
-    # NCHW fp32 comparisons: drop-in kernel, reference CUDA kernel (sm_100a build), torchvision
+    # NCHW fp32 comparisons: drop-in kernel, reference CUDA kernel (sm_90a build), torchvision
     nm = min(a.maps, 64)  # NCHW copies; keep memory bounded
     sub = rois[rois[:, 0] < nm].contiguous()
     Ks = sub.shape[0]
@@ -136,8 +135,9 @@ def main():
         scale_report('torchvision_cuda_nchw_fp32_p7', time_fn(tv, a.iters, flush))
     except Exception as ex:
         print(json.dumps(dict(variant='torchvision', skipped=str(ex))))
-    os.makedirs(os.path.join(ROOT, 'gpurun_out'), exist_ok=True)
-    json.dump(results, open(os.path.join(ROOT, 'gpurun_out', 'roialign_microbench.json'), 'w'), indent=1)
+    out_dir = os.path.join(ROOT, 'bench_out')
+    os.makedirs(out_dir, exist_ok=True)
+    json.dump(results, open(os.path.join(out_dir, 'roialign_microbench.json'), 'w'), indent=1)
 
 
 if __name__ == '__main__':

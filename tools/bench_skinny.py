@@ -89,7 +89,6 @@ def main():
                2 * B * kv_len * H * D * 2)
         report('kv_append', timed_graph(lambda: [kernels.kv_append(qkv, k, v, B, 1, 700) for k, v in caches]), R, 2 * B * H * D * 2 * 2)
         del caches
-    os.makedirs(os.path.join(ROOT, 'gpurun_out'), exist_ok=True)
 
 
 if __name__ == '__main__':

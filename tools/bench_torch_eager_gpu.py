@@ -1,5 +1,5 @@
 """GPU comparison point (SURVEY.md 8(d) / BASELINE.md 3): the reference composition run with stock
-PyTorch + transformers kernels (cuBLAS / cuDNN / eager attention, bf16 autocast) on the SAME B200 and
+PyTorch + transformers kernels (cuBLAS / cuDNN / eager attention, bf16 autocast) on the SAME GPU and
 the SAME workload as bench.py (configs[1]: B=8, 336 px, 8 RoIs, L=706, 7B).  Test/measurement
 infrastructure only (uses oracle/model_oracle.py); prints one JSON line.
 """
@@ -36,7 +36,7 @@ def main():
     e1.record()
     torch.cuda.synchronize()
     ms = e0.elapsed_time(e1) / steps
-    print(json.dumps(dict(what='reference composition, PyTorch eager + transformers %s, bf16 autocast, same B200' %
+    print(json.dumps(dict(what='reference composition, PyTorch eager + transformers %s, bf16 autocast, same GPU' %
                           __import__('transformers').__version__, ms_per_step=ms,
                           samples_per_s=WORKLOAD['batch_per_gpu'] / (ms / 1e3), steps=steps,
                           workload='configs[1]: B=8, 336px, 8 RoIs, L=%d, 7B, full logits' % ids.shape[1])))

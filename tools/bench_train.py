@@ -1,6 +1,6 @@
 """Training step of the 7B LLaMA stack (SURVEY.md 8(a) row 14, first slice; BASELINE config 4 shape: 336 px
 prompt of 706 tokens, per-GPU batch 4 = global batch 32 on 8 GPUs): forward + backward + gradient all-reduce +
-AdamW on the sm_100a kernels, synthetic inputs_embeds/labels, random-init weights.
+AdamW on the sm_90a kernels, synthetic inputs_embeds/labels, random-init weights.
   python tools/bench_train.py [--batch 4] [--steps 5] [--warmup 2]
   python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P tools/bench_train.py
 Prints one JSON line (rank 0).  The SPI / projector / embedding backward is not part of this slice."""

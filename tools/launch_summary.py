@@ -1,5 +1,5 @@
 """Summarise an ncu launch-list CSV (--metrics gpu__time_duration.sum --csv) into a markdown table of kernel shares.
-usage: python tools/launch_summary.py launches.csv "title" > profiles/x.md"""
+usage: python tools/launch_summary.py launches.csv "title" > x.md"""
 import collections
 import csv
 import sys

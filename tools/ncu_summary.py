@@ -1,5 +1,5 @@
 """Summarise an .ncu-rep (read here, no GPU needed) into a small markdown table for profiles/.
-usage: python tools/ncu_summary.py gpurun_out/x.ncu-rep [kernel-regex] > profiles/x.md"""
+usage: python tools/ncu_summary.py x.ncu-rep [kernel-regex] > x.md"""
 import csv
 import io
 import re
