@@ -8,19 +8,25 @@
 //                          llava/model/llava.py:52 (mm_projector), :195 (lm_head), HF CLIP / LLaMA linears
 //   nn.Conv2d 1x1 / 3x3  : gpt4roi/models/layers.py:129-144 (input_conv, fuse_convs), :257-259 (pconvs)
 //
-// Structure (per CTA, 1 CTA / SM, persistent over 128 x 128 output tiles; 3 warpgroups):
+// Structure (per CTA, 1 CTA / SM, persistent over 128 x BN output tiles, BN = 128 or 256; 3 warpgroups):
 //   warpgroup 0, one thread : TMA producer -- cp.async.bulk.tensor loads of the A tile [128 x 64] and the
-//                B tile [128 x 64] (128-byte swizzle) into a kStages-deep smem ring, completion signalled
-//                on `full` mbarriers (expect_tx).  In conv mode the A tile is a 4-D box (64 ch, BW, BH, 1)
-//                of the NHWC map shifted by the filter tap; out-of-bounds coordinates are zero-filled by
-//                TMA = the padding.
-//   warpgroups 1, 2 : consumers -- each issues wgmma m64n128k16 for its 64 rows of the tile (fp32
+//                B tile [BN x 64] (128-byte swizzle) into a Stages-deep smem ring (4 stages at BN = 128,
+//                3 at 256), completion signalled on `full` mbarriers (expect_tx).  In conv mode the A tile
+//                is a 4-D box (64 ch, BW, BH, 1) of the NHWC map shifted by the filter tap; out-of-bounds
+//                coordinates are zero-filled by TMA = the padding.
+//   warpgroups 1, 2 : consumers -- each issues wgmma m64nBNk16 for its 64 rows of the tile (fp32
 //                accumulators in registers) and releases the smem slot (`empty`) once its MMAs have read it.
-//                After the last k-block both stage their accumulators in shared memory and run the
-//                epilogue: thread = (row, half of the columns), 32 columns at a time -- fused bias /
-//                activation / residual / SwiGLU / RoPE / GroupNorm statistics, bf16 or fp32 store.
-//                Meanwhile the producer is already loading the next tile's operands.
+//                After the last k-block both stage their accumulators in shared memory, 128 columns at a
+//                time, and run the epilogue on each 128-column half: thread = (row, half of the columns),
+//                32 columns at a time -- fused bias / activation / residual / SwiGLU / RoPE / GroupNorm
+//                statistics, bf16 or fp32 store.  Meanwhile the producer is already loading the next tile's
+//                operands.
+// The operand majorness (TA, TB) is a template parameter, so each mainloop is straight-line code: every
+// k-block's four MMAs and their commit_group sit in one basic block, and wait_group 1 keeps one k-block of
+// MMAs in flight.  At BN = 256 the 128 accumulators per consumer thread need setmaxnreg: the producer
+// warpgroup gives its registers up (40 per thread) and the consumers grow to 232 (128*40 + 256*232 <= 64 K).
 #include <stdlib.h>
+#include <string.h>
 
 #include "common.cuh"
 #include "ptx.cuh"
@@ -29,12 +35,14 @@
 namespace G4R_NS {
 
 constexpr int kBlockM = 128;
-constexpr int kBlockN = 128;
+constexpr int kEpiN = 128;   // columns staged and drained per epilogue pass (one 128-dim RoPE head)
 constexpr int kBlockK = 64;  // 64 bf16 = 128 B = one swizzle atom
 constexpr int kMmaK = 16;
 constexpr int kGemmThreads = 384;
 constexpr int kConsumerThreads = 256;
-constexpr int kStages = 4;
+constexpr int kProducerRegs = 40;    // setmaxnreg at BN = 256: producer warpgroup ...
+constexpr int kConsumerRegs = 232;   // ... and each consumer warpgroup
+static_assert(128 * kProducerRegs + kConsumerThreads * kConsumerRegs <= 64 * 1024, "register file");
 
 enum { ACT_NONE = 0, ACT_RELU = 1, ACT_QUICK_GELU = 2, ACT_SWIGLU = 3 };
 
@@ -76,16 +84,21 @@ struct GemmParams {
   int gn_groups;         // groups per image (64)
 };
 
+// Shared memory: BN = 128: 4 stages x 32 KB + 66 KB staging = 194 KB;
+//                BN = 256: 3 stages x 48 KB + 66 KB staging = 210 KB (a 4th stage does not fit beside the staging tile).
+template <int BN>
 struct GemmCfg {
+  static constexpr int kStages = BN == 256 ? 3 : 4;
   static constexpr int kABytes = kBlockM * kBlockK * 2;   // 16 KB
-  static constexpr int kBBytes = kBlockN * kBlockK * 2;   // 16 KB
+  static constexpr int kBBytes = BN * kBlockK * 2;        // 16 or 32 KB
   static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kAccLd = kBlockN + 4;              // fp32 staging row stride (conflict-free row reads)
+  static constexpr int kAccLd = kEpiN + 4;                // fp32 staging row stride (conflict-free row reads)
   static constexpr int kAccBytes = kBlockM * kAccLd * 4;  // 66 KB
   static constexpr int kBarBytes = 2 * kStages * 8;
   static constexpr int kSmemBytes = kStages * kStageBytes + kAccBytes + kBarBytes + 1024;  // +1024 alignment slack
 };
-static_assert(GemmCfg::kSmemBytes <= 227 * 1024, "GEMM shared memory exceeds the sm_90 per-block limit");
+static_assert(GemmCfg<128>::kSmemBytes <= 227 * 1024, "GEMM shared memory exceeds the sm_90 per-block limit");
+static_assert(GemmCfg<256>::kSmemBytes <= 227 * 1024, "GEMM shared memory exceeds the sm_90 per-block limit");
 
 __device__ __forceinline__ float act_apply(float x, int act) {
   if (act == ACT_RELU) return fmaxf(x, 0.f);
@@ -102,12 +115,13 @@ __device__ __forceinline__ void acc_ld32(const float* srow, int c0, float (&f)[3
   }
 }
 
-// Epilogue of one 128 x 128 accumulator tile staged in shared memory: thread (`row`, `half`) handles the
-// 32-column chunks half, half + 2 (RoPE: the head's dims [32*half, 32*half + 32) and their partners 64 apart).
+// Epilogue of one 128 x 128 accumulator block staged in shared memory, output columns [col_base, col_base + 128):
+// thread (`row`, `half`) handles the 32-column chunks half, half + 2 (RoPE: the head's dims [32*half, 32*half + 32)
+// and their partners 64 apart).
 template <bool CONV>
-__device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float* srow, int m_blk, int n_blk, int split,
-                                              int row, int half, int lane) {
-  constexpr int BLOCK_N = kBlockN;
+__device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float* srow, int m_blk, int col_base,
+                                              int split, int row, int half, int lane) {
+  constexpr int BLOCK_N = kEpiN;
   // row -> output row offset
   bool row_ok;
   long long out_row;
@@ -123,7 +137,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float* 
     out_row = (long long)m_blk * kBlockM + row;
     row_ok = m_blk < p.num_m_tiles && out_row < p.M;
   }
-  if (!CONV && p.rope_cos != nullptr && n_blk * BLOCK_N < p.rope_cols) {
+  if (!CONV && p.rope_cos != nullptr && col_base < p.rope_cols) {
     // ---- fused RoPE (transformers modeling_llama.py:138-168): the tile holds one whole head of 128 dims;
     // dims (d, d+64) of a head are 64 columns apart -> load both 32-column chunks, rotate, store.
     // Rounding as in the reference: q/k are bf16 GEMM outputs, each bf16 tensor op rounds:
@@ -170,7 +184,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float* 
           ob[h8 * 4 + j] = *reinterpret_cast<uint32_t*>(&h2);
         }
       }
-      __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(p.D) + out_row * p.ldd + n_blk * BLOCK_N;
+      __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(p.D) + out_row * p.ldd + col_base;
 #pragma unroll
       for (int h4 = 0; h4 < 4; h4++) {
         reinterpret_cast<uint4*>(o + cA)[h4] = make_uint4(oa[4 * h4], oa[4 * h4 + 1], oa[4 * h4 + 2], oa[4 * h4 + 3]);
@@ -181,7 +195,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float* 
   }
 #pragma unroll 1
   for (int c0 = half * 32; c0 < BLOCK_N; c0 += 64) {
-    const int col0 = n_blk * BLOCK_N + c0;
+    const int col0 = col_base + c0;
     if (col0 >= p.N) continue;  // (warp-uniform)
     float f[32];
     acc_ld32(srow, c0, f);
@@ -323,20 +337,38 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float* 
   }
 }
 
-// The four MMAs (k = 16 each) of one 64-deep k-block.  K-major operands advance 16 elements = 32 B inside the
-// 128 B swizzle atom (+2 in the >>4 start field); MN-major ones advance 16 k-rows of 128 B (+128).
-template <int TA, int TB>
-__device__ __forceinline__ void mma_kblock(float (&acc)[64], uint64_t da, uint64_t db, int kb) {
-#pragma unroll
-  for (int k = 0; k < kBlockK / kMmaK; k++)
-    ptx::wgmma_m64n128_ss<TA, TB>(acc, da + (TA ? 128 : 2) * k, db + (TB ? 128 : 2) * k, (kb | k) != 0);
+// One k = 16 MMA of the warpgroup's 64 x BN block; ZERO: the tile's first (scale-d = 0, write-only accumulators).
+template <int TA, int TB, int BN, bool ZERO>
+__device__ __forceinline__ void mma_k16(float (&acc)[BN / 2], uint64_t da, uint64_t db) {
+  if constexpr (BN == 256) {
+    if constexpr (ZERO) ptx::wgmma_m64n256_ss_zero<TA, TB>(acc, da, db);
+    else ptx::wgmma_m64n256_ss<TA, TB>(acc, da, db, 1);
+  } else {
+    if constexpr (ZERO) ptx::wgmma_m64n128_ss_zero<TA, TB>(acc, da, db);
+    else ptx::wgmma_m64n128_ss<TA, TB>(acc, da, db, 1);
+  }
 }
 
-template <bool CONV>
+// The four MMAs (k = 16 each) of one 64-deep k-block.  K-major operands advance 16 elements = 32 B inside the
+// 128 B swizzle atom (+2 in the >>4 start field); MN-major ones advance 16 k-rows of 128 B (+128).
+// FIRST: the tile's first k-block, whose first MMA overwrites the accumulators.
+template <int TA, int TB, int BN, bool FIRST>
+__device__ __forceinline__ void mma_kblock(float (&acc)[BN / 2], uint64_t da, uint64_t db) {
+  mma_k16<TA, TB, BN, FIRST>(acc, da, db);
+#pragma unroll
+  for (int k = 1; k < kBlockK / kMmaK; k++)
+    mma_k16<TA, TB, BN, false>(acc, da + (TA ? 128 : 2) * k, db + (TB ? 128 : 2) * k);
+}
+
+// CONV: implicit-GEMM conv (TA = TB = 0).  TA / TB = 1: MN-major A / B (TB also covers b_mn == 2).
+template <bool CONV, int TA, int TB, int BN>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                 const __grid_constant__ GemmParams p) {
-  using Cfg = GemmCfg;
+  static_assert(BN == 128 || BN == 256, "tile width");
+  static_assert(!CONV || (TA == 0 && TB == 0), "conv operands are K-major");
+  using Cfg = GemmCfg<BN>;
+  constexpr int kStages = Cfg::kStages;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smem_a = smem;
@@ -363,9 +395,10 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmap_a, const __grid_constan
   const int tiles_mn = p.num_m_tiles * p.num_n_tiles;
   const int total_tiles = tiles_mn * p.k_splits;
 
-  if (warp == 0) {
-    // ============================ TMA producer ============================
-    if (lane == 0) {
+  if (threadIdx.x < kGemmThreads - kConsumerThreads) {
+    // ============================ TMA producer (warpgroup 0) ============================
+    if constexpr (BN == 256) ptx::setmaxnreg_dec<kProducerRegs>();  // the whole warpgroup, before lanes 1-127 leave
+    if (warp == 0 && lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
       for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
@@ -393,7 +426,7 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmap_a, const __grid_constan
             const int lvl = tap_all / p.taps, tap = tap_all % p.taps;
             const int dy = p.taps == 9 ? tap / 3 - 1 : 0, dx = p.taps == 9 ? tap % 3 - 1 : 0;
             ptx::tma_load_4d(sa, &tmap_a, &full[stage], cc * kBlockK, x0 + dx, y0 + dy, img + lvl * p.lvl_img_stride);
-          } else if (p.a_mn) {
+          } else if (TA) {
             // MN-major A: two [64 k][64 m] boxes (one 128-byte swizzle atom of m each)
 #pragma unroll
             for (int a = 0; a < kBlockM / 64; a++)
@@ -401,18 +434,18 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmap_a, const __grid_constan
           } else {
             ptx::tma_load_2d(sa, &tmap_a, &full[stage], kg * kBlockK, m_blk * kBlockM);
           }
-          if (!CONV && p.b_mn == 2) {
-            const int n0 = n_blk * kBlockN, tap = n0 / p.dw_cin, c0 = n0 % p.dw_cin;
+          if (TB && p.b_mn == 2) {
+            const int n0 = n_blk * BN, tap = n0 / p.dw_cin, c0 = n0 % p.dw_cin;
 #pragma unroll
-            for (int a = 0; a < kBlockN / 64; a++)
+            for (int a = 0; a < BN / 64; a++)
               ptx::tma_load_4d(sb + a * (kBlockK * 128), &tmap_b, &full[stage], c0 + a * 64, tap % 3, kg * kBlockK,
                                tap / 3);
-          } else if (!CONV && p.b_mn) {
+          } else if (TB) {
 #pragma unroll
-            for (int a = 0; a < kBlockN / 64; a++)
-              ptx::tma_load_2d(sb + a * (kBlockK * 128), &tmap_b, &full[stage], n_blk * kBlockN + a * 64, kg * kBlockK);
+            for (int a = 0; a < BN / 64; a++)
+              ptx::tma_load_2d(sb + a * (kBlockK * 128), &tmap_b, &full[stage], n_blk * BN + a * 64, kg * kBlockK);
           } else {
-            ptx::tma_load_2d(sb, &tmap_b, &full[stage], kg * kBlockK, n_blk * kBlockN);
+            ptx::tma_load_2d(sb, &tmap_b, &full[stage], kg * kBlockK, n_blk * BN);
           }
           if (++stage == kStages) { stage = 0; phase ^= 1; }
         }
@@ -420,59 +453,63 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmap_a, const __grid_constan
     }
     return;
   }
-  if (threadIdx.x < kGemmThreads - kConsumerThreads) return;  // rest of the producer warpgroup
 
   // ============================ consumers: MMA + epilogue ============================
+  if constexpr (BN == 256) ptx::setmaxnreg_inc<kConsumerRegs>();
   const int ct = threadIdx.x - (kGemmThreads - kConsumerThreads);  // 0..255
   const int wg = ct >> 7;    // consumer warpgroup: accumulator rows [64 wg, 64 wg + 64)
   const int wt = ct & 127;   // thread in the warpgroup
-  const int a_mn = CONV ? 0 : p.a_mn, b_mn = CONV ? 0 : (p.b_mn ? 1 : 0);
-  // MN-major B: LBO = the 8 KB stride between its two 64-wide n atoms
-  const uint32_t lbo_b = b_mn ? kBlockK * 128 : 0;
+  // MN-major B: LBO = the 8 KB stride between its 64-wide n atoms
+  const uint32_t lbo_b = TB ? kBlockK * 128 : 0;
+  const int row = ct & 127, half = ct >> 7;
   int stage = 0;
   uint32_t phase = 0;
-  float acc[64];
-#pragma unroll
-  for (int i = 0; i < 64; i++) acc[i] = 0.f;
+  float acc[BN / 2];
   for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
     const int split = t / tiles_mn;
     const int mn = t % tiles_mn;
     const int n_blk = p.n_fast ? mn % p.num_n_tiles : mn / p.num_m_tiles;
     const int m_blk = p.n_fast ? mn / p.num_n_tiles : mn % p.num_m_tiles;
-    int prev = -1;
-    for (int kb = 0; kb < p.num_k_blocks; kb++) {
+    // this warpgroup's 64 rows of A start 8 KB into the stage in both layouts (64 rows x 128 B, or mn atom wg)
+    auto desc_a = [&](int s) { return ptx::gmma_desc_sw128(ptx::smem_u32(smem_a + s * Cfg::kABytes + wg * 8192), 0); };
+    auto desc_b = [&](int s) { return ptx::gmma_desc_sw128(ptx::smem_u32(smem_b + s * Cfg::kBBytes), lbo_b); };
+    // k-block 0: overwrites the accumulators
+    ptx::mbar_wait(&full[stage], phase);
+    ptx::wgmma_fence();
+    mma_kblock<TA, TB, BN, true>(acc, desc_a(stage), desc_b(stage));
+    ptx::wgmma_commit();
+    int prev = stage;
+    if (++stage == kStages) { stage = 0; phase ^= 1; }
+    for (int kb = 1; kb < p.num_k_blocks; kb++) {
       ptx::mbar_wait(&full[stage], phase);
-      // this warpgroup's 64 rows of A start 8 KB into the stage in both layouts (64 rows x 128 B, or mn atom wg)
-      const uint64_t da = ptx::gmma_desc_sw128(ptx::smem_u32(smem_a + stage * Cfg::kABytes + wg * 8192), 0);
-      const uint64_t db = ptx::gmma_desc_sw128(ptx::smem_u32(smem_b + stage * Cfg::kBBytes), lbo_b);
       ptx::wgmma_fence();
-      if (!a_mn && !b_mn) mma_kblock<0, 0>(acc, da, db, kb);
-      else if (!a_mn) mma_kblock<0, 1>(acc, da, db, kb);
-      else if (!b_mn) mma_kblock<1, 0>(acc, da, db, kb);
-      else mma_kblock<1, 1>(acc, da, db, kb);
+      mma_kblock<TA, TB, BN, false>(acc, desc_a(stage), desc_b(stage));
       ptx::wgmma_commit();
       ptx::wgmma_wait<1>();  // the MMAs of the previous k-block have completed: its slot can be refilled
-      if (prev >= 0 && wt == 0) ptx::mbar_arrive(&empty[prev]);
+      if (wt == 0) ptx::mbar_arrive(&empty[prev]);
       prev = stage;
       if (++stage == kStages) { stage = 0; phase ^= 1; }
     }
     ptx::wgmma_wait<0>();
     ptx::fence_regs(acc);
     if (wt == 0) ptx::mbar_arrive(&empty[prev]);
-    // ---- stage the accumulators (fragment layout -> row-major fp32) and run the epilogue
-    ptx::named_bar_sync(1, kConsumerThreads);  // the previous tile's epilogue is done reading the staging tile
-    {
-      const int r = wg * 64 + (wt >> 5) * 16 + ((wt & 31) >> 2);
-      float* s = acc_s + r * Cfg::kAccLd + 2 * (wt & 3);
+    // ---- stage the accumulators (fragment layout -> row-major fp32), 128 columns at a time, and run the epilogue
 #pragma unroll
-      for (int j = 0; j < kBlockN / 8; j++) {
-        *reinterpret_cast<float2*>(s + 8 * j) = make_float2(acc[4 * j], acc[4 * j + 1]);
-        *reinterpret_cast<float2*>(s + 8 * Cfg::kAccLd + 8 * j) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+    for (int h = 0; h < BN / kEpiN; h++) {
+      ptx::named_bar_sync(1, kConsumerThreads);  // the previous pass's epilogue is done reading the staging tile
+      {
+        const int r = wg * 64 + (wt >> 5) * 16 + ((wt & 31) >> 2);
+        float* s = acc_s + r * Cfg::kAccLd + 2 * (wt & 3);
+#pragma unroll
+        for (int j = 0; j < kEpiN / 8; j++) {
+          const int a = h * (kEpiN / 2) + 4 * j;
+          *reinterpret_cast<float2*>(s + 8 * j) = make_float2(acc[a], acc[a + 1]);
+          *reinterpret_cast<float2*>(s + 8 * Cfg::kAccLd + 8 * j) = make_float2(acc[a + 2], acc[a + 3]);
+        }
       }
+      ptx::named_bar_sync(1, kConsumerThreads);
+      epilogue_tile<CONV>(p, acc_s + row * Cfg::kAccLd, m_blk, n_blk * BN + h * kEpiN, split, row, half, lane);
     }
-    ptx::named_bar_sync(1, kConsumerThreads);
-    const int row = ct & 127, half = ct >> 7;
-    epilogue_tile<CONV>(p, acc_s + row * Cfg::kAccLd, m_blk, n_blk, split, row, half, lane);
   }
 }
 
@@ -516,19 +553,43 @@ static int make_tmap(CUtensorMap* m, const void* base, int rank, const cuuint64_
   return G4R_OK;
 }
 
-template <bool CONV>
+template <bool CONV, int TA, int TB, int BN>
 static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, cudaStream_t st) {
   static bool attr_set = false;
-  auto kern = gemm_bf16_wgmma<CONV>;
+  auto kern = gemm_bf16_wgmma<CONV, TA, TB, BN>;
   if (!attr_set) {
-    G4R_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, GemmCfg::kSmemBytes));
+    G4R_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, GemmCfg<BN>::kSmemBytes));
     attr_set = true;
   }
   const int total = p.num_m_tiles * p.num_n_tiles * p.k_splits;
   const int grid = total < sm_budget() ? total : sm_budget();
-  kern<<<grid, kGemmThreads, GemmCfg::kSmemBytes, st>>>(ta, tb, p);
+  kern<<<grid, kGemmThreads, GemmCfg<BN>::kSmemBytes, st>>>(ta, tb, p);
   G4R_LAUNCH_CHECK("gemm_bf16_wgmma");
   return G4R_OK;
+}
+
+// Tile width of a forward GEMM / conv launch with `m_tiles` row tiles, N output columns and k_splits.
+// G4R_GEMM_BN=128|256 forces a width (read at every launch, so one process can time both); auto / unset applies
+// the rule: the persistent grid runs ceil(tiles / grid) rounds, and a 128 x 256 tile costs kTileCost256 / 100 of a
+// 128 x 128 tile, so the width with the smaller rounds x cost wins (ties go to 128).
+// kTileCost256 from tools/bench_gemm.py (H100 80GB HBM3, 700 W limit, power-capped at 1425-1590 MHz on these
+// shapes), time per round at 256 over time per round at 128:
+//   LLaMA M = 5648: q|k|v+RoPE 62.8/39.7 us = 1.58 (17 vs 33 rounds), o_proj 60.3/35.7 = 1.69 (6 vs 11),
+//   gate/up 57.3/35.4 = 1.62 (30 vs 59), down 148/97 = 1.52 (6 vs 11), lm_head 57.9/37.4 = 1.55 (43 vs 86);
+//   3x3 fuse conv 192 px 124/75 = 1.65 (70 vs 140).
+// So 256 wins whenever it saves more than ~38 % of the rounds: every LLaMA GEMM (o_proj and down included,
+// 0.362 vs 0.393 ms and 0.887 vs 1.069 ms), the big convs and 1x1 convs, while 3 -> 2 round cases such as ViT
+// out_proj / fc2 (4616 x 1024: 0.057 vs 0.069 ms, 0.120 vs 0.130 ms) stay at 128.
+constexpr int kTileCost256 = 160;   // per cent of a 128 x 128 tile
+static int pick_block_n(int m_tiles, int N, int k_splits) {
+  const char* e = getenv("G4R_GEMM_BN");
+  if (e && !strcmp(e, "128")) return 128;
+  if (e && !strcmp(e, "256")) return 256;
+  const long long grid = sm_budget();
+  const long long t128 = (long long)m_tiles * ((N + 127) / 128) * k_splits;
+  const long long t256 = (long long)m_tiles * ((N + 255) / 256) * k_splits;
+  const long long r128 = (t128 + grid - 1) / grid, r256 = (t256 + grid - 1) / grid;
+  return r256 * kTileCost256 < r128 * 100 ? 256 : 128;
 }
 
 }  // namespace g4r
@@ -615,7 +676,7 @@ extern "C" int g4r_gemm_bf16_t(const void* A, long long lda, int a_mn, const voi
   p.D = D; p.ldd = ldd; p.out_f32 = out_f32;
   p.a_rows = kBlockM;
   p.a_mn = a_mn ? 1 : 0; p.b_mn = b_mn ? 1 : 0;
-  p.num_n_tiles = (N + kBlockN - 1) / kBlockN;
+  p.num_n_tiles = (N + 127) / 128;   // the training GEMMs run 128 x 128 tiles
   CUtensorMap ta, tb;
   {
     cuuint64_t dims[2] = {(cuuint64_t)(a_mn ? M : K), (cuuint64_t)(a_mn ? K : M)};
@@ -627,11 +688,15 @@ extern "C" int g4r_gemm_bf16_t(const void* A, long long lda, int a_mn, const voi
   {
     cuuint64_t dims[2] = {(cuuint64_t)(b_mn ? N : K), (cuuint64_t)(b_mn ? K : N)};
     cuuint64_t str[1] = {(cuuint64_t)ldb * 2};
-    cuuint32_t box[2] = {64, (cuuint32_t)(b_mn ? kBlockK : kBlockN)};
+    cuuint32_t box[2] = {64, (cuuint32_t)(b_mn ? kBlockK : 128)};
     int rc = make_tmap(&tb, B, 2, dims, str, box);
     if (rc) return rc;
   }
-  return launch_gemm<false>(ta, tb, p, (cudaStream_t)stream);
+  const cudaStream_t st = (cudaStream_t)stream;
+  if (!a_mn && !b_mn) return launch_gemm<false, 0, 0, 128>(ta, tb, p, st);
+  if (!a_mn) return launch_gemm<false, 0, 1, 128>(ta, tb, p, st);
+  if (!b_mn) return launch_gemm<false, 1, 0, 128>(ta, tb, p, st);
+  return launch_gemm<false, 1, 1, 128>(ta, tb, p, st);
 }
 #endif
 
@@ -658,7 +723,7 @@ extern "C" int g4r_conv3x3_dw_bf16(const void* dz_pad, const void* x_pad_origin,
   if (accumulate) { p.residual = reinterpret_cast<const __nv_bfloat16*>(dW); p.residual_f32 = 1; p.ldr = p.ldd; }
   p.a_rows = kBlockM;
   p.a_mn = 1; p.b_mn = 2; p.dw_cin = Cin;
-  p.num_n_tiles = p.N / kBlockN;
+  p.num_n_tiles = p.N / 128;
   CUtensorMap ta, tb;
   {
     cuuint64_t dims[2] = {(cuuint64_t)Cout, (cuuint64_t)rows};
@@ -675,7 +740,7 @@ extern "C" int g4r_conv3x3_dw_bf16(const void* dz_pad, const void* x_pad_origin,
     int rc = make_tmap(&tb, x_pad_origin, 4, dims, str, box);
     if (rc) return rc;
   }
-  return launch_gemm<false>(ta, tb, p, (cudaStream_t)stream);
+  return launch_gemm<false, 1, 1, 128>(ta, tb, p, (cudaStream_t)stream);
 }
 #endif
 
@@ -712,7 +777,8 @@ static int gemm_impl(const void* A, long long lda, const void* B, long long ldb,
   p.rope_cols = rope_cols; p.rope_L = rope_L; p.rope_pos0 = rope_pos0; p.rope_pos_dev = rope_pos_dev;
   p.act = act; p.out_f32 = out_f32;
   p.conv = 0; p.a_rows = kBlockM;
-  p.num_n_tiles = (N + kBlockN - 1) / kBlockN;
+  const int bn = pick_block_n(p.num_m_tiles, N, k_splits);
+  p.num_n_tiles = (N + bn - 1) / bn;
   CUtensorMap ta, tb;
   {
     cuuint64_t dims[2] = {(cuuint64_t)K, (cuuint64_t)M};
@@ -724,11 +790,12 @@ static int gemm_impl(const void* A, long long lda, const void* B, long long ldb,
   {
     cuuint64_t dims[2] = {(cuuint64_t)K, (cuuint64_t)N};
     cuuint64_t str[1] = {(cuuint64_t)ldb * 2};
-    cuuint32_t box[2] = {kBlockK, kBlockN};
+    cuuint32_t box[2] = {kBlockK, (cuuint32_t)bn};
     int rc = make_tmap(&tb, B, 2, dims, str, box);
     if (rc) return rc;
   }
-  return launch_gemm<false>(ta, tb, p, (cudaStream_t)stream);
+  return bn == 256 ? launch_gemm<false, 0, 0, 256>(ta, tb, p, (cudaStream_t)stream)
+                   : launch_gemm<false, 0, 0, 128>(ta, tb, p, (cudaStream_t)stream);
 }
 
 // spatial tiling used by the conv kernel for an H x W map (also tells callers how many GN partial slots exist)
@@ -783,7 +850,8 @@ extern "C" int g4r_conv_nhwc_bf16(const void* X, const void* Wt, void* Y, int n_
     p.n_fast = nf;
   }
   p.gn_stats = gn_stats; p.gn_groups = gn_groups; p.gn_group_ch = gn_groups ? Cout / gn_groups : 0;
-  p.num_n_tiles = (Cout + kBlockN - 1) / kBlockN;
+  const int bn = pick_block_n(p.num_m_tiles, Cout, 1);
+  p.num_n_tiles = (Cout + bn - 1) / bn;
   CUtensorMap ta, tb;
   {
     cuuint64_t dims[4] = {(cuuint64_t)Cin, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)n_img * levels};
@@ -795,9 +863,10 @@ extern "C" int g4r_conv_nhwc_bf16(const void* X, const void* Wt, void* Y, int n_
   {
     cuuint64_t dims[2] = {(cuuint64_t)p.K, (cuuint64_t)Cout};
     cuuint64_t str[1] = {(cuuint64_t)p.K * 2};
-    cuuint32_t box[2] = {kBlockK, kBlockN};
+    cuuint32_t box[2] = {kBlockK, (cuuint32_t)bn};
     int rc = make_tmap(&tb, Wt, 2, dims, str, box);
     if (rc) return rc;
   }
-  return launch_gemm<true>(ta, tb, p, (cudaStream_t)stream);
+  return bn == 256 ? launch_gemm<true, 0, 0, 256>(ta, tb, p, (cudaStream_t)stream)
+                   : launch_gemm<true, 0, 0, 128>(ta, tb, p, (cudaStream_t)stream);
 }
