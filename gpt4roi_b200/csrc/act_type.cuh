@@ -51,6 +51,10 @@
 #define g4r_decode_gemm_bf16 g4r_decode_gemm_f16
 #define g4r_kv_append_bf16 g4r_kv_append_f16
 #define g4r_decode_attention_bf16 g4r_decode_attention_f16
+#define g4r_gemm_qkv_rope_rows_bf16 g4r_gemm_qkv_rope_rows_f16
+#define g4r_decode_gemm_rows_bf16 g4r_decode_gemm_rows_f16
+#define g4r_kv_append_rows_bf16 g4r_kv_append_rows_f16
+#define g4r_decode_attention_rows_bf16 g4r_decode_attention_rows_f16
 
 #else
 #define G4R_NS g4r

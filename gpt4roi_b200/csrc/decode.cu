@@ -2,18 +2,21 @@
 // (SURVEY.md 8(f1)): after the region-token prefill, every further step is plain LLaMA with one new
 // token per sample (the vision/SPI branch is skipped, gpt4roi/models/spi_llava.py:47-48;
 // llava/model/llava.py:263-283 prepare_inputs_for_generation; gpt4roi/app.py:293-300).
-// Both kernels are HBM-bound: the step streams the whole KV cache of the batch once.
+// Both kernels are HBM-bound: the step streams the whole KV cache of the batch once.  Both take either one position
+// for the whole batch (launch argument or device scalar) or one per sample (pos_rows, device int32 [B]: a batch of
+// prompts of different lengths, right-padded, each continuing from its own length).
 #include "common.cuh"
 #include <cooperative_groups.h>
 #include "act_type.cuh"   // bf16 as written; fp16 twin with -DG4R_ACT_HALF
 
 namespace G4R_NS {
 
-// rows [B*Ln, 3*HD] packed (q|k|v) -> caches [B, Lmax, HD] at positions pos0 .. pos0+Ln-1
+// rows [B*Ln, 3*HD] packed (q|k|v) -> caches [B, Lmax, HD] at positions pos0 .. pos0+Ln-1, or with pos_rows (a batch
+// of prompts of different lengths) sample b's rows at pos_rows[b] .. pos_rows[b]+Ln-1
 __global__ void __launch_bounds__(256)
 kv_append_bf16(const __nv_bfloat16* __restrict__ qkv, long long ld, __nv_bfloat16* __restrict__ kc,
-               __nv_bfloat16* __restrict__ vc, int B, int Ln, int pos0, const int* __restrict__ pos_dev, int Lmax,
-               int HD) {
+               __nv_bfloat16* __restrict__ vc, int B, int Ln, int pos0, const int* __restrict__ pos_dev,
+               const int* __restrict__ pos_rows, int Lmax, int HD) {
   if (pos_dev) pos0 = *pos_dev;
   const int nvec = HD >> 3;
   const long long total = (long long)B * Ln * nvec * 2;
@@ -23,8 +26,9 @@ kv_append_bf16(const __nv_bfloat16* __restrict__ qkv, long long ld, __nv_bfloat1
     const int which = (int)((i / nvec) & 1);  // 0 = k, 1 = v
     const long long r = i / (2LL * nvec);     // row in [0, B*Ln)
     const int t = (int)(r % Ln), b = (int)(r / Ln);
+    const int p0 = pos_rows ? pos_rows[b] : pos0;
     const uint4 val = *reinterpret_cast<const uint4*>(qkv + r * ld + (long long)(1 + which) * HD + v * 8);
-    __nv_bfloat16* dst = (which ? vc : kc) + ((long long)b * Lmax + pos0 + t) * HD + v * 8;
+    __nv_bfloat16* dst = (which ? vc : kc) + ((long long)b * Lmax + p0 + t) * HD + v * 8;
     *reinterpret_cast<uint4*>(dst) = val;
   }
 }
@@ -36,11 +40,15 @@ kv_append_bf16(const __nv_bfloat16* __restrict__ qkv, long long ld, __nv_bfloat1
 // summation order (bitwise reproducible).  S is chosen so that even batch 1 (32 heads) fills the GPU.
 // 256 threads; a half-warp owns one key/value row (16 lanes x 16 bytes = the 256-byte row, coalesced).
 // Rounding as the reference's eager attention: fp32 softmax, probabilities cast to bf16 before P.V.
+// pos_rows (prompts of different lengths): sample b attends over its own pos_rows[b] + 1 keys.  S and the score buffer
+// still come from the host's bound kv_len (>= every row's length); each row slices its own keys into S parts, so a CTA
+// of a short row may own no key at all -- it still joins every cluster barrier and contributes -inf to the max and 0 to
+// the sum and to the output.  All rows equal: the slicing, and so the result, is the scalar kernel's.
 template <int D>
 __global__ void __launch_bounds__(256)
 decode_attention_bf16(const __nv_bfloat16* q, long long ldq, const __nv_bfloat16* kc, const __nv_bfloat16* vc,
-                      __nv_bfloat16* out, long long ldo, int H, int kv_len, const int* __restrict__ pos_dev, int Lmax,
-                      float scale, int per_max, int pdl) {
+                      __nv_bfloat16* out, long long ldo, int H, int kv_len, const int* __restrict__ pos_dev,
+                      const int* __restrict__ pos_rows, int Lmax, float scale, int per_max, int pdl) {
   // Programmatic dependent launch (common.cuh): q and the newest K/V row come from the q|k|v GEMM that precedes this
   // kernel in the decode step, so there is nothing to fetch ahead; the launch itself and the prologue overlap its tail.
   // q / kc / vc carry no __restrict__: their loads must stay on the coherent path.
@@ -52,7 +60,8 @@ decode_attention_bf16(const __nv_bfloat16* q, long long ldq, const __nv_bfloat16
   namespace cg = cooperative_groups;
   cg::cluster_group cluster = cg::this_cluster();
   const int S = (int)cluster.num_blocks(), rank = (int)cluster.block_rank();
-  if (pos_dev) kv_len = *pos_dev + 1;
+  if (pos_rows) kv_len = pos_rows[blockIdx.y] + 1;
+  else if (pos_dev) kv_len = *pos_dev + 1;
   extern __shared__ float sm[];
   float* sc = sm;                       // [per_max] scores / probabilities of this CTA's slice
   float* part = sm + per_max;           // [GROUPS][D] partial outputs, then [D] CTA total in part[0..D)
@@ -187,24 +196,36 @@ decode_attention_bf16(const __nv_bfloat16* q, long long ldq, const __nv_bfloat16
 
 using namespace G4R_NS;
 
-extern "C" int g4r_kv_append_bf16(const void* qkv, long long ld, void* kcache, void* vcache, int B, int Ln,
-                                  int pos0, const int* pos_dev, int Lmax, int HD, void* stream) {
-  G4R_REQUIRE(qkv && kcache && vcache && B > 0 && Ln > 0 && pos0 >= 0 && pos0 + Ln <= Lmax && HD % 8 == 0 && ld % 8 == 0,
-              "kv_append: bad arguments (pos0=%d Ln=%d Lmax=%d)", pos0, Ln, Lmax);
+static int launch_kv_append(const void* qkv, long long ld, void* kcache, void* vcache, int B, int Ln, int pos0,
+                            const int* pos_dev, const int* pos_rows, int Lmax, int HD, cudaStream_t st) {
   const long long total = (long long)B * Ln * (HD / 8) * 2;
   long long grid = (total + 255) / 256;
   const long long cap = (long long)num_sms() * 16;
   if (grid > cap) grid = cap;
-  kv_append_bf16<<<(unsigned)grid, 256, 0, (cudaStream_t)stream>>>((const __nv_bfloat16*)qkv, ld, (__nv_bfloat16*)kcache,
-                                                                  (__nv_bfloat16*)vcache, B, Ln, pos0, pos_dev, Lmax, HD);
+  kv_append_bf16<<<(unsigned)grid, 256, 0, st>>>((const __nv_bfloat16*)qkv, ld, (__nv_bfloat16*)kcache,
+                                                 (__nv_bfloat16*)vcache, B, Ln, pos0, pos_dev, pos_rows, Lmax, HD);
   G4R_LAUNCH_CHECK("kv_append");
   return G4R_OK;
 }
 
+extern "C" int g4r_kv_append_bf16(const void* qkv, long long ld, void* kcache, void* vcache, int B, int Ln,
+                                  int pos0, const int* pos_dev, int Lmax, int HD, void* stream) {
+  G4R_REQUIRE(qkv && kcache && vcache && B > 0 && Ln > 0 && pos0 >= 0 && pos0 + Ln <= Lmax && HD % 8 == 0 && ld % 8 == 0,
+              "kv_append: bad arguments (pos0=%d Ln=%d Lmax=%d)", pos0, Ln, Lmax);
+  return launch_kv_append(qkv, ld, kcache, vcache, B, Ln, pos0, pos_dev, nullptr, Lmax, HD, (cudaStream_t)stream);
+}
+
+extern "C" int g4r_kv_append_rows_bf16(const void* qkv, long long ld, void* kcache, void* vcache, int B, int Ln,
+                                       const int* pos_rows, int Lmax, int HD, void* stream) {
+  G4R_REQUIRE(qkv && kcache && vcache && pos_rows && B > 0 && Ln > 0 && Ln <= Lmax && HD % 8 == 0 && ld % 8 == 0,
+              "kv_append_rows: bad arguments (Ln=%d Lmax=%d)", Ln, Lmax);
+  return launch_kv_append(qkv, ld, kcache, vcache, B, Ln, 0, nullptr, pos_rows, Lmax, HD, (cudaStream_t)stream);
+}
+
 template <int D>
 static int launch_decode_attention(const void* q, long long ldq, const void* kcache, const void* vcache, void* out,
-                                   long long ldo, int B, int H, int kv_len, const int* pos_dev, int Lmax,
-                                   float scale, cudaStream_t st) {
+                                   long long ldo, int B, int H, int kv_len, const int* pos_dev, const int* pos_rows,
+                                   int Lmax, float scale, cudaStream_t st) {
   // split-KV factor: enough CTAs for >= 2 per SM, slices of >= 64 keys, cluster size <= 8 (portable)
   int S = 1;
   while (S < 8 && H * B * S < 2 * num_sms() && kv_len / (2 * S) >= 64) S *= 2;
@@ -219,18 +240,32 @@ static int launch_decode_attention(const void* q, long long ldq, const void* kca
   }
   G4R_CUDA(launch_pdl(decode_attention_bf16<D>, dim3(H, B, S), dim3(256), smem, st, dim3(1, 1, S),
                       (const __nv_bfloat16*)q, ldq, (const __nv_bfloat16*)kcache, (const __nv_bfloat16*)vcache,
-                      (__nv_bfloat16*)out, ldo, H, kv_len, pos_dev, Lmax, scale, per_max, pdl_mode()));
+                      (__nv_bfloat16*)out, ldo, H, kv_len, pos_dev, pos_rows, Lmax, scale, per_max, pdl_mode()));
   return G4R_OK;
 }
 
-extern "C" int g4r_decode_attention_bf16(const void* q, long long ldq, const void* kcache, const void* vcache,
-                                         void* out, long long ldo, int B, int H, int head_dim, int kv_len,
-                                         const int* pos_dev, int Lmax, float scale, void* stream) {
+static int decode_attention(const void* q, long long ldq, const void* kcache, const void* vcache, void* out,
+                            long long ldo, int B, int H, int head_dim, int kv_len, const int* pos_dev,
+                            const int* pos_rows, int Lmax, float scale, void* stream) {
   G4R_REQUIRE(q && kcache && vcache && out && B > 0 && H > 0 && kv_len > 0 && kv_len <= Lmax, "decode_attention: bad arguments");
   G4R_REQUIRE(head_dim == 64 || head_dim == 128, "decode_attention: head_dim %d", head_dim);
   G4R_REQUIRE(ldq % 8 == 0 && ((uintptr_t)q & 15) == 0, "decode_attention: q rows must be 16-byte aligned");
   cudaStream_t st = (cudaStream_t)stream;
   if (head_dim == 128)
-    return launch_decode_attention<128>(q, ldq, kcache, vcache, out, ldo, B, H, kv_len, pos_dev, Lmax, scale, st);
-  return launch_decode_attention<64>(q, ldq, kcache, vcache, out, ldo, B, H, kv_len, pos_dev, Lmax, scale, st);
+    return launch_decode_attention<128>(q, ldq, kcache, vcache, out, ldo, B, H, kv_len, pos_dev, pos_rows, Lmax, scale, st);
+  return launch_decode_attention<64>(q, ldq, kcache, vcache, out, ldo, B, H, kv_len, pos_dev, pos_rows, Lmax, scale, st);
+}
+
+extern "C" int g4r_decode_attention_bf16(const void* q, long long ldq, const void* kcache, const void* vcache,
+                                         void* out, long long ldo, int B, int H, int head_dim, int kv_len,
+                                         const int* pos_dev, int Lmax, float scale, void* stream) {
+  return decode_attention(q, ldq, kcache, vcache, out, ldo, B, H, head_dim, kv_len, pos_dev, nullptr, Lmax, scale, stream);
+}
+
+extern "C" int g4r_decode_attention_rows_bf16(const void* q, long long ldq, const void* kcache, const void* vcache,
+                                              void* out, long long ldo, int B, int H, int head_dim, int kv_bound,
+                                              const int* pos_rows, int Lmax, float scale, void* stream) {
+  G4R_REQUIRE(pos_rows != nullptr, "decode_attention_rows: pos_rows is NULL");
+  return decode_attention(q, ldq, kcache, vcache, out, ldo, B, H, head_dim, kv_bound, nullptr, pos_rows, Lmax, scale,
+                          stream);
 }

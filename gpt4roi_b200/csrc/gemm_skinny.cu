@@ -39,6 +39,7 @@ struct SkinnyParams {
   const __nv_bfloat16* rope_cos; const __nv_bfloat16* rope_sin;
   int rope_cols, rope_L, rope_pos0;
   const int* rope_pos_dev;
+  const int* rope_pos_rows;   // optional per-sample base [M / rope_L] (prompts of different lengths); wins over the two above
   // decode-step fusions (all optional):
   const __nv_bfloat16* norm_w; float norm_eps;   // RMSNorm of the activation rows before the product (K = hidden)
   __nv_bfloat16* kcache; __nv_bfloat16* vcache;  // [M, cache_lmax, cache_hd]: k / v columns are also written at `pos`
@@ -70,6 +71,12 @@ __device__ __forceinline__ void mma_16816(float (&c)[4], uint32_t a0, uint32_t a
 }
 
 __device__ __forceinline__ float bf16r(float x) { return __bfloat162float(__float2bfloat16_rn(x)); }
+
+// sequence position of activation row m: its sample's base (per-sample, device scalar or launch argument) + m % rope_L
+__device__ __forceinline__ int rope_row_pos(const SkinnyParams& p, int m) {
+  const int base = p.rope_pos_rows ? p.rope_pos_rows[m / p.rope_L] : (p.rope_pos_dev ? *p.rope_pos_dev : p.rope_pos0);
+  return base + m % p.rope_L;
+}
 
 // MT: 16-row weight tiles per CTA (1 or 2); MB: 8-row activation blocks (1: M<=8, 2: M<=16);
 // ROPE: the two tiles are 64 rows apart (dims d and d+64 of one 128-dim head) so the rotation has
@@ -265,7 +272,7 @@ gemm_skinny_bf16(const SkinnyParams p) {
       __nv_bfloat16* o = p.D + (long long)m * p.ldd;
       if (n1 < p.rope_cols) {
         // rounding points as in the wgmma GEMM epilogue / transformers modeling_llama.py:138-168
-        const int pos = (p.rope_pos_dev ? *p.rope_pos_dev : p.rope_pos0) + m % p.rope_L;
+        const int pos = rope_row_pos(p, m);
         const int d = n1 & 127;
         const __nv_bfloat16* ct = p.rope_cos + (long long)pos * 128;
         const __nv_bfloat16* st = p.rope_sin + (long long)pos * 128;
@@ -285,7 +292,7 @@ gemm_skinny_bf16(const SkinnyParams p) {
         o[n1] = r1;
         o[n2] = r2;
         if (p.vcache != nullptr && n1 >= 2 * p.cache_hd) {
-          const int pos = (p.rope_pos_dev ? *p.rope_pos_dev : p.rope_pos0) + m % p.rope_L;
+          const int pos = rope_row_pos(p, m);
           __nv_bfloat16* vc = p.vcache + ((long long)m * p.cache_lmax + pos) * p.cache_hd - 2 * p.cache_hd;
           vc[n1] = r1;
           vc[n2] = r2;
@@ -356,7 +363,7 @@ static bool wide_prefers_8_warps(int tiles) {
 int gemm_skinny_dispatch(const void* A, long long lda, const void* B, long long ldb, void* D, long long ldd, int M,
                          int N, int K, const void* bias, int bias_f32, const void* residual, long long ldr, int act,
                          const void* rope_cos, const void* rope_sin, int rope_cols, int rope_L, int rope_pos0,
-                         const int* rope_pos_dev, void* stream) {
+                         const int* rope_pos_dev, const int* rope_pos_rows, void* stream) {
   if (M > 16 || K % 32 != 0) return -1;
   if (act == SK_ACT_SWIGLU && (N % 2 != 0)) return -1;
   SkinnyParams p{};
@@ -365,6 +372,7 @@ int gemm_skinny_dispatch(const void* A, long long lda, const void* B, long long 
   p.bias = bias; p.bias_f32 = bias_f32; p.residual = (const __nv_bfloat16*)residual; p.ldr = ldr; p.act = act;
   p.rope_cos = (const __nv_bfloat16*)rope_cos; p.rope_sin = (const __nv_bfloat16*)rope_sin;
   p.rope_cols = rope_cols; p.rope_L = rope_L > 0 ? rope_L : 1; p.rope_pos0 = rope_pos0; p.rope_pos_dev = rope_pos_dev;
+  p.rope_pos_rows = rope_pos_rows;
   cudaStream_t st = (cudaStream_t)stream;
   if (rope_cos != nullptr) {
     if (N % 128 != 0) return -1;
@@ -415,11 +423,10 @@ int gemm_skinny_fused(const SkinnyParams& p0, cudaStream_t st) {
 
 using namespace G4R_NS;
 
-extern "C" int g4r_decode_gemm_bf16(const void* x, long long ldx, const void* W, long long ldw, void* out, long long ldo,
-                                    int M, int N, int K, const void* norm_w, float norm_eps, int act, const void* residual,
-                                    long long ldr, const void* rope_cos, const void* rope_sin, int rope_cols, int pos0,
-                                    const int* pos_dev, void* kcache, void* vcache, int cache_lmax, int cache_hd,
-                                    void* stream) {
+static int decode_gemm(const void* x, long long ldx, const void* W, long long ldw, void* out, long long ldo, int M, int N,
+                       int K, const void* norm_w, float norm_eps, int act, const void* residual, long long ldr,
+                       const void* rope_cos, const void* rope_sin, int rope_cols, int pos0, const int* pos_dev,
+                       const int* pos_rows, void* kcache, void* vcache, int cache_lmax, int cache_hd, void* stream) {
   G4R_REQUIRE(x && W && out && M > 0 && M <= 16 && N > 0 && K > 0, "decode_gemm: M must be 1..16 (got %d)", M);
   G4R_REQUIRE(ldx % 8 == 0 && ldw % 8 == 0 && K % 32 == 0, "decode_gemm: K %% 32 == 0 and 16-byte-aligned rows required");
   G4R_REQUIRE(act == SK_ACT_NONE || act == SK_ACT_SWIGLU, "decode_gemm: act must be none or swiglu");
@@ -431,10 +438,29 @@ extern "C" int g4r_decode_gemm_bf16(const void* x, long long ldx, const void* W,
   p.D = (__nv_bfloat16*)out; p.ldd = ldo; p.M = M; p.N = N; p.K = K;
   p.residual = (const __nv_bfloat16*)residual; p.ldr = ldr; p.act = act;
   p.rope_cos = (const __nv_bfloat16*)rope_cos; p.rope_sin = (const __nv_bfloat16*)rope_sin;
-  p.rope_cols = rope_cols; p.rope_L = 1; p.rope_pos0 = pos0; p.rope_pos_dev = pos_dev;
+  p.rope_cols = rope_cols; p.rope_L = 1; p.rope_pos0 = pos0; p.rope_pos_dev = pos_dev; p.rope_pos_rows = pos_rows;
   p.norm_w = (const __nv_bfloat16*)norm_w; p.norm_eps = norm_eps;
   p.kcache = (__nv_bfloat16*)kcache; p.vcache = (__nv_bfloat16*)vcache; p.cache_lmax = cache_lmax; p.cache_hd = cache_hd;
   const int rc = gemm_skinny_fused(p, (cudaStream_t)stream);
   if (rc == -1) { set_error("decode_gemm: shape not supported (M=%d N=%d K=%d)", M, N, K); return G4R_EUNSUPPORTED; }
   return rc;
+}
+
+extern "C" int g4r_decode_gemm_bf16(const void* x, long long ldx, const void* W, long long ldw, void* out, long long ldo,
+                                    int M, int N, int K, const void* norm_w, float norm_eps, int act, const void* residual,
+                                    long long ldr, const void* rope_cos, const void* rope_sin, int rope_cols, int pos0,
+                                    const int* pos_dev, void* kcache, void* vcache, int cache_lmax, int cache_hd,
+                                    void* stream) {
+  return decode_gemm(x, ldx, W, ldw, out, ldo, M, N, K, norm_w, norm_eps, act, residual, ldr, rope_cos, rope_sin, rope_cols,
+                     pos0, pos_dev, nullptr, kcache, vcache, cache_lmax, cache_hd, stream);
+}
+
+extern "C" int g4r_decode_gemm_rows_bf16(const void* x, long long ldx, const void* W, long long ldw, void* out,
+                                         long long ldo, int M, int N, int K, const void* norm_w, float norm_eps, int act,
+                                         const void* residual, long long ldr, const void* rope_cos, const void* rope_sin,
+                                         int rope_cols, const int* pos_rows, void* kcache, void* vcache, int cache_lmax,
+                                         int cache_hd, void* stream) {
+  G4R_REQUIRE(pos_rows && rope_cos, "decode_gemm_rows: per-sample positions need the RoPE tables and a pos_rows vector");
+  return decode_gemm(x, ldx, W, ldw, out, ldo, M, N, K, norm_w, norm_eps, act, residual, ldr, rope_cos, rope_sin, rope_cols,
+                     0, nullptr, pos_rows, kcache, vcache, cache_lmax, cache_hd, stream);
 }

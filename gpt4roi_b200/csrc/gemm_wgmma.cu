@@ -74,6 +74,7 @@ struct GemmParams {
   const __nv_bfloat16* rope_sin;
   int rope_cols, rope_L, rope_pos0;
   const int* rope_pos_dev;  // optional device-side position base (CUDA-graph decode): pos0 = *rope_pos_dev
+  const int* rope_pos_rows; // optional per-sample bases [M / rope_L] (prompts of different lengths); wins over both
   // operand majorness (backward GEMMs): a_mn: A is stored [K][M] (M contiguous); b_mn: B is stored [K][N];
   // b_mn == 2 (conv weight gradient): B is the zero-padded NHWC input seen through a 4-D tensor map
   // {Cin, kx, row, ky} whose kx / ky dimensions alias the row dimension (strides of 1 and W+2 rows), so that
@@ -143,7 +144,8 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float* 
     // Rounding as in the reference: q/k are bf16 GEMM outputs, each bf16 tensor op rounds:
     //   out = bf16( bf16(x*cos) + bf16(rot*sin) ),  rotate_half(x) = cat(-x2, x1).
     if (!row_ok) return;
-    const int pos = (p.rope_pos_dev ? *p.rope_pos_dev : p.rope_pos0) + (int)(out_row % p.rope_L);
+    const int base = p.rope_pos_rows ? p.rope_pos_rows[out_row / p.rope_L] : (p.rope_pos_dev ? *p.rope_pos_dev : p.rope_pos0);
+    const int pos = base + (int)(out_row % p.rope_L);
     const __nv_bfloat16* ct = p.rope_cos + (long long)pos * 128;
     const __nv_bfloat16* st = p.rope_sin + (long long)pos * 128;
 #pragma unroll 1
@@ -616,14 +618,14 @@ static int gemm_impl(const void* A, long long lda, const void* B, long long ldb,
                      int N, int K, const void* bias, int bias_f32, const void* residual, long long ldr,
                      int residual_f32, int bias_round_bf16, int act, int out_f32, int k_splits,
                      const void* rope_cos, const void* rope_sin, int rope_cols, int rope_L, void* stream,
-                     int rope_pos0 = 0, const int* rope_pos_dev = nullptr);
+                     int rope_pos0 = 0, const int* rope_pos_dev = nullptr, const int* rope_pos_rows = nullptr);
 
 namespace G4R_NS {
 // gemm_skinny.cu: M <= 16 weight-streaming path; returns -1 when the shape does not qualify
 int gemm_skinny_dispatch(const void* A, long long lda, const void* B, long long ldb, void* D, long long ldd, int M,
                          int N, int K, const void* bias, int bias_f32, const void* residual, long long ldr, int act,
                          const void* rope_cos, const void* rope_sin, int rope_cols, int rope_L, int rope_pos0,
-                         const int* rope_pos_dev, void* stream);
+                         const int* rope_pos_dev, const int* rope_pos_rows, void* stream);
 }
 static bool skinny_enabled() {
   static int v = -1;
@@ -650,6 +652,18 @@ extern "C" int g4r_gemm_qkv_rope_bf16(const void* A, long long lda, const void* 
   G4R_REQUIRE(rope_cols % 256 == 0 && rope_cols <= N && N % 128 == 0 && ldd % 8 == 0, "qkv_rope: rope_cols must be a multiple of 256 (whole tiles of 128-dim heads)");
   return gemm_impl(A, lda, B, ldb, D, ldd, M, N, K, nullptr, 0, nullptr, 0, 0, 0, ACT_NONE, 0, 1, rope_cos, rope_sin,
                    rope_cols, L, stream, pos0, pos0_dev);
+}
+
+// The same with a per-sample position base: row r (sample r / L) is rotated at pos_rows[r / L] + r % L -- a batch of
+// prompts of different lengths in the decode step (L = 1).
+extern "C" int g4r_gemm_qkv_rope_rows_bf16(const void* A, long long lda, const void* B, long long ldb, void* D,
+                                           long long ldd, int M, int N, int K, const void* rope_cos,
+                                           const void* rope_sin, int rope_cols, int L, const int* pos_rows,
+                                           void* stream) {
+  G4R_REQUIRE(rope_cos && rope_sin && pos_rows && L > 0 && M % L == 0, "qkv_rope_rows: null tables / pos_rows, or M %% L != 0");
+  G4R_REQUIRE(rope_cols % 256 == 0 && rope_cols <= N && N % 128 == 0 && ldd % 8 == 0, "qkv_rope: rope_cols must be a multiple of 256 (whole tiles of 128-dim heads)");
+  return gemm_impl(A, lda, B, ldb, D, ldd, M, N, K, nullptr, 0, nullptr, 0, 0, 0, ACT_NONE, 0, 1, rope_cos, rope_sin,
+                   rope_cols, L, stream, 0, nullptr, pos_rows);
 }
 
 // Backward-pass GEMM: D[M, N] = op(A) . op(B)^T with either operand optionally stored "MN-major":
@@ -748,7 +762,7 @@ static int gemm_impl(const void* A, long long lda, const void* B, long long ldb,
                      int N, int K, const void* bias, int bias_f32, const void* residual, long long ldr,
                      int residual_f32, int bias_round_bf16, int act, int out_f32, int k_splits,
                      const void* rope_cos, const void* rope_sin, int rope_cols, int rope_L, void* stream,
-                     int rope_pos0, const int* rope_pos_dev) {
+                     int rope_pos0, const int* rope_pos_dev, const int* rope_pos_rows) {
   G4R_REQUIRE(A && B && D, "null operand");
   G4R_REQUIRE(M > 0 && N > 0 && K > 0, "bad sizes M=%d N=%d K=%d", M, N, K);
   G4R_REQUIRE(lda % 8 == 0 && ldb % 8 == 0 && lda >= K && ldb >= K, "lda/ldb must be >= K and multiples of 8 (16-byte TMA strides)");
@@ -760,7 +774,7 @@ static int gemm_impl(const void* A, long long lda, const void* B, long long ldb,
   // M <= 16 (decode step): HBM-bound weight-streaming kernel instead of a mostly empty 128-row tile
   if (M <= 16 && !out_f32 && k_splits == 1 && !residual_f32 && !bias_round_bf16 && skinny_enabled()) {
     const int rc = gemm_skinny_dispatch(A, lda, B, ldb, D, ldd, M, N, K, bias, bias_f32, residual, ldr, act, rope_cos,
-                                        rope_sin, rope_cols, rope_L, rope_pos0, rope_pos_dev, stream);
+                                        rope_sin, rope_cols, rope_L, rope_pos0, rope_pos_dev, rope_pos_rows, stream);
     if (rc >= 0) return rc;
   }
   GemmParams p{};
@@ -775,6 +789,7 @@ static int gemm_impl(const void* A, long long lda, const void* B, long long ldb,
   p.round_branch = bias_round_bf16;
   p.rope_cos = (const __nv_bfloat16*)rope_cos; p.rope_sin = (const __nv_bfloat16*)rope_sin;
   p.rope_cols = rope_cols; p.rope_L = rope_L; p.rope_pos0 = rope_pos0; p.rope_pos_dev = rope_pos_dev;
+  p.rope_pos_rows = rope_pos_rows;
   p.act = act; p.out_f32 = out_f32;
   p.conv = 0; p.a_rows = kBlockM;
   const int bn = pick_block_n(p.num_m_tiles, N, k_splits);

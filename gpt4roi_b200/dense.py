@@ -129,19 +129,31 @@ def matmul_t(a, b, a_mn=False, b_mn=False, out_dtype=torch.bfloat16, out=None):
     return out
 
 
-def qkv_rope(x, wqkv, cos, sin, L, rope_cols, pos0=0, pos_dev=None):
+def _pos_rows(pos_rows, n):
+    if pos_rows.dtype != torch.int32 or tuple(pos_rows.shape) != (n,) or not pos_rows.is_contiguous():
+        raise RuntimeError('pos_rows must be a contiguous device int32 [%d] vector' % n)
+    return pos_rows
+
+
+def qkv_rope(x, wqkv, cos, sin, L, rope_cols, pos0=0, pos_dev=None, pos_rows=None):
     """Fused LLaMA q/k/v projection + rotary embedding: x [M,K] bf16, wqkv [N,K] (q|k|v rows), cos/sin
-    bf16 [L,128]; columns [0,rope_cols) (q and k heads, head_dim 128) are rotated at position row % L."""
+    bf16 [L,128]; columns [0,rope_cols) (q and k heads, head_dim 128) are rotated at position row % L.
+    pos_rows: device int32 [M / L] -- row r is rotated at pos_rows[r // L] + r % L instead (pos0 / pos_dev unused)."""
     M, K = x.shape
     N = wqkv.shape[0]
-    dev = _L.require_cuda_same_device([('x', x), ('wqkv', wqkv), ('cos', cos), ('sin', sin)])
+    dev = _L.require_cuda_same_device([('x', x), ('wqkv', wqkv), ('cos', cos), ('sin', sin), ('pos_rows', pos_rows)])
     a16 = _act16('qkv_rope', x, wqkv, cos, sin)
     out = torch.empty((M, N), dtype=a16, device=dev)
     with torch.cuda.device(dev):
         _ps = _prof_begin(dev)
-        _L.check(getattr(_L.load(), _L.sym('g4r_gemm_qkv_rope_bf16', a16))(
-            _L.ptr(x), x.stride(0), _L.ptr(wqkv), wqkv.stride(0), _L.ptr(out), N, M, N, K, _L.ptr(cos), _L.ptr(sin),
-            int(rope_cols), int(L), int(pos0), _L.ptr(pos_dev), _L.stream_ptr(dev)))
+        if pos_rows is not None:
+            _L.check(getattr(_L.load(), _L.sym('g4r_gemm_qkv_rope_rows_bf16', a16))(
+                _L.ptr(x), x.stride(0), _L.ptr(wqkv), wqkv.stride(0), _L.ptr(out), N, M, N, K, _L.ptr(cos), _L.ptr(sin),
+                int(rope_cols), int(L), _L.ptr(_pos_rows(pos_rows, M // L)), _L.stream_ptr(dev)))
+        else:
+            _L.check(getattr(_L.load(), _L.sym('g4r_gemm_qkv_rope_bf16', a16))(
+                _L.ptr(x), x.stride(0), _L.ptr(wqkv), wqkv.stride(0), _L.ptr(out), N, M, N, K, _L.ptr(cos), _L.ptr(sin),
+                int(rope_cols), int(L), int(pos0), _L.ptr(pos_dev), _L.stream_ptr(dev)))
         _prof_end(dev, _ps, 'gemm', 2.0 * M * N * K)
     return out
 
@@ -190,10 +202,11 @@ def conv_nhwc(x, weight_khwc, bias=None, act=None, gn_stats=None, out=None, leve
     return out
 
 
-def decode_gemm(x, weight, norm_w=None, norm_eps=1e-6, act=None, residual=None, rope=None, kv=None):
+def decode_gemm(x, weight, norm_w=None, norm_eps=1e-6, act=None, residual=None, rope=None, kv=None, pos_rows=None):
     """Decode-step GEMM (M = batch <= 16): out = [RoPE | SwiGLU | + residual](RMSNorm(x) @ weight.T), the norm, the
     rotary embedding and the KV-cache append folded into one weight-streaming launch (g4r_decode_gemm_bf16).
-    rope = (cos, sin, rope_cols, pos0, pos_dev); kv = (kcache [B,Lmax,HD], vcache) -- needs rope on the fused q|k|v weight."""
+    rope = (cos, sin, rope_cols, pos0, pos_dev); kv = (kcache [B,Lmax,HD], vcache) -- needs rope on the fused q|k|v weight.
+    pos_rows: device int32 [M] -- sample m is rotated at (and cached at) pos_rows[m] instead of pos0 / pos_dev."""
     M, K = x.shape
     N = weight.shape[0]
     dev = _L.require_cuda_same_device([('x', x), ('weight', weight), ('norm_w', norm_w), ('residual', residual)])
@@ -211,6 +224,16 @@ def decode_gemm(x, weight, norm_w=None, norm_eps=1e-6, act=None, residual=None, 
         lmax, hd = kc.shape[1], kc.shape[2]
     with torch.cuda.device(dev):
         _ps = _prof_begin(dev)
+        if pos_rows is not None:
+            if rope is None:
+                raise RuntimeError('decode_gemm: pos_rows needs rope')
+            _L.check(getattr(_L.load(), _L.sym('g4r_decode_gemm_rows_bf16', a16))(
+                _L.ptr(x), x.stride(0), _L.ptr(weight), weight.stride(0), _L.ptr(out), out.stride(0), M, N, K,
+                _L.ptr(norm_w), float(norm_eps), ACT[act], _L.ptr(residual), residual.stride(0) if residual is not None else 0,
+                _L.ptr(cos), _L.ptr(sin), int(rope_cols), _L.ptr(_pos_rows(pos_rows, M)), _L.ptr(kc), _L.ptr(vc), int(lmax),
+                int(hd), _L.stream_ptr(dev)))
+            _prof_end(dev, _ps, 'gemm', 2.0 * M * N * K)
+            return out
         _L.check(getattr(_L.load(), _L.sym('g4r_decode_gemm_bf16', a16))(
             _L.ptr(x), x.stride(0), _L.ptr(weight), weight.stride(0), _L.ptr(out), out.stride(0), M, N, K,
             _L.ptr(norm_w), float(norm_eps), ACT[act], _L.ptr(residual), residual.stride(0) if residual is not None else 0,

@@ -291,7 +291,9 @@ class PrefillEngine:
             x = dense.linear(f, w['wdown'], residual=x, **f32)
             if hidden_taps is not None and (li + 1) in hidden_taps:
                 hidden_taps[li + 1] = x.view(B, L, c.hidden).clone()
-        if last_only:
+        if last_only and seqlens is not None:   # each row's last valid position (right-padded rows)
+            x = x.view(B * L, c.hidden).index_select(0, torch.arange(B, device=x.device) * L + seqlens.long() - 1)
+        elif last_only:
             x = x.view(B, L, c.hidden)[:, -1].contiguous()
         x = kernels.rmsnorm(x, self.norm_w, c.rms_eps)
         if want == 'hidden':
@@ -333,7 +335,7 @@ class PrefillEngine:
             embeds = splice_region_tokens(input_ids, self.embed, None, None, 0, c.im_patch_token, c.im_start_token,
                                           c.im_end_token, c.bbox_token, validate=False)
             if cache is not None:
-                cache.length = L
+                cache.start(L, seqlens)
             return self.llama(embeds, B, L, last_only=last_only, seqlens=seqlens, cache=cache,
                               hidden_taps=hidden_taps, want=want)
         taps = self.vit(images)
@@ -354,7 +356,7 @@ class PrefillEngine:
             stage_taps['region'] = region[0] if (region is not None and plan['K'] > 0) else None
             stage_taps['embeds'] = embeds
         if cache is not None:
-            cache.length = L
+            cache.start(L, seqlens)
         return self.llama(embeds, B, L, last_only=last_only, seqlens=seqlens, cache=cache, hidden_taps=hidden_taps,
                           want=want)
 
@@ -362,27 +364,72 @@ class PrefillEngine:
                 hidden_taps=None, want='logits', stage_taps=None, cache=None):
         """Public entry: input_ids int64 [B,L]; images [B,3,S,S]; bboxes list (len B) of [K_i,4]
         normalised xyxy or None (host or device tensors).  Returns logits [B,L,V] (bf16) -- [B,1,V]
-        with last_only.  attention_mask: None / all-ones, or a RIGHT-padded 0/1 mask [B,L] (the collator's
-        pad_sequence layout, data_modules.py:33-44); logits at padded positions are don't-care."""
+        with last_only, taken at each row's last valid position.  attention_mask: None / all-ones, or a 0/1 mask [B,L]
+        whose rows are right-padded (the collator's pad_sequence layout, data_modules.py:33-44) or left-padded (HF's
+        layout for decoder-only generation).  Left-padded rows are rotated to the right-padded layout for the run and
+        the logits rotated back, so they come in the caller's layout; logits at padded positions are don't-care.
+        hidden_taps / stage_taps / the cache hold the right-padded layout."""
         plan = self.plan_boxes(bboxes)
         seqlens = None
+        input_ids = input_ids.to(self.dev, non_blocking=True)
+        shift = None
         if attention_mask is not None:
-            m = attention_mask.to(self.dev).to(torch.int32)
-            lens = m.sum(1)
-            if not bool((m == (torch.arange(m.shape[1], device=self.dev)[None] < lens[:, None])).all()):
-                raise NotImplementedError('only right-padded attention masks are supported')
+            lens, shift = right_pad_layout(attention_mask.to(self.dev))
             seqlens = lens.to(torch.int32).contiguous()
-        return self.forward_device(input_ids.to(self.dev, non_blocking=True).contiguous(),
-                                   None if images is None else images.to(self.dev, self.dt, non_blocking=True).contiguous(),
-                                   plan, validate, last_only, seqlens, cache=cache, hidden_taps=hidden_taps, want=want,
-                                   stage_taps=stage_taps)
+            if bool(shift.any()):
+                input_ids = to_right_padded(input_ids, shift)
+            else:
+                shift = None
+        out = self.forward_device(input_ids.contiguous(),
+                                  None if images is None else images.to(self.dev, self.dt, non_blocking=True).contiguous(),
+                                  plan, validate, last_only, seqlens, cache=cache, hidden_taps=hidden_taps, want=want,
+                                  stage_taps=stage_taps)
+        if shift is not None and not last_only:
+            out = from_right_padded(out, shift)
+        return out
+
+
+def right_pad_layout(attention_mask):
+    """0/1 mask [B, L] whose rows are each right- or left-padded -> (lens, shift), int64 [B] on the mask's device:
+    row b's tokens are columns shift[b] .. shift[b] + lens[b] - 1 (shift 0: right-padded, L - lens[b]: left-padded).
+    Any other layout (holes, padding on both sides, an empty row) raises NotImplementedError."""
+    m = attention_mask.to(torch.int64)
+    B, L = m.shape
+    lens = m.sum(1)
+    shift = m.argmax(1)                      # first 1 of the row
+    col = torch.arange(L, device=m.device)[None]
+    want = (col >= shift[:, None]) & (col < (shift + lens)[:, None])
+    ok = (m == want.to(torch.int64)).all(1) & (lens > 0) & ((shift == 0) | (shift + lens == L))
+    if not bool(ok.all()):
+        raise NotImplementedError('attention_mask rows must be right- or left-padded runs of ones (rows %s are not)'
+                                  % (~ok).nonzero().flatten().tolist())
+    return lens, shift
+
+
+def _rotate(x, shift):
+    B, L = x.shape[:2]
+    idx = (torch.arange(L, device=x.device)[None] + shift.to(x.device)[:, None]) % L
+    return x.gather(1, idx.view(B, L, *([1] * (x.dim() - 2))).expand(x.shape))
+
+
+def to_right_padded(x, shift):
+    """[B, L, ...] in the caller's layout -> right-padded layout: row b rotated left by shift[b] (right_pad_layout)."""
+    return _rotate(x, shift)
+
+
+def from_right_padded(x, shift):
+    """Inverse of to_right_padded."""
+    return _rotate(x, (x.shape[1] - shift) % x.shape[1])
 
 
 _DECODE_FUSED = int(__import__('os').environ.get('G4R_DECODE_FUSED', '1'))
 
 
 class KVCache:
-    """Per-layer K/V cache [B, Lmax, n_heads*head_dim] (the engine's 16-bit type, post-RoPE keys) for the decode loop."""
+    """Per-layer K/V cache [B, Lmax, n_heads*head_dim] (the engine's 16-bit type, post-RoPE keys) for the decode loop.
+    length: columns in use (padded prompt length + decode steps).  lens: None when every sample uses all `length`
+    columns, else a device int32 [B] with each sample's own length (a right-padded batch of prompts of different
+    lengths): sample b's next token sits at position lens[b] and attends over columns 0..lens[b]."""
 
     def __init__(self, cfg, B, max_len, device):
         hd = cfg.n_heads * cfg.head_dim
@@ -390,13 +437,21 @@ class KVCache:
         self.k = [torch.empty((B, max_len, hd), dtype=dt, device=device) for _ in range(cfg.n_layers)]
         self.v = [torch.empty((B, max_len, hd), dtype=dt, device=device) for _ in range(cfg.n_layers)]
         self.B, self.max_len, self.length = B, max_len, 0
+        self.lens = None
+
+    def start(self, L, seqlens=None):
+        """A prefill of L columns fills the cache; seqlens (device int32 [B]): the valid length of each row."""
+        self.length = L
+        self.lens = None if seqlens is None else seqlens.to(torch.int32).clone()
 
 
 def _decode_step(self, token_ids, cache, pos_dev=None):
     """One decode step (SURVEY.md 8(f1)): token_ids int64 [B,1] -> logits [B,1,V]; the vision / SPI branch
     is skipped exactly as the reference does for input_ids.shape[1] == 1 (spi_llava.py:47-48).
     pos_dev: optional device int32 holding the current length (CUDA-graph replay: the kernels read the
-    position from memory instead of from a launch argument)."""
+    position from memory instead of from a launch argument).
+    On a cache with per-sample lengths (cache.lens) every kernel takes sample b's position from cache.lens[b], which
+    the step advances on the device -- except under graph capture (pos_dev given), where GraphedDecode.step does."""
     from . import lib
     if cache.length + 1 > cache.max_len:
         raise RuntimeError('KV cache is full (%d)' % cache.max_len)
@@ -414,6 +469,7 @@ def _decode_step_chain(self, token_ids, cache, pos_dev):
     B = token_ids.shape[0]
     pos = cache.length
     kv_len = cache.max_len if pos_dev is not None else pos + 1   # sizes the score buffer when device-driven
+    rows = cache.lens        # per-sample positions (<= pos): these override pos / pos_dev in every kernel
     x = splice_region_tokens(token_ids, self.embed, None, None, 0, c.im_patch_token, c.im_start_token,
                              c.im_end_token, c.bbox_token, validate=False).view(B, c.hidden)
     cos, sin = self._rope(cache.max_len)
@@ -428,8 +484,10 @@ def _decode_step_chain(self, token_ids, cache, pos_dev):
             nrm = _DECODE_FUSED >= 2
             h = x if nrm else kernels.rmsnorm(x, w['ln_in'], c.rms_eps)
             qkv = dense.decode_gemm(h, w['wqkv'], norm_w=w['ln_in'] if nrm else None, norm_eps=c.rms_eps,
-                                    rope=(cos, sin, 2 * c.hidden, pos, pos_dev), kv=(cache.k[li], cache.v[li]))
-            a = kernels.decode_attention(qkv, cache.k[li], cache.v[li], B, c.n_heads, c.head_dim, kv_len, scale, pos_dev)
+                                    rope=(cos, sin, 2 * c.hidden, pos, pos_dev), kv=(cache.k[li], cache.v[li]),
+                                    pos_rows=rows)
+            a = kernels.decode_attention(qkv, cache.k[li], cache.v[li], B, c.n_heads, c.head_dim, kv_len, scale, pos_dev,
+                                         pos_rows=rows)
             x = dense.linear(a, w['wo'], residual=x)
             h = x if nrm else kernels.rmsnorm(x, w['ln_post'], c.rms_eps)
             f = dense.decode_gemm(h, w['wgu'], norm_w=w['ln_post'] if nrm else None, norm_eps=c.rms_eps, act='swiglu')
@@ -437,19 +495,24 @@ def _decode_step_chain(self, token_ids, cache, pos_dev):
             continue
         h = kernels.rmsnorm(x, w['ln_in'], c.rms_eps)
         if fused:
-            qkv = dense.qkv_rope(h, w['wqkv'], cos, sin, 1, 2 * c.hidden, pos0=pos, pos_dev=pos_dev)
+            qkv = dense.qkv_rope(h, w['wqkv'], cos, sin, 1, 2 * c.hidden, pos0=pos, pos_dev=pos_dev, pos_rows=rows)
         else:
             if pos_dev is not None:
                 raise NotImplementedError('graph decode needs the fused-RoPE QKV GEMM (head_dim 128)')
+            if rows is not None:
+                raise NotImplementedError('prompts of different lengths need the fused-RoPE QKV GEMM (head_dim 128)')
             qkv = dense.linear(h, w['wqkv'])
             kernels.rope_inplace(qkv, cos[pos:pos + 1].contiguous(), sin[pos:pos + 1].contiguous(), 1, 2 * c.n_heads, c.head_dim)
-        kernels.kv_append(qkv, cache.k[li], cache.v[li], B, 1, pos, pos_dev)
-        a = kernels.decode_attention(qkv, cache.k[li], cache.v[li], B, c.n_heads, c.head_dim, kv_len, scale, pos_dev)
+        kernels.kv_append(qkv, cache.k[li], cache.v[li], B, 1, pos, pos_dev, pos_rows=rows)
+        a = kernels.decode_attention(qkv, cache.k[li], cache.v[li], B, c.n_heads, c.head_dim, kv_len, scale, pos_dev,
+                                     pos_rows=rows)
         x = dense.linear(a, w['wo'], residual=x)
         h = kernels.rmsnorm(x, w['ln_post'], c.rms_eps)
         f = dense.linear(h, w['wgu'], act='swiglu')
         x = dense.linear(f, w['wdown'], residual=x)
     cache.length = pos + 1
+    if rows is not None and pos_dev is None:
+        rows.add_(1)
     x = kernels.rmsnorm(x, self.norm_w, c.rms_eps)
     buf = torch.empty((B, self.vocab_pad), dtype=self.dt, device=self.dev)
     dense.linear(x, self.lm_head, out=buf[:, :c.vocab])
@@ -458,27 +521,50 @@ def _decode_step_chain(self, token_ids, cache, pos_dev):
 
 @torch.no_grad()
 def _generate(self, input_ids, images, bboxes, max_new_tokens=32, do_sample=False, temperature=1.0,
-              stopping_criteria=None, eos_token_id=None, generator=None, use_graph=True):
+              stopping_criteria=None, eos_token_id=None, generator=None, use_graph=True, attention_mask=None,
+              pad_token_id=None):
     """Prefill + greedy / temperature-sampled decode (gpt4roi/app.py:286-300 calls
     model.generate(input_ids, images=..., do_sample=True, temperature=0.2, max_new_tokens=1024,
-    stopping_criteria=[...]) with the boxes bound to forward).  Returns ids [B, L + new]."""
+    stopping_criteria=[...]) with the boxes bound to forward).  Returns ids [B, L + new]: the prompt as given,
+    then the new tokens (HF's layout).
+    attention_mask: 0/1 [B, L] for a batch of prompts of different lengths, each row right- or left-padded; the
+    prefill runs on the right-padded layout and every sample continues from its own last token.
+    pad_token_id (with eos_token_id): a sample that has emitted eos_token_id gets pad_token_id from then on and the
+    loop ends once every sample has (transformers' GenerationMixin rule); without it the loop ends when all samples
+    emit eos_token_id at the same step."""
     B, L = input_ids.shape
     cache = KVCache(self.cfg, B, L + max_new_tokens, self.dev)
     plan = self.plan_boxes(bboxes)
     ids = input_ids.to(self.dev)
-    logits = self.forward_device(ids, images.to(self.dev, self.dt), plan, validate=True, last_only=True, cache=cache)
+    run_ids, seqlens = ids, None
+    if attention_mask is not None:
+        lens, shift = right_pad_layout(attention_mask.to(self.dev))
+        if bool(shift.any()):
+            run_ids = to_right_padded(ids, shift).contiguous()
+        if not bool((lens == L).all()):
+            seqlens = lens.to(torch.int32).contiguous()
+    logits = self.forward_device(run_ids, images.to(self.dev, self.dt), plan, validate=True, last_only=True,
+                                 seqlens=seqlens, cache=cache)
     out = ids
     stepper = None
     if use_graph and max_new_tokens > 4 and self.cfg.head_dim == 128:
         stepper = GraphedDecode(self, cache)
+    finished = None
     for step in range(max_new_tokens):
         last = logits[:, -1].float()
         if do_sample and temperature > 0:
             nxt = torch.multinomial(torch.softmax(last / temperature, -1), 1, generator=generator)
         else:
             nxt = last.argmax(-1, keepdim=True)
+        if pad_token_id is not None and eos_token_id is not None:
+            if finished is not None:
+                nxt = torch.where(finished, torch.full_like(nxt, pad_token_id), nxt)
+            finished = (nxt == eos_token_id) if finished is None else finished | (nxt == eos_token_id)
         out = torch.cat([out, nxt], 1)
-        if eos_token_id is not None and bool((nxt == eos_token_id).all()):
+        if finished is not None:
+            if bool(finished.all()):
+                break
+        elif eos_token_id is not None and bool((nxt == eos_token_id).all()):
             break
         if stopping_criteria is not None and any(bool(torch.as_tensor(sc(out, last)).all()) for sc in stopping_criteria):
             break
@@ -489,7 +575,8 @@ def _generate(self, input_ids, images, bboxes, max_new_tokens=32, do_sample=Fals
 
 class GraphedDecode:
     """CUDA-graph replay of one decode step: ~260 launches become one.  The current length lives in a
-    device int32 that the QKV-RoPE epilogue, kv_append and decode_attention read; `step` bumps it."""
+    device int32 that the QKV-RoPE epilogue, kv_append and decode_attention read; `step` bumps it (and the
+    per-sample lengths cache.lens of a batch of prompts of different lengths, which those kernels then read instead)."""
 
     def __init__(self, engine, cache):
         self.eng, self.cache = engine, cache
@@ -516,6 +603,8 @@ class GraphedDecode:
         self.ids.copy_(token_ids, non_blocking=True)
         self.graph.replay()
         self.pos.add_(1)
+        if self.cache.lens is not None:   # per-sample positions: the graph reads this very tensor
+            self.cache.lens.add_(1)
         self.cache.length += 1
         return self.logits
 

@@ -190,17 +190,36 @@ def add_bias_pos_cast(acc, bias, pos):
     return out
 
 
-def kv_append(qkv, kcache, vcache, B, Ln, pos0, pos_dev=None):
-    """Copy the k|v parts of packed qkv rows [B*Ln, 3*HD] into caches [B, Lmax, HD] at pos0..pos0+Ln-1."""
+def _pos_rows(pos_rows, B):
+    if pos_rows.dtype != torch.int32 or tuple(pos_rows.shape) != (B,) or not pos_rows.is_contiguous():
+        raise RuntimeError('pos_rows must be a contiguous device int32 [%d] vector' % B)
+    return pos_rows
+
+
+def kv_append(qkv, kcache, vcache, B, Ln, pos0, pos_dev=None, pos_rows=None):
+    """Copy the k|v parts of packed qkv rows [B*Ln, 3*HD] into caches [B, Lmax, HD] at pos0..pos0+Ln-1.
+    pos_rows: device int32 [B] -- sample b's rows go to pos_rows[b]..pos_rows[b]+Ln-1 instead (pos0 / pos_dev unused)."""
     HD = kcache.shape[-1]
+    act = _bf16(qkv, kcache, vcache)
+    if pos_rows is not None:
+        _call('g4r_kv_append_rows_bf16', qkv.device, _L.ptr(qkv), qkv.stride(0), _L.ptr(kcache), _L.ptr(vcache), B, Ln,
+              _L.ptr(_pos_rows(pos_rows, B)), kcache.shape[1], HD, act=act)
+        return
     _call('g4r_kv_append_bf16', qkv.device, _L.ptr(qkv), qkv.stride(0), _L.ptr(kcache), _L.ptr(vcache), B, Ln,
-          int(pos0), _L.ptr(pos_dev), kcache.shape[1], HD, act=_bf16(qkv, kcache, vcache))
+          int(pos0), _L.ptr(pos_dev), kcache.shape[1], HD, act=act)
 
 
-def decode_attention(qkv, kcache, vcache, B, n_heads, head_dim, kv_len, scale, pos_dev=None):
-    """qkv [B, 3*HD] (one new token per sample); caches [B, Lmax, HD]; returns [B, HD]."""
+def decode_attention(qkv, kcache, vcache, B, n_heads, head_dim, kv_len, scale, pos_dev=None, pos_rows=None):
+    """qkv [B, 3*HD] (one new token per sample); caches [B, Lmax, HD]; returns [B, HD].
+    pos_rows: device int32 [B] -- sample b attends over its first pos_rows[b] + 1 keys; kv_len is then only the bound
+    (>= every row's length) that sizes the split and the score buffer."""
     act = _bf16(qkv, kcache, vcache)
     out = torch.empty((B, n_heads * head_dim), dtype=act, device=qkv.device)
+    if pos_rows is not None:
+        _call('g4r_decode_attention_rows_bf16', qkv.device, _L.ptr(qkv), qkv.stride(0), _L.ptr(kcache), _L.ptr(vcache),
+              _L.ptr(out), out.stride(0), B, n_heads, head_dim, int(kv_len), _L.ptr(_pos_rows(pos_rows, B)),
+              kcache.shape[1], float(scale), act=act)
+        return out
     _call('g4r_decode_attention_bf16', qkv.device, _L.ptr(qkv), qkv.stride(0), _L.ptr(kcache), _L.ptr(vcache),
           _L.ptr(out), out.stride(0), B, n_heads, head_dim, int(kv_len), _L.ptr(pos_dev), kcache.shape[1], float(scale),
           act=act)

@@ -48,6 +48,11 @@ SIGNATURES = {
                                   _i, _i, _vp]),
     'g4r_kv_append_bf16': (_i, [_vp, _ll, _vp, _vp, _i, _i, _i, _vp, _i, _i, _vp]),
     'g4r_decode_attention_bf16': (_i, [_vp, _ll, _vp, _vp, _vp, _ll, _i, _i, _i, _i, _vp, _i, _f, _vp]),
+    'g4r_gemm_qkv_rope_rows_bf16': (_i, [_vp, _ll, _vp, _ll, _vp, _ll, _i, _i, _i, _vp, _vp, _i, _i, _vp, _vp]),
+    'g4r_decode_gemm_rows_bf16': (_i, [_vp, _ll, _vp, _ll, _vp, _ll, _i, _i, _i, _vp, _f, _i, _vp, _ll, _vp, _vp, _i, _vp,
+                                       _vp, _vp, _i, _i, _vp]),
+    'g4r_kv_append_rows_bf16': (_i, [_vp, _ll, _vp, _vp, _i, _i, _vp, _i, _i, _vp]),
+    'g4r_decode_attention_rows_bf16': (_i, [_vp, _ll, _vp, _vp, _vp, _ll, _i, _i, _i, _i, _vp, _i, _f, _vp]),
     'g4r_conv_nhwc_bf16': (_i, [_vp] * 3 + [_i] * 7 + [_vp, _i, _i, _vp, _i, _vp]),
     'g4r_attention_bf16': (_i, [_vp] * 4 + [_ll] * 4 + [_i] * 5 + [_f, _vp, _vp]),
     'g4r_attention_tc_bf16': (_i, [_vp] * 4 + [_ll] * 4 + [_i] * 5 + [_f, _vp, _vp]),
@@ -122,6 +127,10 @@ F16_TWINS = {
     'g4r_decode_gemm_bf16': 'g4r_decode_gemm_f16',
     'g4r_kv_append_bf16': 'g4r_kv_append_f16',
     'g4r_decode_attention_bf16': 'g4r_decode_attention_f16',
+    'g4r_gemm_qkv_rope_rows_bf16': 'g4r_gemm_qkv_rope_rows_f16',
+    'g4r_decode_gemm_rows_bf16': 'g4r_decode_gemm_rows_f16',
+    'g4r_kv_append_rows_bf16': 'g4r_kv_append_rows_f16',
+    'g4r_decode_attention_rows_bf16': 'g4r_decode_attention_rows_f16',
 }
 SIGNATURES.update({twin: SIGNATURES[name] for name, twin in F16_TWINS.items()})
 

@@ -35,7 +35,8 @@ import torch.nn as nn
 from transformers import LlamaConfig, LlamaForCausalLM, LlamaModel
 from transformers.modeling_outputs import BaseModelOutputWithPast, CausalLMOutputWithPast
 
-from .engine import BF16, EngineConfig, KVCache, PrefillEngine
+from .engine import (BF16, EngineConfig, KVCache, PrefillEngine, from_right_padded, right_pad_layout,
+                     to_right_padded)
 from .roi_align import RoIAlign
 
 DEFAULT_IMAGE_PATCH_TOKEN = '<im_patch>'
@@ -364,11 +365,9 @@ def _seqlens(eng, attention_mask, L):
     m = attention_mask.to(eng.dev).to(torch.int32)
     if m.shape[1] != L:
         return None          # a grown decode-time mask (HF generate appends ones): positions come from the cache
-    lens = m.sum(1)
-    if bool((lens == L).all()):
+    if bool((m == 1).all()):
         return None
-    if not bool((m == (torch.arange(L, device=eng.dev)[None] < lens[:, None])).all()):
-        raise NotImplementedError('only right-padded attention masks are supported (data_modules.py:33-44 pads right)')
+    lens, _ = right_pad_layout(m)   # right-padded (data_modules.py:33-44) or left-padded (HF generate) rows
     return lens.to(torch.int32).contiguous()
 
 
@@ -423,10 +422,19 @@ def _run_engine(eng, input_ids, images, bboxes, attention_mask, past_key_values,
     kv = new_cache.kv if new_cache is not None else None
     if inputs_embeds is not None:
         B, L = inputs_embeds.shape[:2]
-        x = inputs_embeds.to(eng.dev, eng.dt).contiguous()
+        x = inputs_embeds.to(eng.dev, eng.dt)
+        seqlens = _seqlens(eng, attention_mask, L)
+        shift = None
+        if seqlens is not None:
+            _, shift = right_pad_layout(attention_mask.to(eng.dev))
+            shift = shift if bool(shift.any()) else None
+            if shift is not None:
+                x = to_right_padded(x, shift)
         if kv is not None:
-            kv.length = L
-        out = eng.llama(x, B, L, seqlens=_seqlens(eng, attention_mask, L), cache=kv, want=want, last_only=last_only)
+            kv.start(L, seqlens)
+        out = eng.llama(x.contiguous(), B, L, seqlens=seqlens, cache=kv, want=want, last_only=last_only)
+        if shift is not None and not last_only:
+            out = from_right_padded(out, shift)
         return out, new_cache
     B, L = input_ids.shape
     run_vision = images is not None and (L != 1 or training)
@@ -616,7 +624,9 @@ class SPILlavaMPTForCausalLM(LlamaForCausalLM, _EngineHost):
         passes (gpt4roi/app.py:293-300); boxes may be given here or bound the way app.py does
         (`self.forward = partial(self.forward, bboxes=...)`, :286-291).  Returns ids [B, L+new] like HF.
         use_hf_loop=True runs transformers' own GenerationMixin.generate over this model's forward /
-        prepare_inputs_for_generation / past_key_values instead of the engine's loop."""
+        prepare_inputs_for_generation / past_key_values instead of the engine's loop.
+        attention_mask (right- or left-padded) and pad_token_id reach either loop: prompts of different lengths in one
+        batch each continue from their own last token, and finished rows are filled with pad_token_id."""
         if bboxes is None:
             bboxes = getattr(getattr(self, 'forward', None), 'keywords', {}).get('bboxes')
         if use_hf_loop:
@@ -633,7 +643,8 @@ class SPILlavaMPTForCausalLM(LlamaForCausalLM, _EngineHost):
                                     do_sample=do_sample, use_cache=True, **kw)
         eng = self._get_engine(input_ids.device)
         return eng.generate(input_ids, images, bboxes, max_new_tokens=max_new_tokens, do_sample=do_sample,
-                            temperature=temperature, stopping_criteria=stopping_criteria, eos_token_id=eos_token_id)
+                            temperature=temperature, stopping_criteria=stopping_criteria, eos_token_id=eos_token_id,
+                            attention_mask=kwargs.get('attention_mask'), pad_token_id=kwargs.get('pad_token_id'))
 
     def initialize_vision_tokenizer(self, mm_use_im_start_end, tokenizer, device, tune_mm_mlp_adapter=False,
                                     pretrain_mm_mlp_adapter=None):

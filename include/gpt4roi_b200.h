@@ -249,6 +249,35 @@ int g4r_decode_attention_bf16(const void* q, long long ldq, const void* kcache, 
                               const int* pos_dev /* kv_len = *pos_dev + 1 when non-NULL; kv_len then sizes smem */,
                               int Lmax, float scale, void* stream);
 
+/* ---- decode loop over prompts of different lengths (per-sample positions) ------------------
+ * The four decode entry points above with one position per sample instead of one for the whole batch: pos_rows is a
+ * device int32 [B] vector, sample b's new token sits at position pos_rows[b] and attends over cache rows
+ * 0..pos_rows[b].  This is what transformers' generate() does for a padded batch (per-row position_ids from the
+ * attention mask, padded keys masked out); here the prompts are packed to the left of the cache instead (right
+ * padding) and each sample's length lives on the device, so the step stays capturable in a CUDA graph.  The vector is
+ * read where the scalar *pos_dev is read, so it may be updated between graph replays.  Results for a vector whose
+ * entries are all equal are bitwise those of the scalar entry at that position.  Caller's contract: pos_rows[b] + Ln
+ * <= Lmax (append), pos_rows[b] < kv_bound (attention), and the RoPE tables cover every position. */
+/* g4r_gemm_qkv_rope_bf16 with row r (sample r / L) rotated at pos_rows[r / L] + r % L. */
+int g4r_gemm_qkv_rope_rows_bf16(const void* A, long long lda, const void* B, long long ldb,
+                                void* D, long long ldd, int M, int N, int K,
+                                const void* rope_cos, const void* rope_sin, int rope_cols, int L,
+                                const int* pos_rows, void* stream);
+/* g4r_decode_gemm_bf16 with sample m rotated at, and its k / v columns written to cache[m, pos_rows[m], :]. */
+int g4r_decode_gemm_rows_bf16(const void* x, long long ldx, const void* W, long long ldw, void* out, long long ldo,
+                              int M, int N, int K, const void* norm_w, float norm_eps, int act, const void* residual,
+                              long long ldr, const void* rope_cos, const void* rope_sin, int rope_cols,
+                              const int* pos_rows, void* kcache, void* vcache, int cache_lmax, int cache_hd,
+                              void* stream);
+/* g4r_kv_append_bf16 with sample b's rows at positions pos_rows[b] .. pos_rows[b]+Ln-1. */
+int g4r_kv_append_rows_bf16(const void* qkv, long long ld, void* kcache, void* vcache,
+                            int B, int Ln, const int* pos_rows, int Lmax, int HD, void* stream);
+/* g4r_decode_attention_bf16 with sample b over its first pos_rows[b] + 1 cached positions; kv_bound (>= every
+ * pos_rows[b] + 1, e.g. Lmax in a CUDA graph) sizes the split-KV factor and the shared-memory score buffer. */
+int g4r_decode_attention_rows_bf16(const void* q, long long ldq, const void* kcache, const void* vcache,
+                                   void* out, long long ldo, int B, int H, int head_dim, int kv_bound,
+                                   const int* pos_rows, int Lmax, float scale, void* stream);
+
 /*
  * NHWC convolution as an implicit GEMM (stride 1, pad (ksize-1)/2, ksize 1 or 3):
  *   Y[n,y,x,co] = act( sum_{ky,kx,ci} X[n,y+ky-1,x+kx-1,ci] * Wt[co,(ky*ks+kx)*Cin+ci] + bias[co] )
@@ -575,6 +604,20 @@ int g4r_decode_attention_f16(const void* q, long long ldq, const void* kcache, c
                               void* out, long long ldo, int B, int H, int head_dim, int kv_len,
                               const int* pos_dev /* kv_len = *pos_dev + 1 when non-NULL; kv_len then sizes smem */,
                               int Lmax, float scale, void* stream);
+int g4r_gemm_qkv_rope_rows_f16(const void* A, long long lda, const void* B, long long ldb,
+                               void* D, long long ldd, int M, int N, int K,
+                               const void* rope_cos, const void* rope_sin, int rope_cols, int L,
+                               const int* pos_rows, void* stream);
+int g4r_decode_gemm_rows_f16(const void* x, long long ldx, const void* W, long long ldw, void* out, long long ldo,
+                             int M, int N, int K, const void* norm_w, float norm_eps, int act, const void* residual,
+                             long long ldr, const void* rope_cos, const void* rope_sin, int rope_cols,
+                             const int* pos_rows, void* kcache, void* vcache, int cache_lmax, int cache_hd,
+                             void* stream);
+int g4r_kv_append_rows_f16(const void* qkv, long long ld, void* kcache, void* vcache,
+                           int B, int Ln, const int* pos_rows, int Lmax, int HD, void* stream);
+int g4r_decode_attention_rows_f16(const void* q, long long ldq, const void* kcache, const void* vcache,
+                                  void* out, long long ldo, int B, int H, int head_dim, int kv_bound,
+                                  const int* pos_rows, int Lmax, float scale, void* stream);
 
 #ifdef __cplusplus
 }
