@@ -55,6 +55,7 @@
 #define g4r_decode_gemm_rows_bf16 g4r_decode_gemm_rows_f16
 #define g4r_kv_append_rows_bf16 g4r_kv_append_rows_f16
 #define g4r_decode_attention_rows_bf16 g4r_decode_attention_rows_f16
+#define g4r_attention_cached_bf16 g4r_attention_cached_f16
 
 #else
 #define G4R_NS g4r

@@ -11,6 +11,16 @@
 //                            O += P_j V_j  (wgmma with P as the register A operand, bf16; V consumed as an
 //                            MN-major B operand straight from its [keys][d] layout -- no transpose pass)
 // Scores stay fp32 through the softmax (see attention.cu header).
+//
+// CACHED mode (g4r_attention_cached_bf16): the queries are a chunk of Lc new tokens per row that continues a sequence
+// held in the KV cache [B, Lmax, H*D]; its own K/V were appended to the cache before the launch, so every key comes
+// from the cache.  Row b's chunk starts at position start[b] (the number of cached tokens before it) and has qlen[b]
+// valid queries; query i attends over cache positions 0 .. start[b] + i.  Key blocks stay aligned to position 0.
+// Output rows >= qlen[b] stay finite: rows inside a computed tile attend over the valid keys, and 128-row tiles
+// wholly past qlen[b] are written as zeros.
+// The last key block reads cache rows past start[b] + qlen[b], up to the next multiple of 64: those rows must hold
+// finite values (masked scores give p = 0, but 0 * NaN in P.V would still poison the row), so the cache is allocated
+// zero-filled.
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -31,6 +41,10 @@ struct FaParams {
   float scale;
   const int* seqlens;
   float* lse;   // optional [B, H, L]: natural-log sum-exp of the scaled scores (training forward; attention_bwd reads it)
+  // CACHED mode only
+  int kv_L;            // Lmax: rows per batch entry in the K/V tensor maps
+  const int* start;    // [B] first position of each row's chunk
+  const int* qlen;     // [B] valid queries of each row's chunk, or NULL (all L)
 };
 
 __device__ __forceinline__ uint32_t pack_act2(float a, float b) {
@@ -44,7 +58,7 @@ __device__ __forceinline__ void wgmma_pv(float (&o)[D / 2], const uint32_t (&a)[
   else ptx::wgmma_m64n64_rs<1>(o, a, db, 1);
 }
 
-template <int D, bool CAUSAL>
+template <int D, bool CAUSAL, bool CACHED = false>
 __global__ void __launch_bounds__(kFaThreads, 1)
 fa_fwd_wgmma(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ CUtensorMap tm_k,
              const __grid_constant__ CUtensorMap tm_v, const __grid_constant__ FaParams p) {
@@ -70,8 +84,27 @@ fa_fwd_wgmma(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ C
   const int qb = CAUSAL ? (int)(gridDim.x - 1 - blockIdx.x) : (int)blockIdx.x, h = blockIdx.y, b = blockIdx.z;
   const int q0 = qb * kFaBM;
   const int row_base = b * p.L;
-  const int Lk = p.seqlens ? min(max(p.seqlens[b], 1), p.L) : p.L;
-  const int nblk = CAUSAL ? min((Lk + kFaBN - 1) / kFaBN, (q0 + kFaBM + kFaBN - 1) / kFaBN) : (Lk + kFaBN - 1) / kFaBN;
+  int kv_base = row_base, koff = 0, Lk, nblk;
+  if constexpr (CACHED) {
+    // causal in cache coordinates: query i of the chunk sits at position koff + i
+    const int ql = p.qlen ? min(max(p.qlen[b], 1), p.L) : p.L;
+    if (q0 >= ql) {
+      // whole tile past the valid rows: no work, but its outputs are zeroed -- the engine feeds them on through wo
+      // into the next layer's K/V, which later chunks read masked (p = 0) and need finite
+      const int rows = min(kFaBM, p.L - q0);
+      for (int i = threadIdx.x; i < rows * (D / 8); i += kFaThreads)
+        *reinterpret_cast<uint4*>(p.out + (long long)b * p.bso + (long long)(q0 + i / (D / 8)) * p.ldo +
+                                  (long long)h * D + (i % (D / 8)) * 8) = make_uint4(0, 0, 0, 0);
+      return;
+    }
+    kv_base = b * p.kv_L;
+    koff = p.start[b];
+    Lk = koff + min(q0 + kFaBM, ql);
+    nblk = (Lk + kFaBN - 1) / kFaBN;
+  } else {
+    Lk = p.seqlens ? min(max(p.seqlens[b], 1), p.L) : p.L;
+    nblk = CAUSAL ? min((Lk + kFaBN - 1) / kFaBN, (q0 + kFaBM + kFaBN - 1) / kFaBN) : (Lk + kFaBN - 1) / kFaBN;
+  }
 
   if (threadIdx.x == 0) {
     ptx::prefetch_tensormap(&tm_q);
@@ -101,12 +134,12 @@ fa_fwd_wgmma(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ C
         ptx::mbar_arrive_expect_tx(&k_full[st], TILE_BYTES);
         for (int a = 0; a < ATOMS; a++)
           ptx::tma_load_2d(sK + st * TILE_BYTES + a * KV_ATOM, &tm_k, &k_full[st], h * D + a * 64,
-                           row_base + j * kFaBN);
+                           kv_base + j * kFaBN);
         ptx::mbar_wait(&v_empty[st], ph ^ 1);
         ptx::mbar_arrive_expect_tx(&v_full[st], TILE_BYTES);
         for (int a = 0; a < ATOMS; a++)
           ptx::tma_load_2d(sV + st * TILE_BYTES + a * KV_ATOM, &tm_v, &v_full[st], h * D + a * 64,
-                           row_base + j * kFaBN);
+                           kv_base + j * kFaBN);
       }
     }
     return;
@@ -145,14 +178,14 @@ fa_fwd_wgmma(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ C
     if (wt == 0) ptx::mbar_arrive(&k_empty[st]);
     // ---- mask, row max (a row's 64 scores are spread over the 4 threads of a quad)
     const int key0 = j * kFaBN;
-    const bool need_mask = (key0 + kFaBN > Lk) || (CAUSAL && key0 + kFaBN - 1 > wg_q0);
+    const bool need_mask = (key0 + kFaBN > Lk) || (CAUSAL && key0 + kFaBN - 1 > koff + wg_q0);
     float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
     for (int i = 0; i < kFaBN / 2; i++) {
       const int hr = (i >> 1) & 1;
       if (need_mask) {
         const int key = key0 + (i >> 2) * 8 + 2 * quad + (i & 1);
-        if (key >= Lk || (CAUSAL && key > (hr ? qrow1 : qrow0))) s[i] = -INFINITY;
+        if (key >= Lk || (CAUSAL && key > koff + (hr ? qrow1 : qrow0))) s[i] = -INFINITY;
       }
       mx[hr] = fmaxf(mx[hr], s[i]);
     }
@@ -248,12 +281,12 @@ static int make_tmap_rows(CUtensorMap* m, const void* base, long long cols, long
   return G4R_OK;
 }
 
-template <int D, bool CAUSAL>
+template <int D, bool CAUSAL, bool CACHED = false>
 static int launch_fa(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const FaParams& p, int B,
                      cudaStream_t st) {
   constexpr int smem = (D / 64) * kAtomBytes + 4 * (D / 64) * kFaBN * 128 + 128 + 1024;  // +1024 alignment slack
   static bool set = false;
-  auto kern = fa_fwd_wgmma<D, CAUSAL>;
+  auto kern = fa_fwd_wgmma<D, CAUSAL, CACHED>;
   if (!set) {
     G4R_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     set = true;
@@ -284,7 +317,7 @@ static int attention_tc_impl(const void* q, const void* k, const void* v, void* 
   if ((rc = make_tmap_rows(&tq, q, cols, rows, ld, kFaBM))) return rc;
   if ((rc = make_tmap_rows(&tk, k, cols, rows, ld, kFaBN))) return rc;
   if ((rc = make_tmap_rows(&tv, v, cols, rows, ld, kFaBN))) return rc;
-  FaParams p{(__nv_bfloat16*)out, ldo, bso, L, H, scale, seqlens, lse};
+  FaParams p{(__nv_bfloat16*)out, ldo, bso, L, H, scale, seqlens, lse, 0, nullptr, nullptr};
   cudaStream_t st = (cudaStream_t)stream;
 #define G4R_FA(DD) (causal ? launch_fa<DD, true>(tq, tk, tv, p, B, st) : launch_fa<DD, false>(tq, tk, tv, p, B, st))
   if (head_dim == 64) return G4R_FA(64);
@@ -307,3 +340,27 @@ extern "C" int g4r_attention_tc_lse_bf16(const void* q, const void* k, const voi
   return attention_tc_impl(q, k, v, out, ld, bs, ldo, bso, B, H, L, head_dim, causal, scale, nullptr, lse, stream);
 }
 #endif
+
+// Chunk attention over the KV cache (multi-turn generation): q is the chunk's packed, RoPE-rotated [B*Lc, >= H*D] rows
+// (row stride ldq), kcache / vcache the [B, lmax, H*D] caches the chunk's own K/V were already appended to, start /
+// qlen device int32 [B] (qlen may be NULL: every row has Lc valid queries).  See the CACHED note at the top.
+extern "C" int g4r_attention_cached_bf16(const void* q, long long ldq, const void* kcache, const void* vcache, int lmax,
+                                         void* out, long long ldo, int B, int H, int Lc, int head_dim, float scale,
+                                         const int* start, const int* qlen, void* stream) {
+  G4R_REQUIRE(q && kcache && vcache && out && start && B > 0 && H > 0 && Lc > 0 && lmax > 0,
+              "attention_cached: bad arguments");
+  G4R_REQUIRE(head_dim == 64 || head_dim == 128, "attention_cached: head_dim %d (64 or 128)", head_dim);
+  G4R_REQUIRE(ldq % 8 == 0 && ldo % 8 == 0, "attention_cached: strides must keep 16-byte alignment");
+  G4R_REQUIRE((((uintptr_t)q | (uintptr_t)kcache | (uintptr_t)vcache | (uintptr_t)out) & 15) == 0,
+              "attention_cached: misaligned pointers");
+  CUtensorMap tq, tk, tv;
+  const long long cols = (long long)H * head_dim;
+  int rc;
+  if ((rc = make_tmap_rows(&tq, q, cols, (long long)B * Lc, ldq, kFaBM))) return rc;
+  if ((rc = make_tmap_rows(&tk, kcache, cols, (long long)B * lmax, cols, kFaBN))) return rc;
+  if ((rc = make_tmap_rows(&tv, vcache, cols, (long long)B * lmax, cols, kFaBN))) return rc;
+  FaParams p{(__nv_bfloat16*)out, ldo, (long long)Lc * ldo, Lc, H, scale, nullptr, nullptr, lmax, start, qlen};
+  cudaStream_t st = (cudaStream_t)stream;
+  if (head_dim == 64) return launch_fa<64, true, true>(tq, tk, tv, p, B, st);
+  return launch_fa<128, true, true>(tq, tk, tv, p, B, st);
+}

@@ -5,6 +5,8 @@
 // device->host syncs per sample in the reference become two launches per batch:
 //   splice_plan : one CTA per sample scans input_ids once, validates the reference's
 //                 span rules and writes a per-token source code (int32);
+//                 continuation mode (a chunk that continues a sequence held in the KV cache, after the image
+//                 span): no image tokens allowed, every <bbox> takes region row offs[b] + its ordinal;
 //   splice_move : pure HBM copy, one 128-bit load + store per thread per step; each row
 //                 (D 16-bit elements) comes from exactly one of {embed table, projected
 //                 image patches, region tokens}.
@@ -21,7 +23,7 @@ constexpr int kTagMask = 0x60000000;
 __global__ void __launch_bounds__(kPlanThreads)
 splice_plan(const int64_t* __restrict__ input_ids, const int32_t* __restrict__ region_offsets,
             int32_t* __restrict__ plan, int32_t* __restrict__ status, int L, int P, int V,
-            int64_t tok_patch, int64_t tok_start, int64_t tok_end, int64_t tok_bbox) {
+            int64_t tok_patch, int64_t tok_start, int64_t tok_end, int64_t tok_bbox, int continuation) {
   __shared__ int s_cnt[4];       // patch, start, end, bad-id
   __shared__ int s_start_pos;
   __shared__ int s_scan[kPlanThreads + 1];
@@ -62,19 +64,20 @@ splice_plan(const int64_t* __restrict__ input_ids, const int32_t* __restrict__ r
 
   int err = 0;
   const bool multimodal = tot_patch > 0;  // spi_llava.py:104-111: otherwise rows stay embeddings
+  const int kb = region_offsets ? region_offsets[b + 1] - region_offsets[b] : 0;
   if (s_cnt[3] > 0) err = 6;
-  else if (multimodal) {
+  else if (continuation) {
+    if (tot_patch || tot_start || tot_end) err = 7;
+    else if (total_bbox != kb) err = 3;
+  } else if (multimodal) {
     if (tot_start != tot_end) err = 1;                                  // :114-118
     else if (tot_start > 1) err = 4;
     else if (tot_start == 0) err = 5;
     else if (s + P + 1 >= L || ids[s + P + 1] != tok_end) err = 2;      // :124-128
-    else {
-      const int kb = region_offsets ? region_offsets[b + 1] - region_offsets[b] : 0;
-      if (total_bbox != kb) err = 3;                                    // :154 / :158-161
-    }
+    else if (total_bbox != kb) err = 3;                                 // :154 / :158-161
   }
   if (tid == 0) status[b] = err;
-  const bool do_splice = multimodal && err == 0;
+  const bool do_splice = (multimodal || continuation) && err == 0;
   const int kbase = (do_splice && region_offsets) ? region_offsets[b] : 0;
   int ord = s_scan[tid];
   for (int t = t0; t < t1; t++) {
@@ -185,12 +188,11 @@ extern "C" int g4r_embed_grad_rows(const void* d_out, const int32_t* order, cons
   return G4R_OK;
 }
 
-extern "C" int g4r_splice_region_tokens(const int64_t* input_ids, const void* embed_table,
-                                        const void* image_rows, const void* region_rows,
-                                        const int32_t* region_offsets, void* out, int32_t* plan,
-                                        int32_t* status, int B, int L, int P, int D, int V,
-                                        int64_t im_patch_token, int64_t im_start_token,
-                                        int64_t im_end_token, int64_t bbox_token, void* stream) {
+static int splice_impl(const int64_t* input_ids, const void* embed_table, const void* image_rows,
+                       const void* region_rows, const int32_t* region_offsets, void* out, int32_t* plan,
+                       int32_t* status, int B, int L, int P, int D, int V, int64_t im_patch_token,
+                       int64_t im_start_token, int64_t im_end_token, int64_t bbox_token, int continuation,
+                       void* stream) {
   G4R_REQUIRE(B > 0 && L > 0 && P >= 0 && D > 0 && V > 0, "bad sizes B=%d L=%d P=%d D=%d V=%d", B, L, P, D, V);
   G4R_REQUIRE(input_ids && embed_table && out && plan && status, "null argument");
   G4R_REQUIRE(D % 8 == 0, "D=%d must be a multiple of 8 (128-bit rows of 16-bit elements)", D);
@@ -202,7 +204,7 @@ extern "C" int g4r_splice_region_tokens(const int64_t* input_ids, const void* em
               "region_rows given without region_offsets");
   cudaStream_t st = (cudaStream_t)stream;
   splice_plan<<<B, kPlanThreads, 0, st>>>(input_ids, region_offsets, plan, status, L, P, V,
-                                          im_patch_token, im_start_token, im_end_token, bbox_token);
+                                          im_patch_token, im_start_token, im_end_token, bbox_token, continuation);
   G4R_LAUNCH_CHECK("splice_plan");
   const int n_rows = B * L;
   constexpr int ROWS = 4, TPR = 64;
@@ -211,4 +213,22 @@ extern "C" int g4r_splice_region_tokens(const int64_t* input_ids, const void* em
       n_rows, L, P, D / 8);
   G4R_LAUNCH_CHECK("splice_move");
   return G4R_OK;
+}
+
+extern "C" int g4r_splice_region_tokens(const int64_t* input_ids, const void* embed_table,
+                                        const void* image_rows, const void* region_rows,
+                                        const int32_t* region_offsets, void* out, int32_t* plan,
+                                        int32_t* status, int B, int L, int P, int D, int V,
+                                        int64_t im_patch_token, int64_t im_start_token,
+                                        int64_t im_end_token, int64_t bbox_token, void* stream) {
+  return splice_impl(input_ids, embed_table, image_rows, region_rows, region_offsets, out, plan, status, B, L, P, D, V,
+                     im_patch_token, im_start_token, im_end_token, bbox_token, 0, stream);
+}
+
+extern "C" int g4r_splice_continuation(const int64_t* input_ids, const void* embed_table, const void* region_rows,
+                                       const int32_t* region_offsets, void* out, int32_t* plan, int32_t* status,
+                                       int B, int L, int D, int V, int64_t im_patch_token, int64_t im_start_token,
+                                       int64_t im_end_token, int64_t bbox_token, void* stream) {
+  return splice_impl(input_ids, embed_table, nullptr, region_rows, region_offsets, out, plan, status, B, L, 0, D, V,
+                     im_patch_token, im_start_token, im_end_token, bbox_token, 1, stream);
 }

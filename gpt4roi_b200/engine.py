@@ -182,6 +182,12 @@ class PrefillEngine:
             self._rope_cache[L] = (emb.cos().to(self.dev, self.dt).contiguous(), emb.sin().to(self.dev, self.dt).contiguous())
         return self._rope_cache[L]
 
+    def _rope_span(self, n):
+        """cos/sin tables covering positions 0..n-1, for kernels that index them by position (decode steps, chunks
+        continuing a cache).  Sized to a power of two >= 1024, so a cache that grows every turn adds a table only when it
+        doubles."""
+        return self._rope(max(1024, 1 << (int(n) - 1).bit_length()))
+
     # ------------------------------------------------------------------ stages
     def vit(self, images):
         """images bf16 [B,3,S,S] -> dict{layer index: hidden state [B,P+1,C]} for the consumed layers."""
@@ -264,27 +270,37 @@ class PrefillEngine:
         t = kernels.add_bias_pos_cast(acc, self.flat_b, pos)
         return dense.linear(t, self.up_w, self.up_b)
 
-    def llama(self, embeds, B, L, last_only=False, seqlens=None, cache=None, hidden_taps=None, want='logits'):
+    def llama(self, embeds, B, L, last_only=False, seqlens=None, cache=None, hidden_taps=None, want='logits',
+              start=None):
         """hidden_taps: optional dict {n: None}; filled with a copy of the residual stream after decoder layer n
         (1-based; the parity tests record error growth with depth).  want='hidden' returns the final-norm
-        hidden states [B, L, hidden] instead of logits (LlamaModel.forward's last_hidden_state)."""
+        hidden states [B, L, hidden] instead of logits (LlamaModel.forward's last_hidden_state).
+        start: device int32 [B] -- the L rows of each sample continue the sequence held in `cache`: they sit at
+        positions start[b].. (seqlens: each sample's valid rows), are appended there and attend over the cached prefix
+        too (kernels.attention_cached; head_dim 128)."""
         c = self.cfg
         x = embeds.view(B * L, c.hidden)
-        cos, sin = self._rope(L)
+        cos, sin = self._rope(L) if start is None else self._rope_span(cache.max_len)
         scale = c.head_dim ** -0.5
         # fp32 residual stream: the first o_proj epilogue widens it (bf16 residual in, fp32 out); every branch output
         # is rounded to bf16 before the fp32 add, as a bf16 nn.Linear output added to an fp32 stream under autocast
         f32 = dict(out_dtype=torch.float32, round_branch=True) if c.llama_stream == 'fp32' else {}
         for li, w in enumerate(self.layers):
             h = kernels.rmsnorm(x, w['ln_in'], c.rms_eps)
-            if c.head_dim == 128 and (2 * c.hidden) % 256 == 0:
+            if start is not None:
+                qkv = dense.qkv_rope(h, w['wqkv'], cos, sin, L, 2 * c.hidden, pos_rows=start)
+                kernels.kv_append(qkv, cache.k[li], cache.v[li], B, L, 0, pos_rows=start)
+                a = kernels.attention_cached(qkv, cache.k[li], cache.v[li], B, c.n_heads, c.head_dim, L, scale, start,
+                                             seqlens)
+            elif c.head_dim == 128 and (2 * c.hidden) % 256 == 0:
                 qkv = dense.qkv_rope(h, w['wqkv'], cos, sin, L, 2 * c.hidden)   # RoPE fused into the GEMM epilogue
             else:
                 qkv = dense.linear(h, w['wqkv'])
                 kernels.rope_inplace(qkv, cos, sin, L, 2 * c.n_heads, c.head_dim)
-            if cache is not None:  # keep post-RoPE K and V for the decode loop
-                kernels.kv_append(qkv, cache.k[li], cache.v[li], B, L, 0)
-            a = kernels.attention(qkv, B, L, c.n_heads, c.head_dim, True, scale, seqlens=seqlens)
+            if start is None:
+                if cache is not None:  # keep post-RoPE K and V for the decode loop
+                    kernels.kv_append(qkv, cache.k[li], cache.v[li], B, L, 0)
+                a = kernels.attention(qkv, B, L, c.n_heads, c.head_dim, True, scale, seqlens=seqlens)
             x = dense.linear(a, w['wo'], residual=x, **f32)
             h = kernels.rmsnorm(x, w['ln_post'], c.rms_eps)
             f = dense.linear(h, w['wgu'], act='swiglu')
@@ -335,7 +351,7 @@ class PrefillEngine:
             embeds = splice_region_tokens(input_ids, self.embed, None, None, 0, c.im_patch_token, c.im_start_token,
                                           c.im_end_token, c.bbox_token, validate=False)
             if cache is not None:
-                cache.start(L, seqlens)
+                cache.start(L, seqlens, input_ids)
             return self.llama(embeds, B, L, last_only=last_only, seqlens=seqlens, cache=cache,
                               hidden_taps=hidden_taps, want=want)
         taps = self.vit(images)
@@ -356,7 +372,7 @@ class PrefillEngine:
             stage_taps['region'] = region[0] if (region is not None and plan['K'] > 0) else None
             stage_taps['embeds'] = embeds
         if cache is not None:
-            cache.start(L, seqlens)
+            cache.start(L, seqlens, input_ids)
         return self.llama(embeds, B, L, last_only=last_only, seqlens=seqlens, cache=cache, hidden_taps=hidden_taps,
                           want=want)
 
@@ -368,7 +384,8 @@ class PrefillEngine:
         whose rows are right-padded (the collator's pad_sequence layout, data_modules.py:33-44) or left-padded (HF's
         layout for decoder-only generation).  Left-padded rows are rotated to the right-padded layout for the run and
         the logits rotated back, so they come in the caller's layout; logits at padded positions are don't-care.
-        hidden_taps / stage_taps / the cache hold the right-padded layout."""
+        hidden_taps / stage_taps / the cache hold the right-padded layout; the cache also records the token ids, images
+        and boxes it was computed from (a later turn reuses it: generate(cache=))."""
         plan = self.plan_boxes(bboxes)
         seqlens = None
         input_ids = input_ids.to(self.dev, non_blocking=True)
@@ -380,13 +397,124 @@ class PrefillEngine:
                 input_ids = to_right_padded(input_ids, shift)
             else:
                 shift = None
-        out = self.forward_device(input_ids.contiguous(),
-                                  None if images is None else images.to(self.dev, self.dt, non_blocking=True).contiguous(),
-                                  plan, validate, last_only, seqlens, cache=cache, hidden_taps=hidden_taps, want=want,
-                                  stage_taps=stage_taps)
+        images = None if images is None else images.to(self.dev, self.dt, non_blocking=True).contiguous()
+        out = self.forward_device(input_ids.contiguous(), images, plan, validate, last_only, seqlens, cache=cache,
+                                  hidden_taps=hidden_taps, want=want, stage_taps=stage_taps)
+        if cache is not None:
+            cache.set_source(images, bboxes)
         if shift is not None and not last_only:
             out = from_right_padded(out, shift)
         return out
+
+
+    # ------------------------------------------------------------------ multi-turn generation
+    def extend(self, cache, input_ids, images, bboxes, attention_mask=None, last_only=True):
+        """Prefill a chunk that continues the sequences `cache` holds (a later turn of a conversation): input_ids int64
+        [B, Lc], right-padded (attention_mask: 0/1 [B, Lc], None: every row has Lc tokens); row b's tokens go to
+        positions cache.row_lens()[b] onwards and attend over the cached prefix.  The chunk may hold <bbox> tokens but
+        no image tokens; bboxes: per row, the boxes of the chunk's <bbox> tokens (those beyond the boxes already
+        cached), whose region tokens come from a ViT + fuse rerun on `images` (only when the chunk holds any).
+        Returns logits [B, 1, V] at each row's last chunk token (last_only=False: [B, Lc, V] at every chunk position);
+        the cache then holds prefix + chunk and records them.  It grows (zero-filled) when a row's start plus Lc exceeds
+        its length, so a CUDA graph captured on it must be rebuilt afterwards."""
+        c = self.cfg
+        if c.head_dim != 128:
+            raise NotImplementedError('continuing a cached sequence needs the fused-RoPE QKV GEMM (head_dim 128)')
+        ids = input_ids.to(self.dev).contiguous()
+        B, Lc = ids.shape
+        valid = torch.full((B,), Lc, dtype=torch.int32, device=self.dev)
+        qlen = None
+        if attention_mask is not None:
+            lens, shift = right_pad_layout(attention_mask.to(self.dev))
+            if bool(shift.any()):
+                raise NotImplementedError('extend takes right-padded chunks')
+            valid = lens.to(torch.int32).contiguous()
+            qlen = None if bool((valid == Lc).all()) else valid
+        start = cache.row_lens().clone()
+        start_h = start.cpu()
+        cache.grow(int(start_h.max()) + Lc)   # every row appends all Lc chunk rows, its padding included
+        region = None
+        plan = self.plan_boxes(bboxes)
+        if plan is not None:   # the splice checks each row's <bbox> count against its boxes (status 3)
+            if plan['K'] > 0 and bool((ids == c.bbox_token).any()):
+                images = images.to(self.dev, self.dt).contiguous()
+                maps, ss = self.fuse_maps(self.vit(images))
+                rows = self.region_tokens(maps, ss, plan['boxes'], plan['bidx'])
+            else:
+                rows = torch.zeros((1, c.hidden), dtype=self.dt, device=self.dev)
+            region = (rows, plan['offs'])
+        embeds = splice_region_tokens(ids, self.embed, None, region, 0, c.im_patch_token, c.im_start_token,
+                                      c.im_end_token, c.bbox_token, validate=True, continuation=True)
+        logits = self.llama(embeds, B, Lc, last_only=last_only, seqlens=qlen, cache=cache, start=start)
+        # what the cache now holds: the kept boxes of the prefix, then the chunk's
+        rec = cache.ids.cpu()
+        boxes = []
+        for b in range(B):
+            n_old = int((rec[b, :int(start_h[b])] == c.bbox_token).sum())
+            old = cache.boxes[b] if cache.boxes is not None and cache.boxes[b] is not None else torch.zeros(0, 4)
+            new = _row_boxes(bboxes, b)
+            new = torch.zeros(0, 4) if new is None else new.detach().to('cpu', torch.float32)
+            boxes.append(torch.cat([old[:n_old], new], 0))
+        cache.record_ids(ids, start)
+        cache.lens = (start + valid).to(torch.int32)
+        cache.length = int(cache.lens.max())
+        if images is not None:
+            cache.images = images.to(self.dev, self.dt).clone()
+        cache.boxes = boxes
+        cache.source_known = True
+        return logits
+
+    def prefill_cached(self, cache, input_ids, images, bboxes, attention_mask=None, new_tokens=0):
+        """Prefill a prompt into an existing cache that may hold an earlier turn of the conversation: the prefix it
+        already holds (KVCache.reusable) is kept and only the rest is computed (extend) when every row's reusable prefix
+        covers its image span; otherwise a full prefill overwrites the cache.  The cache first grows (zero-filled) to
+        hold the prompt plus `new_tokens`.  input_ids [B, L] (attention_mask: rows right- or left-padded).
+        Returns logits [B, 1, V] at each row's last token."""
+        c = self.cfg
+        B, L = input_ids.shape
+        if B != cache.B:
+            raise ValueError('the cache holds %d rows, the prompt has %d' % (cache.B, B))
+        ids = input_ids.to(self.dev)
+        lens = torch.full((B,), L, dtype=torch.int64, device=self.dev)
+        if attention_mask is not None:
+            lens, shift = right_pad_layout(attention_mask.to(self.dev))
+            if bool(shift.any()):
+                ids = to_right_padded(ids, shift)
+        ids = ids.contiguous()
+        cache.grow(L + new_tokens)
+        reuse = cache.reusable(input_ids, images, bboxes, attention_mask)
+        ids_h, lens_h = ids.cpu(), lens.cpu()
+        image_tok = (ids_h == c.im_patch_token) | (ids_h == c.im_start_token) | (ids_h == c.im_end_token)
+        covered = c.head_dim == 128
+        for b in range(B):
+            span = image_tok[b, :int(lens_h[b])].nonzero()
+            covered = covered and (len(span) == 0 or int(span.max()) < int(reuse[b]))
+        if not covered:
+            seqlens = None if bool((lens_h == L).all()) else lens.to(torch.int32).contiguous()
+            images = None if images is None else images.to(self.dev, self.dt).contiguous()
+            logits = self.forward_device(ids, images, self.plan_boxes(bboxes), validate=True, last_only=True,
+                                         seqlens=seqlens, cache=cache)
+            cache.set_source(images, bboxes)
+            return logits
+        tl = lens_h - reuse
+        Lc = int(tl.max())
+        tail = torch.zeros((B, Lc), dtype=torch.int64)
+        tail_boxes = []
+        for b in range(B):
+            r = int(reuse[b])
+            tail[b, :int(tl[b])] = ids_h[b, r:int(lens_h[b])]
+            n_old = int((ids_h[b, :r] == c.bbox_token).sum())
+            row = _row_boxes(bboxes, b)
+            tail_boxes.append(None if row is None else row[n_old:])
+        mask = (torch.arange(Lc)[None] < tl[:, None]).long()
+        cache.lens = reuse.to(self.dev, torch.int32)
+        cache.length = int(reuse.max())
+        return self.extend(cache, tail, images, tail_boxes, attention_mask=mask)
+
+
+def _row_boxes(bboxes, b):
+    """Row b's boxes of a per-row box list, or None (bboxes None or empty, as plan_boxes takes them: no boxes)."""
+    return None if bboxes is None or len(bboxes) == 0 else bboxes[b]
 
 
 def right_pad_layout(attention_mask):
@@ -429,20 +557,110 @@ class KVCache:
     """Per-layer K/V cache [B, Lmax, n_heads*head_dim] (the engine's 16-bit type, post-RoPE keys) for the decode loop.
     length: columns in use (padded prompt length + decode steps).  lens: None when every sample uses all `length`
     columns, else a device int32 [B] with each sample's own length (a right-padded batch of prompts of different
-    lengths): sample b's next token sits at position lens[b] and attends over columns 0..lens[b]."""
+    lengths): sample b's next token sits at position lens[b] and attends over columns 0..lens[b].
+
+    For multi-turn generation the cache also records what its K/V were computed from, so that a later turn can reuse
+    them (reusable, generate(cache=)): `ids` (int64 [B, Lmax], on the cache's device) holds the token id at every
+    position whose K/V the same write filled, -1 elsewhere; `images` the rows' images (None: text-only) and `boxes`
+    each row's boxes (host fp32 [K, 4] or None) for its <bbox> tokens.  Until a writer records the images and boxes
+    (`source_known`), nothing is reusable.
+    The K/V tensors are zero-filled, and grow() zero-fills the new space: the chunk attention (kernels.attention_cached)
+    reads cache rows past each row's valid length, up to the next multiple of 64, and needs them finite."""
 
     def __init__(self, cfg, B, max_len, device):
         hd = cfg.n_heads * cfg.head_dim
         dt = cfg.torch_dtype
-        self.k = [torch.empty((B, max_len, hd), dtype=dt, device=device) for _ in range(cfg.n_layers)]
-        self.v = [torch.empty((B, max_len, hd), dtype=dt, device=device) for _ in range(cfg.n_layers)]
+        self.cfg = cfg
+        self.k = [torch.zeros((B, max_len, hd), dtype=dt, device=device) for _ in range(cfg.n_layers)]
+        self.v = [torch.zeros((B, max_len, hd), dtype=dt, device=device) for _ in range(cfg.n_layers)]
+        self.ids = torch.full((B, max_len), -1, dtype=torch.int64, device=device)
         self.B, self.max_len, self.length = B, max_len, 0
         self.lens = None
+        self.images, self.boxes, self.source_known = None, None, False
 
-    def start(self, L, seqlens=None):
-        """A prefill of L columns fills the cache; seqlens (device int32 [B]): the valid length of each row."""
+    def start(self, L, seqlens=None, ids=None):
+        """A prefill of L columns fills the cache; seqlens (device int32 [B]): the valid length of each row; ids (int64
+        [B, L], right-padded layout): the token ids it was computed from (None: unknown, e.g. a prefill from embeddings).
+        The images and boxes are unknown until set_source."""
         self.length = L
         self.lens = None if seqlens is None else seqlens.to(torch.int32).clone()
+        self.ids.fill_(-1)
+        if ids is not None:
+            self.ids[:, :L] = ids
+        self.source_known = False
+
+    def set_source(self, images, bboxes):
+        """Record the images [B, 3, S, S] (None: text-only) and per-row box lists the cached K/V were computed from."""
+        self.images = None if images is None else images.detach().clone()
+        self.boxes = [None if _row_boxes(bboxes, b) is None else bboxes[b].detach().to('cpu', torch.float32).clone()
+                      for b in range(self.B)]
+        self.source_known = True
+
+    def row_lens(self):
+        """Each row's valid length, device int32 [B]."""
+        if self.lens is not None:
+            return self.lens
+        return torch.full((self.B,), self.length, dtype=torch.int32, device=self.ids.device)
+
+    def record_ids(self, tokens, pos):
+        """tokens int64 [B, n] whose K/V were written at positions pos[b] .. pos[b] + n - 1 (pos: int32 [B])."""
+        idx = pos.to(self.ids.device, torch.int64)[:, None] + torch.arange(tokens.shape[1], device=self.ids.device)[None]
+        self.ids.scatter_(1, idx, tokens.to(self.ids.device, torch.int64))
+
+    def grow(self, max_len):
+        """Enlarge to max_len positions, keeping the contents; the new space is zero-filled (ids: -1).  The K/V tensors
+        are replaced, so a CUDA graph captured on the old ones must be rebuilt."""
+        if max_len <= self.max_len:
+            return
+
+        def big(t, fill):
+            n = torch.full((t.shape[0], max_len) + tuple(t.shape[2:]), fill, dtype=t.dtype, device=t.device)
+            n[:, :self.max_len] = t
+            return n
+        for kv in (self.k, self.v):
+            for i in range(len(kv)):
+                kv[i] = big(kv[i], 0)
+        self.ids = big(self.ids, -1)
+        self.max_len = max_len
+
+    def _same_image(self, b, images):
+        if self.images is None or images is None:
+            return self.images is None and images is None
+        return torch.equal(self.images[b], images[b].to(self.images.device, self.images.dtype))
+
+    def reusable(self, input_ids, images, bboxes, attention_mask=None):
+        """How many leading tokens of each row of a new prompt the cache already holds, as a host int64 [B]: the longest
+        prefix of the row's tokens (unpadded: attention_mask rows right- or left-padded) equal to the recorded ids,
+        cut at the first <bbox> whose box differs from the recorded one, 0 when the row's image differs, and at most
+        len - 1 so that at least the last token is computed and gives logits."""
+        B, L = input_ids.shape
+        out = torch.zeros(B, dtype=torch.int64)
+        if B != self.B or not self.source_known:
+            return out
+        ids = input_ids.cpu()
+        if attention_mask is not None:
+            lens, shift = right_pad_layout(attention_mask.cpu())
+        else:
+            lens, shift = torch.full((B,), L, dtype=torch.int64), torch.zeros(B, dtype=torch.int64)
+        held = self.row_lens().cpu()
+        rec = self.ids.cpu()
+        for b in range(B):
+            if not self._same_image(b, images):
+                continue
+            n, s = int(lens[b]), int(shift[b])
+            row = ids[b, s:s + n]
+            m = min(n - 1, int(held[b]))
+            diff = (row[:m] != rec[b, :m]).nonzero()
+            p = int(diff[0]) if len(diff) else m
+            old = self.boxes[b]
+            new = _row_boxes(bboxes, b)
+            new = None if new is None else new.detach().to('cpu', torch.float32)
+            for k, t in enumerate((row[:p] == self.cfg.bbox_token).nonzero().flatten().tolist()):
+                if old is None or new is None or k >= old.shape[0] or k >= new.shape[0] or not torch.equal(old[k], new[k]):
+                    p = t
+                    break
+            out[b] = max(p, 0)
+        return out
 
 
 def _decode_step(self, token_ids, cache, pos_dev=None):
@@ -472,7 +690,7 @@ def _decode_step_chain(self, token_ids, cache, pos_dev):
     rows = cache.lens        # per-sample positions (<= pos): these override pos / pos_dev in every kernel
     x = splice_region_tokens(token_ids, self.embed, None, None, 0, c.im_patch_token, c.im_start_token,
                              c.im_end_token, c.bbox_token, validate=False).view(B, c.hidden)
-    cos, sin = self._rope(cache.max_len)
+    cos, sin = self._rope_span(cache.max_len)
     scale = c.head_dim ** -0.5
     fused = c.head_dim == 128 and (2 * c.hidden) % 256 == 0
     # KV-cache append folded into the q|k|v GEMM's RoPE epilogue (7 launches per layer instead of 8).  Folding the two
@@ -522,7 +740,7 @@ def _decode_step_chain(self, token_ids, cache, pos_dev):
 @torch.no_grad()
 def _generate(self, input_ids, images, bboxes, max_new_tokens=32, do_sample=False, temperature=1.0,
               stopping_criteria=None, eos_token_id=None, generator=None, use_graph=True, attention_mask=None,
-              pad_token_id=None):
+              pad_token_id=None, cache=None):
     """Prefill + greedy / temperature-sampled decode (gpt4roi/app.py:286-300 calls
     model.generate(input_ids, images=..., do_sample=True, temperature=0.2, max_new_tokens=1024,
     stopping_criteria=[...]) with the boxes bound to forward).  Returns ids [B, L + new]: the prompt as given,
@@ -531,20 +749,30 @@ def _generate(self, input_ids, images, bboxes, max_new_tokens=32, do_sample=Fals
     prefill runs on the right-padded layout and every sample continues from its own last token.
     pad_token_id (with eos_token_id): a sample that has emitted eos_token_id gets pad_token_id from then on and the
     loop ends once every sample has (transformers' GenerationMixin rule); without it the loop ends when all samples
-    emit eos_token_id at the same step."""
+    emit eos_token_id at the same step.
+    cache: a KVCache to generate into -- a conversation's earlier turns (gpt4roi/app.py re-submits the whole
+    conversation every turn): the prefix it already holds is reused and only the rest is prefilled (prefill_cached);
+    afterwards it holds the conversation including this turn's answer (the last new token excepted), ready for the next.
+    Rows that finished with pad_token_id keep those pads in the recorded ids, so the next turn's reuse stops there."""
     B, L = input_ids.shape
-    cache = KVCache(self.cfg, B, L + max_new_tokens, self.dev)
-    plan = self.plan_boxes(bboxes)
     ids = input_ids.to(self.dev)
-    run_ids, seqlens = ids, None
-    if attention_mask is not None:
-        lens, shift = right_pad_layout(attention_mask.to(self.dev))
-        if bool(shift.any()):
-            run_ids = to_right_padded(ids, shift).contiguous()
-        if not bool((lens == L).all()):
-            seqlens = lens.to(torch.int32).contiguous()
-    logits = self.forward_device(run_ids, images.to(self.dev, self.dt), plan, validate=True, last_only=True,
-                                 seqlens=seqlens, cache=cache)
+    if cache is not None:
+        logits = self.prefill_cached(cache, input_ids, images, bboxes, attention_mask, new_tokens=max_new_tokens)
+        pos0 = cache.row_lens().clone()
+    else:
+        cache = KVCache(self.cfg, B, L + max_new_tokens, self.dev)
+        plan = self.plan_boxes(bboxes)
+        run_ids, seqlens = ids, None
+        if attention_mask is not None:
+            lens, shift = right_pad_layout(attention_mask.to(self.dev))
+            if bool(shift.any()):
+                run_ids = to_right_padded(ids, shift).contiguous()
+            if not bool((lens == L).all()):
+                seqlens = lens.to(torch.int32).contiguous()
+        logits = self.forward_device(run_ids, images.to(self.dev, self.dt), plan, validate=True, last_only=True,
+                                     seqlens=seqlens, cache=cache)
+        pos0 = None
+    fed = []
     out = ids
     stepper = None
     if use_graph and max_new_tokens > 4 and self.cfg.head_dim == 128:
@@ -569,7 +797,10 @@ def _generate(self, input_ids, images, bboxes, max_new_tokens=32, do_sample=Fals
         if stopping_criteria is not None and any(bool(torch.as_tensor(sc(out, last)).all()) for sc in stopping_criteria):
             break
         if step + 1 < max_new_tokens:
+            fed.append(nxt)
             logits = stepper.step(nxt) if stepper is not None else self.decode_step(nxt, cache)
+    if pos0 is not None and fed:   # outside the decode step, so its (graphed) launch sequence is unchanged
+        cache.record_ids(torch.cat(fed, 1), pos0)
     return out
 
 

@@ -99,6 +99,20 @@ def attention(qkv, B, L, n_heads, head_dim, causal, scale, out=None, seqlens=Non
     return out
 
 
+def attention_cached(qkv, kcache, vcache, B, n_heads, head_dim, Lc, scale, start, qlen=None):
+    """Chunk attention over the KV cache: qkv packed [B*Lc, 3*HD] (RoPE-rotated at each row's positions), whose k|v were
+    already appended to caches [B, Lmax, HD] at start[b]..; start / qlen device int32 [B] (qlen None: all Lc rows valid).
+    Query i of row b attends over cache positions 0 .. start[b] + i.  Returns [B*Lc, HD]; rows >= qlen[b] hold finite
+    filler (zeros for 128-row tiles wholly past qlen[b])."""
+    act = _bf16(qkv, kcache, vcache)
+    hd = n_heads * head_dim
+    out = torch.empty((B * Lc, hd), dtype=act, device=qkv.device)
+    _call('g4r_attention_cached_bf16', qkv.device, _L.ptr(qkv), qkv.stride(0), _L.ptr(kcache), _L.ptr(vcache),
+          kcache.shape[1], _L.ptr(out), out.stride(0), B, n_heads, Lc, head_dim, float(scale),
+          _L.ptr(_pos_rows(start, B)), None if qlen is None else _L.ptr(_pos_rows(qlen, B)), act=act)
+    return out
+
+
 def patchify(images, ps, kpad):
     act = _bf16(images)
     B, _, S, _ = images.shape

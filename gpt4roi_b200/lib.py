@@ -40,6 +40,7 @@ SIGNATURES = {
     'g4r_roi_align_mlvl_forward': (_i, [_vp] * 4 + [_i] + [_vp] * 2 + [_i] * 9 + [_vp] * 3),
     'g4r_roi_align_mlvl_backward': (_i, [_vp] * 4 + [_i] + [_vp] * 2 + [_i] * 8 + [_vp]),
     'g4r_splice_region_tokens': (_i, [_vp] * 8 + [_i] * 5 + [_i64] * 4 + [_vp]),
+    'g4r_splice_continuation': (_i, [_vp] * 7 + [_i] * 4 + [_i64] * 4 + [_vp]),
     'g4r_gemm_bf16': (_i, [_vp, _ll, _vp, _ll, _vp, _ll, _i, _i, _i, _vp, _i, _vp, _ll, _i, _i, _i, _vp]),
     'g4r_gemm_bf16_ex': (_i, [_vp, _ll, _vp, _ll, _vp, _ll, _i, _i, _i, _vp, _i, _vp, _ll, _i, _i, _i, _i, _i, _vp]),
     'g4r_gemm_bf16_t': (_i, [_vp, _ll, _i, _vp, _ll, _i, _vp, _ll, _i, _i, _i, _i, _vp]),
@@ -56,6 +57,7 @@ SIGNATURES = {
     'g4r_conv_nhwc_bf16': (_i, [_vp] * 3 + [_i] * 7 + [_vp, _i, _i, _vp, _i, _vp]),
     'g4r_attention_bf16': (_i, [_vp] * 4 + [_ll] * 4 + [_i] * 5 + [_f, _vp, _vp]),
     'g4r_attention_tc_bf16': (_i, [_vp] * 4 + [_ll] * 4 + [_i] * 5 + [_f, _vp, _vp]),
+    'g4r_attention_cached_bf16': (_i, [_vp, _ll, _vp, _vp, _i, _vp, _ll, _i, _i, _i, _i, _f, _vp, _vp, _vp]),
     'g4r_layernorm_bf16': (_i, [_vp, _ll, _vp, _vp, _vp, _ll, _i, _i, _f, _vp]),
     'g4r_layernorm_ex': (_i, [_vp, _ll, _i, _vp, _vp, _vp, _ll, _i, _i, _i, _f, _vp]),
     'g4r_cast_f32_bf16': (_i, [_vp, _ll, _ll, _vp, _i, _i, _i, _vp]),
@@ -131,6 +133,7 @@ F16_TWINS = {
     'g4r_decode_gemm_rows_bf16': 'g4r_decode_gemm_rows_f16',
     'g4r_kv_append_rows_bf16': 'g4r_kv_append_rows_f16',
     'g4r_decode_attention_rows_bf16': 'g4r_decode_attention_rows_f16',
+    'g4r_attention_cached_bf16': 'g4r_attention_cached_f16',
 }
 SIGNATURES.update({twin: SIGNATURES[name] for name, twin in F16_TWINS.items()})
 

@@ -390,24 +390,35 @@ def _stack_images(images):
 
 @torch.no_grad()
 def _run_engine(eng, input_ids, images, bboxes, attention_mask, past_key_values, inputs_embeds, use_cache, want,
-                training=False, max_cache=None, last_only=False):
+                training=False, max_cache=None, last_only=False, new_prompt=False):
     """Inference dispatch shared by both model classes: prefill (ids or embeds, with or without the vision
     branch) or one decode step on our cache.  Mirrors spi_llava.py:44-48: the vision branch runs when images are
-    given and (the input is longer than one token or the module is in training mode)."""
+    given and (the input is longer than one token or the module is in training mode).
+    On a non-empty cache, an input one token longer than what the cache holds is a decode step of its last token; a
+    longer one, or any input marked as a generate call's prompt (new_prompt: HF's first iteration), is a later turn of
+    the conversation (HF's documented past_key_values reuse): the prefix the cache holds is reused and the rest
+    prefilled (PrefillEngine.prefill_cached)."""
     c = eng.cfg
     cache = _find_cache(past_key_values)
     if cache is not None and cache.kv.length > 0:
         if inputs_embeds is not None:
             raise NotImplementedError('decode steps take input_ids')
+        if want == 'hidden':
+            raise NotImplementedError('decode steps return logits (use the CausalLM wrapper)')
+        if new_prompt or input_ids.shape[1] > cache.kv.length + 1:
+            cache.stepper = None          # the cache is extended or grown: a captured step would be stale
+            budget = max_cache - input_ids.shape[1] if max_cache is not None else int(getattr(eng, 'decode_budget', 1024))
+            out = eng.prefill_cached(cache.kv, input_ids, _stack_images(images), bboxes, attention_mask,
+                                     new_tokens=max(budget, 1))
+            return out, cache
         if input_ids.shape[1] != 1:
             input_ids = input_ids[:, -1:]
         ids = input_ids.to(eng.dev).contiguous()
         if cache.stepper is None and c.head_dim == 128 and cache.kv.length + 4 < cache.kv.max_len:
             from .engine import GraphedDecode
             cache.stepper = GraphedDecode(eng, cache.kv)
+        cache.kv.record_ids(ids, cache.kv.row_lens())   # outside the (graphed) step: its launches stay unchanged
         out = cache.stepper.step(ids) if cache.stepper is not None else eng.decode_step(ids, cache.kv)
-        if want == 'hidden':
-            raise NotImplementedError('decode steps return logits (use the CausalLM wrapper)')
         return out, cache
     new_cache = None
     if use_cache:
@@ -589,7 +600,8 @@ class SPILlavaMPTForCausalLM(LlamaForCausalLM, _EngineHost):
         eng = self._get_engine(dev)
         logits, cache = _run_engine(eng, input_ids, images, bboxes, attention_mask, past_key_values, inputs_embeds,
                                     use_cache, want='logits', training=self.training,
-                                    last_only=(logits_to_keep == 1 and labels is None))
+                                    last_only=(logits_to_keep == 1 and labels is None),
+                                    new_prompt=bool(kwargs.get('is_first_iteration')))
         loss = None
         if labels is not None:  # llava.py:238-249
             shift_logits = logits[..., :-1, :].float().reshape(-1, self.config.vocab_size)
@@ -602,10 +614,16 @@ class SPILlavaMPTForCausalLM(LlamaForCausalLM, _EngineHost):
     def prepare_inputs_for_generation(self, input_ids, past_key_values=None, attention_mask=None, inputs_embeds=None,
                                       **kwargs):
         """llava/model/llava.py:263-283: after the first step only the last token is fed; `images` ride along (the
-        forward skips the vision branch for one-token inputs, spi_llava.py:47-48)."""
+        forward skips the vision branch for one-token inputs, spi_llava.py:47-48).  A generate call's prompt on a
+        non-empty cache (a later turn of a conversation, a regenerated or a shorter one) is passed whole, with its mask:
+        the forward reuses the prefix the cache holds and prefills the rest.  The prompt is HF's first iteration
+        (`is_first_iteration`); without that flag, an input longer than the cache plus one token is taken as one."""
         cache = _find_cache(past_key_values)
+        first = kwargs.get('is_first_iteration')
         if cache is not None and cache.kv.length > 0:
-            input_ids = input_ids[:, -1:]
+            decode = (input_ids.shape[1] == cache.kv.length + 1) if first is None else not first
+            if decode:
+                input_ids = input_ids[:, -1:]
         if inputs_embeds is not None and (cache is None or cache.kv.length == 0):
             model_inputs = {'inputs_embeds': inputs_embeds}
         else:
@@ -615,6 +633,8 @@ class SPILlavaMPTForCausalLM(LlamaForCausalLM, _EngineHost):
                              'logits_to_keep': 1})
         if 'bboxes' in kwargs:
             model_inputs['bboxes'] = kwargs['bboxes']
+        if first:
+            model_inputs['is_first_iteration'] = True
         return model_inputs
 
     @torch.no_grad()
@@ -642,9 +662,19 @@ class SPILlavaMPTForCausalLM(LlamaForCausalLM, _EngineHost):
             return super().generate(input_ids, images=images, bboxes=bboxes, max_new_tokens=max_new_tokens,
                                     do_sample=do_sample, use_cache=True, **kw)
         eng = self._get_engine(input_ids.device)
+        kv = None
+        pkv = kwargs.get('past_key_values')
+        if pkv is not None:   # a conversation's cache: reused and left holding this turn too
+            cache = _find_cache(pkv)
+            if cache is None:
+                cache = G4RCache(KVCache(eng.cfg, input_ids.shape[0], input_ids.shape[1] + max_new_tokens, eng.dev))
+                pkv._g4r_cache = cache      # ride on HF's Cache object, as the HF loop's prefill does
+            cache.stepper = None
+            kv = cache.kv
         return eng.generate(input_ids, images, bboxes, max_new_tokens=max_new_tokens, do_sample=do_sample,
                             temperature=temperature, stopping_criteria=stopping_criteria, eos_token_id=eos_token_id,
-                            attention_mask=kwargs.get('attention_mask'), pad_token_id=kwargs.get('pad_token_id'))
+                            attention_mask=kwargs.get('attention_mask'), pad_token_id=kwargs.get('pad_token_id'),
+                            cache=kv)
 
     def initialize_vision_tokenizer(self, mm_use_im_start_end, tokenizer, device, tune_mm_mlp_adapter=False,
                                     pretrain_mm_mlp_adapter=None):

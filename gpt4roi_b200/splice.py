@@ -19,12 +19,13 @@ _MESSAGES = {
     4: 'More than one <im_start> per sample is not supported.',
     5: '<im_patch> tokens present without <im_start>.',
     6: 'Token id out of range of the embedding table.',
+    7: 'Image tokens in a continuation chunk (the image span must lie in the cached prefix).',
 }
 
 
 def splice_region_tokens(input_ids, embed_weight, image_features, region_features, num_patches,
                          im_patch_token, im_start_token, im_end_token, bbox_token,
-                         out=None, validate=True, return_plan=False):
+                         out=None, validate=True, return_plan=False, continuation=False):
     """Build `inputs_embeds` [B,L,D].
 
     input_ids       int64 [B,L] (cuda)
@@ -32,6 +33,9 @@ def splice_region_tokens(input_ids, embed_weight, image_features, region_feature
     image_features  [B,P,D] projected patch rows (same dtype), or None when P == 0
     region_features list (len B) of [K_i,D] tensors / None entries, a packed
                     (rows [K,D], offsets int32 [B+1]) tuple, or None (bboxes=None)
+    continuation    the rows continue a sequence held in the KV cache (multi-turn generation): no image tokens may
+                    appear (ValueError), and every sample's <bbox> tokens take its region rows in order
+                    (g4r_splice_continuation); image_features must be None
     """
     B, L = input_ids.shape
     V, D = embed_weight.shape
@@ -67,10 +71,18 @@ def splice_region_tokens(input_ids, embed_weight, image_features, region_feature
     plan = torch.empty((B, L), dtype=torch.int32, device=dev)
     status = torch.empty((B,), dtype=torch.int32, device=dev)
     with torch.cuda.device(dev):
-        _L.check(_L.load().g4r_splice_region_tokens(
-            _L.ptr(input_ids), _L.ptr(embed_weight), _L.ptr(image_features), _L.ptr(rows), _L.ptr(offs),
-            _L.ptr(out), _L.ptr(plan), _L.ptr(status), B, L, P, D, V, int(im_patch_token),
-            int(im_start_token), int(im_end_token), int(bbox_token), _L.stream_ptr(dev)), launches=2)
+        if continuation:
+            if image_features is not None:
+                raise RuntimeError('a continuation chunk takes no image_features')
+            _L.check(_L.load().g4r_splice_continuation(
+                _L.ptr(input_ids), _L.ptr(embed_weight), _L.ptr(rows), _L.ptr(offs), _L.ptr(out), _L.ptr(plan),
+                _L.ptr(status), B, L, D, V, int(im_patch_token), int(im_start_token), int(im_end_token),
+                int(bbox_token), _L.stream_ptr(dev)), launches=2)
+        else:
+            _L.check(_L.load().g4r_splice_region_tokens(
+                _L.ptr(input_ids), _L.ptr(embed_weight), _L.ptr(image_features), _L.ptr(rows), _L.ptr(offs),
+                _L.ptr(out), _L.ptr(plan), _L.ptr(status), B, L, P, D, V, int(im_patch_token),
+                int(im_start_token), int(im_end_token), int(bbox_token), _L.stream_ptr(dev)), launches=2)
     if validate:
         st = status.cpu()
         bad = torch.nonzero(st)

@@ -168,6 +168,16 @@ int g4r_splice_region_tokens(const int64_t* input_ids, const void* embed_table,
                              int64_t im_patch_token, int64_t im_start_token,
                              int64_t im_end_token, int64_t bbox_token,
                              void* stream);
+/*
+ * Continuation chunk (multi-turn generation: the tokens after a prefix already held in the KV cache, past the image
+ * span; gpt4roi/app.py:110-188,242-328 re-submits the whole conversation every turn): rows come from the embedding
+ * table, and the j-th <bbox> of sample b from region_rows[region_offsets[b]+j].  status: 0, 3 (#<bbox> != K_b), 6,
+ * or 7 = an <im_patch> / <im_start> / <im_end> token in the chunk.
+ */
+int g4r_splice_continuation(const int64_t* input_ids, const void* embed_table, const void* region_rows,
+                            const int32_t* region_offsets, void* out, int32_t* plan, int32_t* status,
+                            int B, int L, int D, int V, int64_t im_patch_token, int64_t im_start_token,
+                            int64_t im_end_token, int64_t bbox_token, void* stream);
 
 /* ---- dense contractions on the wgmma tensor cores -------------------------- */
 enum { G4R_ACT_NONE = 0, G4R_ACT_RELU = 1, G4R_ACT_QUICK_GELU = 2, G4R_ACT_SWIGLU = 3 };
@@ -323,6 +333,20 @@ int g4r_attention_tc_bf16(const void* q, const void* k, const void* v, void* out
                           long long ld, long long bs, long long ldo, long long bso,
                           int B, int H, int L, int head_dim, int causal, float scale,
                           const int* seqlens, void* stream);
+
+/*
+ * Chunk attention over the KV cache (multi-turn generation: gpt4roi/app.py:110-188,242-328 appends each answer and
+ * the next question to the conversation and generates again; transformers' generate(past_key_values=...) reuses the
+ * cache of the earlier turns).  q: the chunk's packed, RoPE-rotated rows [B*Lc, >= H*head_dim] (row stride ldq);
+ * kcache / vcache: [B, lmax, H*head_dim], the chunk's own K/V already appended at positions start[b]..;
+ * start: device int32 [B], the number of cached tokens before row b's chunk; qlen: device int32 [B] valid queries of
+ * each right-padded row, or NULL (all Lc).  Query i of row b attends over cache positions 0 .. start[b] + i; output
+ * rows >= qlen[b] hold finite filler (zeros for 128-row tiles wholly past qlen[b]).  Cache rows past start[b] + qlen[b], up to the next multiple of 64, must hold finite
+ * values (the engine's cache is zero-filled).  head_dim 64 or 128; out [B*Lc, H*head_dim] with row stride ldo.
+ */
+int g4r_attention_cached_bf16(const void* q, long long ldq, const void* kcache, const void* vcache, int lmax,
+                              void* out, long long ldo, int B, int H, int Lc, int head_dim, float scale,
+                              const int* start, const int* qlen, void* stream);
 
 /* ---- HBM-bound glue (csrc/elementwise.cu); bf16 rows, fp32 math ------------- */
 /* nn.LayerNorm over the last dim (CLIP layer norms; gpt4roi/models/layers.py:263,266). */
@@ -618,6 +642,9 @@ int g4r_kv_append_rows_f16(const void* qkv, long long ld, void* kcache, void* vc
 int g4r_decode_attention_rows_f16(const void* q, long long ldq, const void* kcache, const void* vcache,
                                   void* out, long long ldo, int B, int H, int head_dim, int kv_bound,
                                   const int* pos_rows, int Lmax, float scale, void* stream);
+int g4r_attention_cached_f16(const void* q, long long ldq, const void* kcache, const void* vcache, int lmax,
+                             void* out, long long ldo, int B, int H, int Lc, int head_dim, float scale,
+                             const int* start, const int* qlen, void* stream);
 
 #ifdef __cplusplus
 }
