@@ -63,6 +63,7 @@ struct GemmParams {
   long long ldr;
   int act;
   int out_f32;   // 1: fp32 output
+  int d_vec, r_vec;  // D / residual rows take 16-byte vector accesses: 16-byte aligned base and row pitch (launch_gemm)
   // conv mode
   int conv;
   int cH, cW, cBH, cBW, tiles_x, tiles_y, cin_blocks, taps;  // taps = 9 (3x3) or 1
@@ -229,7 +230,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float* 
           __nv_bfloat162 h = __floats2bfloat162_rn(s0, s1);
           pk[j] = *reinterpret_cast<uint32_t*>(&h);
         }
-        if (full_chunk && (p.ldd % 8 == 0)) {
+        if (full_chunk && p.d_vec) {
           reinterpret_cast<uint4*>(o)[0] = make_uint4(pk[0], pk[1], pk[2], pk[3]);
           reinterpret_cast<uint4*>(o)[1] = make_uint4(pk[4], pk[5], pk[6], pk[7]);
         } else {
@@ -248,7 +249,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float* 
         // fp32 residual stream (CLIP under autocast keeps it in fp32: LayerNorm outputs fp32 and
         // `residual + bf16_branch` promotes)
         const float* rr = reinterpret_cast<const float*>(p.residual) + out_row * p.ldr + col0;
-        if (full_chunk && (p.ldr % 4 == 0)) {
+        if (full_chunk && p.r_vec) {
 #pragma unroll
           for (int h = 0; h < 8; h++) {
             const float4 r4 = reinterpret_cast<const float4*>(rr)[h];
@@ -259,7 +260,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float* 
         }
       } else {
         const __nv_bfloat16* rr = p.residual + out_row * p.ldr + col0;
-        if (full_chunk && (p.ldr % 8 == 0)) {
+        if (full_chunk && p.r_vec) {
 #pragma unroll
           for (int h = 0; h < 4; h++) {
             const uint4 raw = reinterpret_cast<const uint4*>(rr)[h];
@@ -277,7 +278,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float* 
         // split-K: split s writes slab s of a [k_splits][M][ldd] fp32 buffer (no atomics; the consumer
         // sums the slabs in a fixed order, so the result is bitwise reproducible)
         float* o = reinterpret_cast<float*>(p.D) + ((long long)split * p.M + out_row) * p.ldd + col0;
-        if (full_chunk && (p.ldd % 4 == 0)) {
+        if (full_chunk && p.d_vec) {
 #pragma unroll
           for (int h = 0; h < 8; h++)
             reinterpret_cast<float4*>(o)[h] = make_float4(f[4 * h], f[4 * h + 1], f[4 * h + 2], f[4 * h + 3]);
@@ -294,7 +295,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float* 
       }
       if (row_ok) {
         __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(p.D) + out_row * p.ldd + col0;
-        if (full_chunk && (p.ldd % 8 == 0)) {
+        if (full_chunk && p.d_vec) {
 #pragma unroll
           for (int h = 0; h < 4; h++)
             reinterpret_cast<uint4*>(o)[h] = make_uint4(pk[4 * h], pk[4 * h + 1], pk[4 * h + 2], pk[4 * h + 3]);
@@ -308,7 +309,8 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float* 
         // mmcv cnn/bricks/conv_module.py:196-208 runs GN on the conv's bf16 result).
         // 32 columns = 2 groups of 16 channels; reduce over the 32 rows of this warp, then ONE plain
         // store per (tile, warp) slot -- no atomics, so the statistics are bitwise reproducible;
-        // gn_finalize sums the slots in a fixed order.
+        // gn_finalize sums the slots in a fixed order.  Lane l stores group col0 / 16 + l when that group lies
+        // inside N: the last chunk of Cout = 16, 48, 80, ... holds one whole group.
         const __nv_bfloat16* e = reinterpret_cast<const __nv_bfloat16*>(pk);
         float s[2] = {0.f, 0.f}, ss[2] = {0.f, 0.f};
         if (row_ok) {
@@ -326,7 +328,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float* 
           ss[0] += __shfl_xor_sync(0xffffffffu, ss[0], o);
           ss[1] += __shfl_xor_sync(0xffffffffu, ss[1], o);
         }
-        if (lane < 2 && full_chunk && m_blk < p.num_m_tiles) {
+        if (lane < 2 && col0 + 16 * (lane + 1) <= p.N && m_blk < p.num_m_tiles) {
           const int tiles_per_img = p.tiles_x * p.tiles_y;
           const int slot = (m_blk % tiles_per_img) * 4 + (row >> 5);
           float* st = p.gn_stats + (((long long)img * (tiles_per_img * 4) + slot) * p.gn_groups +
@@ -555,8 +557,16 @@ static int make_tmap(CUtensorMap* m, const void* base, int rank, const cuuint64_
   return G4R_OK;
 }
 
+// A row of D / the residual may be read or written with 16-byte vectors when its base and its row pitch are both
+// multiples of 16 bytes; otherwise the epilogue takes its scalar path (e.g. a one-row output at an odd offset).
+static int vec16(const void* base, long long ld, int elem_bytes) {
+  return ((uintptr_t)base % 16 == 0) && (ld * elem_bytes % 16 == 0);
+}
+
 template <bool CONV, int TA, int TB, int BN>
-static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, cudaStream_t st) {
+static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, GemmParams p, cudaStream_t st) {
+  p.d_vec = vec16(p.D, p.ldd, p.out_f32 ? 4 : 2);
+  p.r_vec = vec16(p.residual, p.ldr, p.residual_f32 ? 4 : 2);
   static bool attr_set = false;
   auto kern = gemm_bf16_wgmma<CONV, TA, TB, BN>;
   if (!attr_set) {
@@ -649,8 +659,7 @@ extern "C" int g4r_gemm_qkv_rope_bf16(const void* A, long long lda, const void* 
                                       const void* rope_sin, int rope_cols, int L, int pos0, const int* pos0_dev,
                                       void* stream) {
   G4R_REQUIRE(rope_cos && rope_sin && L > 0, "qkv_rope: null tables");
-  G4R_REQUIRE(rope_cols % 256 == 0 && rope_cols <= N && N % 128 == 0 && ldd % 8 == 0, "qkv_rope: rope_cols must be a multiple of 256 (whole tiles of 128-dim heads)");
-  return gemm_impl(A, lda, B, ldb, D, ldd, M, N, K, nullptr, 0, nullptr, 0, 0, 0, ACT_NONE, 0, 1, rope_cos, rope_sin,
+  G4R_REQUIRE(rope_cols % 256 == 0 && rope_cols <= N && N % 128 == 0 && ldd % 8 == 0, "qkv_rope: rope_cols must be a multiple of 256 (whole tiles of 128-dim heads)");  return gemm_impl(A, lda, B, ldb, D, ldd, M, N, K, nullptr, 0, nullptr, 0, 0, 0, ACT_NONE, 0, 1, rope_cos, rope_sin,
                    rope_cols, L, stream, pos0, pos0_dev);
 }
 
@@ -661,8 +670,7 @@ extern "C" int g4r_gemm_qkv_rope_rows_bf16(const void* A, long long lda, const v
                                            const void* rope_sin, int rope_cols, int L, const int* pos_rows,
                                            void* stream) {
   G4R_REQUIRE(rope_cos && rope_sin && pos_rows && L > 0 && M % L == 0, "qkv_rope_rows: null tables / pos_rows, or M %% L != 0");
-  G4R_REQUIRE(rope_cols % 256 == 0 && rope_cols <= N && N % 128 == 0 && ldd % 8 == 0, "qkv_rope: rope_cols must be a multiple of 256 (whole tiles of 128-dim heads)");
-  return gemm_impl(A, lda, B, ldb, D, ldd, M, N, K, nullptr, 0, nullptr, 0, 0, 0, ACT_NONE, 0, 1, rope_cos, rope_sin,
+  G4R_REQUIRE(rope_cols % 256 == 0 && rope_cols <= N && N % 128 == 0 && ldd % 8 == 0, "qkv_rope: rope_cols must be a multiple of 256 (whole tiles of 128-dim heads)");  return gemm_impl(A, lda, B, ldb, D, ldd, M, N, K, nullptr, 0, nullptr, 0, 0, 0, ACT_NONE, 0, 1, rope_cos, rope_sin,
                    rope_cols, L, stream, 0, nullptr, pos_rows);
 }
 
