@@ -637,11 +637,6 @@ int gemm_skinny_dispatch(const void* A, long long lda, const void* B, long long 
                          const void* rope_cos, const void* rope_sin, int rope_cols, int rope_L, int rope_pos0,
                          const int* rope_pos_dev, const int* rope_pos_rows, void* stream);
 }
-static bool skinny_enabled() {
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("G4R_SKINNY"); v = (e && e[0] == '0') ? 0 : 1; }
-  return v == 1;
-}
 
 extern "C" int g4r_gemm_bf16_ex(const void* A, long long lda, const void* B, long long ldb, void* D,
                                 long long ldd, int M, int N, int K, const void* bias, int bias_f32,
@@ -780,7 +775,7 @@ static int gemm_impl(const void* A, long long lda, const void* B, long long ldb,
   if (act == ACT_SWIGLU) G4R_REQUIRE(N % 2 == 0 && !out_f32 && k_splits == 1 && !residual, "SwiGLU epilogue: even N, bf16 out, no split-K/residual");
   if (k_splits > 1) G4R_REQUIRE(out_f32 && act == ACT_NONE && !residual && !bias, "split-K writes fp32 partial slabs [k_splits][M][ldd]: out_f32, no bias/act/residual");
   // M <= 16 (decode step): HBM-bound weight-streaming kernel instead of a mostly empty 128-row tile
-  if (M <= 16 && !out_f32 && k_splits == 1 && !residual_f32 && !bias_round_bf16 && skinny_enabled()) {
+  if (M <= 16 && !out_f32 && k_splits == 1 && !residual_f32 && !bias_round_bf16) {
     const int rc = gemm_skinny_dispatch(A, lda, B, ldb, D, ldd, M, N, K, bias, bias_f32, residual, ldr, act, rope_cos,
                                         rope_sin, rope_cols, rope_L, rope_pos0, rope_pos_dev, rope_pos_rows, stream);
     if (rc >= 0) return rc;
@@ -867,11 +862,7 @@ extern "C" int g4r_conv_nhwc_bf16(const void* X, const void* Wt, void* Y, int n_
   p.k_splits = 1;
   p.D = Y; p.ldd = Cout; p.bias = bias; p.bias_f32 = bias_f32; p.act = act;
   p.conv = 1;
-  {
-    static int nf = -1;
-    if (nf < 0) { const char* e = getenv("G4R_CONV_NFAST"); nf = e ? atoi(e) : 1; }
-    p.n_fast = nf;
-  }
+  p.n_fast = 1;
   p.gn_stats = gn_stats; p.gn_groups = gn_groups; p.gn_group_ch = gn_groups ? Cout / gn_groups : 0;
   const int bn = pick_block_n(p.num_m_tiles, Cout, 1);
   p.num_n_tiles = (Cout + bn - 1) / bn;

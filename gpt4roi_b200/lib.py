@@ -45,12 +45,12 @@ SIGNATURES = {
     'g4r_gemm_bf16_ex': (_i, [_vp, _ll, _vp, _ll, _vp, _ll, _i, _i, _i, _vp, _i, _vp, _ll, _i, _i, _i, _i, _i, _vp]),
     'g4r_gemm_bf16_t': (_i, [_vp, _ll, _i, _vp, _ll, _i, _vp, _ll, _i, _i, _i, _i, _vp]),
     'g4r_gemm_qkv_rope_bf16': (_i, [_vp, _ll, _vp, _ll, _vp, _ll, _i, _i, _i, _vp, _vp, _i, _i, _i, _vp, _vp]),
-    'g4r_decode_gemm_bf16': (_i, [_vp, _ll, _vp, _ll, _vp, _ll, _i, _i, _i, _vp, _f, _i, _vp, _ll, _vp, _vp, _i, _i, _vp, _vp, _vp,
+    'g4r_decode_gemm_bf16': (_i, [_vp, _ll, _vp, _ll, _vp, _ll, _i, _i, _i, _i, _vp, _ll, _vp, _vp, _i, _i, _vp, _vp, _vp,
                                   _i, _i, _vp]),
     'g4r_kv_append_bf16': (_i, [_vp, _ll, _vp, _vp, _i, _i, _i, _vp, _i, _i, _vp]),
     'g4r_decode_attention_bf16': (_i, [_vp, _ll, _vp, _vp, _vp, _ll, _i, _i, _i, _i, _vp, _i, _f, _vp]),
     'g4r_gemm_qkv_rope_rows_bf16': (_i, [_vp, _ll, _vp, _ll, _vp, _ll, _i, _i, _i, _vp, _vp, _i, _i, _vp, _vp]),
-    'g4r_decode_gemm_rows_bf16': (_i, [_vp, _ll, _vp, _ll, _vp, _ll, _i, _i, _i, _vp, _f, _i, _vp, _ll, _vp, _vp, _i, _vp,
+    'g4r_decode_gemm_rows_bf16': (_i, [_vp, _ll, _vp, _ll, _vp, _ll, _i, _i, _i, _i, _vp, _ll, _vp, _vp, _i, _vp,
                                        _vp, _vp, _i, _i, _vp]),
     'g4r_kv_append_rows_bf16': (_i, [_vp, _ll, _vp, _vp, _i, _i, _vp, _i, _i, _vp]),
     'g4r_decode_attention_rows_bf16': (_i, [_vp, _ll, _vp, _vp, _vp, _ll, _i, _i, _i, _i, _vp, _i, _f, _vp]),

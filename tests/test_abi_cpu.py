@@ -13,10 +13,22 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def _declared_symbols():
+def _header_source():
     src = open(os.path.join(ROOT, 'include', 'gpt4roi_b200.h')).read()
-    src = re.sub(r'/\*.*?\*/', '', src, flags=re.S)
-    return sorted(set(re.findall(r'\b(g4r_[a-z0-9_]+)\s*\(', src)))
+    return re.sub(r'/\*.*?\*/', '', src, flags=re.S)
+
+
+def _declared_symbols():
+    return sorted(set(re.findall(r'\b(g4r_[a-z0-9_]+)\s*\(', _header_source())))
+
+
+def _declared_param_counts():
+    """name -> number of parameters of its declaration in include/gpt4roi_b200.h (`(void)` counts 0)."""
+    counts = {}
+    for name, params in re.findall(r'\b(g4r_[a-z0-9_]+)\s*\(([^()]*)\)\s*;', _header_source()):
+        params = params.strip()
+        counts[name] = 0 if params in ('', 'void') else len(params.split(','))
+    return counts
 
 
 @pytest.fixture(scope='module')
@@ -36,8 +48,13 @@ def test_header_symbols_are_exported(built_lib):
 
 def test_python_signature_table_matches_header(built_lib):
     assert sorted(built_lib.SIGNATURES) == _declared_symbols()
+    counts = _declared_param_counts()
+    assert sorted(counts) == _declared_symbols()
+    wrong = {name: (counts[name], len(args)) for name, (_, args) in built_lib.SIGNATURES.items()
+             if len(args) != counts[name]}
+    assert not wrong, 'parameter count (header, lib.SIGNATURES) differs: %s' % wrong
     lib = built_lib.load()
-    assert lib.g4r_version() >= 1000
+    assert lib.g4r_version() >= 2000
     assert lib.g4r_built_arch() == 90
 
 

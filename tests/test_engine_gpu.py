@@ -267,11 +267,9 @@ def test_graphed_decode_is_bitwise_equal_to_eager_decode():
 
 
 def test_fused_decode_step_matches_the_unfused_sequence():
-    """g4r_decode_gemm_bf16 (RMSNorm + q|k|v + RoPE + KV append in one launch; RMSNorm + gate/up + SwiGLU in one) vs the
-    8-launch sequence it replaces: same rounding points -> logits within 1e-2 rel-L2 (the norm's row sum is accumulated in
-    a different order, and the norm-fused gate/up GEMM splits K over 4 warps where the plain one uses 8: fp32 sums in a
-    different order flip last bf16 bits, 2^-8 each), KV cache rows equal to the same tolerance; batch 1, 8 and 16 (both
-    activation-block variants)."""
+    """g4r_decode_gemm_bf16 (q|k|v + RoPE + KV append in one launch; gate/up + SwiGLU in one) vs the 8-launch sequence it
+    replaces: the KV append rides in the GEMM epilogue and changes no arithmetic, so logits and KV cache rows are
+    bitwise equal; batch 1, 8 and 16 (both activation-block variants)."""
     import gpt4roi_b200.engine as E
     from gpt4roi_b200.engine import KVCache
     cfg = EngineConfig(image_size=224, vit_layers=12, n_layers=2)
@@ -283,14 +281,12 @@ def test_fused_decode_step_matches_the_unfused_sequence():
         plan = eng.plan_boxes(boxes)
         toks = torch.randint(3, 32000, (3, B, 1), generator=torch.Generator().manual_seed(B)).to(DEV)
         res = {}
-        for fused in (2, 1, 0):
+        for fused in (1, 0):
             E._DECODE_FUSED = fused
             cache = KVCache(cfg, B, ids.shape[1] + 4, DEV)
             eng.forward_device(ids.to(DEV), images, plan, last_only=True, cache=cache)
             outs = [eng.decode_step(toks[t], cache).float().clone() for t in range(3)]
             res[fused] = (torch.stack(outs), cache.k[1][:, :cache.length].float().clone(), cache.v[1][:, :cache.length].float().clone())
         E._DECODE_FUSED = 1
-        for a, b in zip(res[2], res[0]):
-            assert rel(a, b) < 1e-2, (B, rel(a, b))
         for a, b in zip(res[1], res[0]):      # KV append in the epilogue only: the very same values
             assert torch.equal(a, b), B
