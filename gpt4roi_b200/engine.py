@@ -734,14 +734,67 @@ def _decode_step_chain(self, token_ids, cache, pos_dev):
     return buf[:, None, :c.vocab]
 
 
+class Sampler:
+    """Next-token selection of the decode loop (kernels.sample_tokens): arg-max, or a draw from the temperature /
+    top-k / top-p processed softmax, with transformers' eos -> pad rule when eos_id and pad_id are both given.
+    Its per-step state lives on the device, so a CUDA graph can capture the call: `rng_step` (int64 [1], the Philox
+    counter, advanced once per selected token) and `finished` (int32 [B], the rows that have emitted eos_id)."""
+
+    def __init__(self, B, device, greedy=True, temperature=1.0, top_k=None, top_p=None, seed=0, eos_id=None,
+                 pad_id=None):
+        self.greedy = bool(greedy)
+        self.temperature = float(temperature)
+        self.top_k = 0 if top_k is None else int(top_k)
+        self.top_p = 1.0 if top_p is None else float(top_p)
+        self.seed = int(seed)
+        rule = eos_id is not None and pad_id is not None
+        self.eos_id, self.pad_id = (int(eos_id), int(pad_id)) if rule else (-1, -1)
+        self.rng_step = torch.zeros(1, dtype=torch.int64, device=device)
+        self.finished = torch.zeros(B, dtype=torch.int32, device=device)
+
+    def __call__(self, logits, out, update=True):
+        """Select from logits [B, 1, V] into out (int64 [B, 1]).  update=False leaves `finished` alone (warm-up)."""
+        if not logits.is_cuda:
+            return self._host(logits, out, update)
+        return kernels.sample_tokens(logits, out, self.greedy, self.temperature, self.top_k, self.top_p, self.seed,
+                                     self.rng_step, self.eos_id, self.pad_id, self.finished if update else None)
+
+    def _host(self, logits, out, update):
+        """Host tensors come only from CPU stand-ins of the engine (the loop's host-side tests): the arg-max and the
+        eos -> pad rule, restated.  Sampling exists on the device only."""
+        if not self.greedy:
+            raise RuntimeError('token sampling runs on the CUDA device only (csrc/sample.cu): logits are on %s'
+                               % logits.device)
+        tok = logits.reshape(logits.shape[0], -1).argmax(-1)
+        if update and self.eos_id >= 0:
+            tok = torch.where(self.finished.bool(), torch.full_like(tok, self.pad_id), tok)
+            self.finished |= (tok == self.eos_id).to(torch.int32)
+        out.copy_(tok.view(out.shape))
+        return out
+
+    def advance(self):
+        self.rng_step.add_(1)
+
+
+def sampling_seed(generator=None):
+    """The Philox key of one generate call, drawn from `generator` (default: torch's default CPU generator), so that
+    torch.manual_seed makes sampling reproducible."""
+    dev = generator.device if generator is not None else 'cpu'
+    return int(torch.randint(0, 2 ** 62, (1,), generator=generator, device=dev).item())
+
+
 @torch.no_grad()
 def _generate(self, input_ids, images, bboxes, max_new_tokens=32, do_sample=False, temperature=1.0,
               stopping_criteria=None, eos_token_id=None, generator=None, use_graph=True, attention_mask=None,
-              pad_token_id=None, cache=None):
-    """Prefill + greedy / temperature-sampled decode (gpt4roi/app.py:286-300 calls
+              pad_token_id=None, cache=None, top_k=None, top_p=None):
+    """Prefill + greedy / sampled decode (gpt4roi/app.py:286-300 calls
     model.generate(input_ids, images=..., do_sample=True, temperature=0.2, max_new_tokens=1024,
     stopping_criteria=[...]) with the boxes bound to forward).  Returns ids [B, L + new]: the prompt as given,
     then the new tokens (HF's layout).
+    do_sample with temperature > 0: every token is drawn on the device (Sampler) from softmax(logits / temperature),
+    restricted to the top_k largest values (None / 0: all) and then to the top_p nucleus (None / 1: all), as
+    transformers' TemperatureLogitsWarper -> TopKLogitsWarper -> TopPLogitsWarper; the draws are keyed by a seed taken
+    from `generator` (default: torch's default generator).  Otherwise the arg-max.
     attention_mask: 0/1 [B, L] for a batch of prompts of different lengths, each row right- or left-padded; the
     prefill runs on the right-padded layout and every sample continues from its own last token.
     pad_token_id (with eos_token_id): a sample that has emitted eos_token_id gets pad_token_id from then on and the
@@ -769,45 +822,53 @@ def _generate(self, input_ids, images, bboxes, max_new_tokens=32, do_sample=Fals
         logits = self.forward_device(run_ids, images.to(self.dev, self.dt), plan, validate=True, last_only=True,
                                      seqlens=seqlens, cache=cache)
         pos0 = None
-    fed = []
-    out = ids
+    greedy = not (do_sample and temperature > 0)
+    rule = pad_token_id is not None and eos_token_id is not None
+    sampler = Sampler(B, self.dev, greedy, temperature, top_k, top_p, seed=0 if greedy else sampling_seed(generator),
+                      eos_id=eos_token_id, pad_id=pad_token_id)
+    out = torch.empty((B, L + max_new_tokens), dtype=torch.int64, device=self.dev)
+    out[:, :L] = ids
     stepper = None
     if use_graph and max_new_tokens > 4 and self.cfg.head_dim == 128:
-        stepper = GraphedDecode(self, cache)
-    finished = None
+        stepper = GraphedDecode(self, cache, sampler=sampler)   # each replay also selects the next token into its ids
+    tok = stepper.ids if stepper is not None else torch.empty((B, 1), dtype=torch.int64, device=self.dev)
+    sampler(logits, tok)              # the first new token, from the prefill logits
+    sampler.advance()
+    n = 0
     for step in range(max_new_tokens):
-        last = logits[:, -1].float()
-        if do_sample and temperature > 0:
-            nxt = torch.multinomial(torch.softmax(last / temperature, -1), 1, generator=generator)
-        else:
-            nxt = last.argmax(-1, keepdim=True)
-        if pad_token_id is not None and eos_token_id is not None:
-            if finished is not None:
-                nxt = torch.where(finished, torch.full_like(nxt, pad_token_id), nxt)
-            finished = (nxt == eos_token_id) if finished is None else finished | (nxt == eos_token_id)
-        out = torch.cat([out, nxt], 1)
-        if finished is not None:
-            if bool(finished.all()):
+        out[:, L + step:L + step + 1].copy_(tok)
+        n = step + 1
+        if rule:
+            if bool(sampler.finished.all()):
                 break
-        elif eos_token_id is not None and bool((nxt == eos_token_id).all()):
+        elif eos_token_id is not None and bool((tok == eos_token_id).all()):
             break
-        if stopping_criteria is not None and any(bool(torch.as_tensor(sc(out, last)).all()) for sc in stopping_criteria):
+        if stopping_criteria is not None and any(bool(torch.as_tensor(sc(out[:, :L + n], logits[:, -1].float())).all())
+                                                 for sc in stopping_criteria):
             break
         if step + 1 < max_new_tokens:
-            fed.append(nxt)
-            logits = stepper.step(nxt) if stepper is not None else self.decode_step(nxt, cache)
-    if pos0 is not None and fed:   # outside the decode step, so its (graphed) launch sequence is unchanged
-        cache.record_ids(torch.cat(fed, 1), pos0)
+            if stepper is not None:
+                logits = stepper.step()
+            else:
+                logits = self.decode_step(tok, cache)
+                sampler(logits, tok)
+                sampler.advance()
+    out = out[:, :L + n]
+    if pos0 is not None and n > 1:   # outside the decode step, so its (graphed) launch sequence is unchanged
+        cache.record_ids(out[:, L:L + n - 1], pos0)
     return out
 
 
 class GraphedDecode:
     """CUDA-graph replay of one decode step: ~260 launches become one.  The current length lives in a
     device int32 that the QKV-RoPE epilogue, kv_append and decode_attention read; `step` bumps it (and the
-    per-sample lengths cache.lens of a batch of prompts of different lengths, which those kernels then read instead)."""
+    per-sample lengths cache.lens of a batch of prompts of different lengths, which those kernels then read instead).
+    sampler (a Sampler): the captured step ends with it selecting the next token from the step's logits into `ids`,
+    the graph's own input, so the host copies no token in: write the first token into `ids`, then call step() with no
+    argument, once per token; step() also advances the sampler's Philox counter."""
 
-    def __init__(self, engine, cache):
-        self.eng, self.cache = engine, cache
+    def __init__(self, engine, cache, sampler=None):
+        self.eng, self.cache, self.sampler = engine, cache, sampler
         dev = engine.dev
         self.ids = torch.zeros((cache.B, 1), dtype=torch.int64, device=dev)
         self.pos = torch.tensor([cache.length], dtype=torch.int32, device=dev)
@@ -816,24 +877,32 @@ class GraphedDecode:
         side.wait_stream(torch.cuda.current_stream(dev))
         with torch.cuda.stream(side):
             for _ in range(2):  # warm-up (writes slot `start`, overwritten by the first real step)
-                engine.decode_step(self.ids, cache, self.pos)
+                logits = engine.decode_step(self.ids, cache, self.pos)
                 cache.length = start
+            if sampler is not None:   # into a scratch buffer, `finished` untouched
+                sampler(logits, torch.empty_like(self.ids), update=False)
         torch.cuda.current_stream(dev).wait_stream(side)
         torch.cuda.synchronize(dev)
         self.graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(self.graph):
             self.logits = engine.decode_step(self.ids, cache, self.pos)
+            if sampler is not None:
+                sampler(self.logits, self.ids)
         cache.length = start
 
-    def step(self, token_ids):
+    def step(self, token_ids=None):
+        """token_ids: int64 [B, 1], the tokens to feed (without a sampler); with one, None: the graph feeds itself."""
         if self.cache.length + 1 > self.cache.max_len:
             raise RuntimeError('KV cache is full (%d)' % self.cache.max_len)
-        self.ids.copy_(token_ids, non_blocking=True)
+        if token_ids is not None:
+            self.ids.copy_(token_ids, non_blocking=True)
         self.graph.replay()
         self.pos.add_(1)
         if self.cache.lens is not None:   # per-sample positions: the graph reads this very tensor
             self.cache.lens.add_(1)
         self.cache.length += 1
+        if self.sampler is not None:
+            self.sampler.advance()
         return self.logits
 
 

@@ -204,6 +204,31 @@ def add_bias_pos_cast(acc, bias, pos):
     return out
 
 
+def sample_tokens(logits, out, greedy, temperature=1.0, top_k=0, top_p=1.0, seed=0, rng_step=None, eos_id=-1,
+                  pad_id=-1, finished=None):
+    """Next token of every row of 16-bit logits [B, V] (or [B, 1, V]; unit column stride) into out (int64, B contiguous
+    elements, e.g. the [B, 1] ids buffer of a decode step): the arg-max (greedy), or a draw from the temperature /
+    top-k / top-p processed softmax with Philox key `seed` and counter (*rng_step, row) -- rng_step: device int64 [1].
+    top_k 0 / top_p 1 switch that filter off.  finished (device int32 [B]) with eos_id, pad_id >= 0: transformers'
+    eos -> pad rule, updated in place."""
+    rows = logits.reshape(logits.shape[0], logits.shape[-1]) if logits.dim() == 3 else logits
+    act = _bf16(rows)
+    B, V = rows.shape
+    if rows.stride(1) != 1:
+        raise RuntimeError('sample_tokens: logits rows must have unit column stride')
+    if out.dtype != torch.int64 or out.numel() != B or not out.is_contiguous():
+        raise RuntimeError('sample_tokens: out must be a contiguous int64 tensor of %d elements' % B)
+    if rng_step is not None and (rng_step.dtype != torch.int64 or rng_step.numel() != 1):
+        raise RuntimeError('sample_tokens: rng_step must be a device int64 [1] counter')
+    if finished is not None and (finished.dtype != torch.int32 or finished.numel() != B or not finished.is_contiguous()):
+        raise RuntimeError('sample_tokens: finished must be a contiguous device int32 [%d] vector' % B)
+    _L.require_cuda_same_device([('logits', rows), ('out', out), ('rng_step', rng_step), ('finished', finished)])
+    _call('g4r_sample_tokens_bf16', rows.device, _L.ptr(rows), rows.stride(0), B, V, float(temperature), int(top_k),
+          float(top_p), int(bool(greedy)), int(seed) & 0xFFFFFFFFFFFFFFFF, _L.ptr(rng_step), int(eos_id), int(pad_id),
+          _L.ptr(finished), _L.ptr(out), act=act)
+    return out
+
+
 def _pos_rows(pos_rows, B):
     if pos_rows.dtype != torch.int32 or tuple(pos_rows.shape) != (B,) or not pos_rows.is_contiguous():
         raise RuntimeError('pos_rows must be a contiguous device int32 [%d] vector' % B)

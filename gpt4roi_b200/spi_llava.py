@@ -476,6 +476,40 @@ class _TrainStepFn(torch.autograd.Function):
         return (None,) * 6 + out
 
 
+def resolve_sampling(model, input_len, do_sample=None, temperature=None, **kwargs):
+    """The engine loop's selection rule for a generate call, resolved as transformers resolves it: explicit kwargs, then
+    `generation_config=`, then model.generation_config, then HF's global defaults (GenerationMixin.
+    _prepare_generation_config; `do_sample=True` alone therefore samples with top_k=50).  Returns (do_sample,
+    temperature, top_k, top_p) with top_k 0 / top_p 1 meaning off.  A call whose resolved config would make HF apply
+    any logits processor beyond TemperatureLogitsWarper, TopKLogitsWarper and TopPLogitsWarper (repetition_penalty,
+    min_p, typical_p, no_repeat_ngram_size, a caller's logits_processor, ...), or run beam search, raises
+    NotImplementedError: the engine loop does not implement it, the HF loop (use_hf_loop=True) does."""
+    from transformers.generation.logits_process import TemperatureLogitsWarper, TopKLogitsWarper, TopPLogitsWarper
+    from transformers.utils import logging as hf_logging
+    given = {k: v for k, v in dict(kwargs, do_sample=do_sample, temperature=temperature).items() if v is not None}
+    verbosity = hf_logging.get_verbosity()
+    hf_logging.set_verbosity_error()     # HF's notes on flags and pad tokens belong to its own loop
+    try:
+        gc, _ = model._prepare_generation_config(given.pop('generation_config', None), **given)
+        model._prepare_special_tokens(gc, True, 'cpu')
+    finally:
+        hf_logging.set_verbosity(verbosity)
+    if (gc.num_beams or 1) > 1:
+        raise NotImplementedError('beam search (num_beams=%d) runs on the HF loop only: pass use_hf_loop=True'
+                                  % gc.num_beams)
+    procs = model._get_logits_processor(gc, input_ids_seq_length=input_len, device='cpu', model_kwargs={},
+                                        logits_processor=kwargs.get('logits_processor'))
+    other = [type(p).__name__ for p in procs
+             if not isinstance(p, (TemperatureLogitsWarper, TopKLogitsWarper, TopPLogitsWarper))]
+    if other:
+        raise NotImplementedError('the engine loop applies temperature, top_k and top_p only; %s run on the HF loop: '
+                                  'pass use_hf_loop=True' % ', '.join(other))
+    if not gc.do_sample:
+        return False, 1.0, 0, 1.0
+    return (True, float(gc.temperature if gc.temperature is not None else 1.0), int(gc.top_k or 0),
+            float(gc.top_p if gc.top_p is not None else 1.0))
+
+
 class SPILlavaMPTForCausalLM(LlamaForCausalLM, _EngineHost):
     """Drop-in for gpt4roi.models.spi_llava.SPILlavaMPTForCausalLM (spi_llava.py:215-306)."""
     config_class = LlavaConfig
@@ -638,15 +672,19 @@ class SPILlavaMPTForCausalLM(LlamaForCausalLM, _EngineHost):
         return model_inputs
 
     @torch.no_grad()
-    def generate(self, input_ids=None, images=None, bboxes=None, max_new_tokens=32, do_sample=False,
-                 temperature=1.0, stopping_criteria=None, eos_token_id=None, use_hf_loop=False, **kwargs):
+    def generate(self, input_ids=None, images=None, bboxes=None, max_new_tokens=32, do_sample=None,
+                 temperature=None, stopping_criteria=None, eos_token_id=None, use_hf_loop=False, **kwargs):
         """Region-token prefill + KV-cache decode on the sm_90a engine.  Accepts the arguments the demo
         passes (gpt4roi/app.py:293-300); boxes may be given here or bound the way app.py does
         (`self.forward = partial(self.forward, bboxes=...)`, :286-291).  Returns ids [B, L+new] like HF.
         use_hf_loop=True runs transformers' own GenerationMixin.generate over this model's forward /
         prepare_inputs_for_generation / past_key_values instead of the engine's loop.
         attention_mask (right- or left-padded) and pad_token_id reach either loop: prompts of different lengths in one
-        batch each continue from their own last token, and finished rows are filled with pad_token_id."""
+        batch each continue from their own last token, and finished rows are filled with pad_token_id.
+        Sampling on the engine loop follows HF's resolution of do_sample / temperature / top_k / top_p /
+        generation_config (resolve_sampling: the demo's call samples from the top 50 at T = 0.2, as on the HF loop);
+        the draws are keyed by torch's default generator (or `generator=`), so torch.manual_seed makes them
+        reproducible.  Other logits processors and beam search raise NotImplementedError there."""
         if bboxes is None:
             bboxes = getattr(getattr(self, 'forward', None), 'keywords', {}).get('bboxes')
         if use_hf_loop:
@@ -657,10 +695,13 @@ class SPILlavaMPTForCausalLM(LlamaForCausalLM, _EngineHost):
                 kw['stopping_criteria'] = stopping_criteria
             if eos_token_id is not None:
                 kw['eos_token_id'] = eos_token_id
-            if do_sample:
+            if do_sample and temperature is not None:
                 kw['temperature'] = temperature
             return super().generate(input_ids, images=images, bboxes=bboxes, max_new_tokens=max_new_tokens,
-                                    do_sample=do_sample, use_cache=True, **kw)
+                                    do_sample=bool(do_sample), use_cache=True, **kw)
+        gen = {k: v for k, v in kwargs.items() if k not in ('attention_mask', 'pad_token_id', 'past_key_values',
+                                                             'generator')}
+        do_sample, temperature, top_k, top_p = resolve_sampling(self, input_ids.shape[1], do_sample, temperature, **gen)
         eng = self._get_engine(input_ids.device)
         kv = None
         pkv = kwargs.get('past_key_values')
@@ -672,9 +713,9 @@ class SPILlavaMPTForCausalLM(LlamaForCausalLM, _EngineHost):
             cache.stepper = None
             kv = cache.kv
         return eng.generate(input_ids, images, bboxes, max_new_tokens=max_new_tokens, do_sample=do_sample,
-                            temperature=temperature, stopping_criteria=stopping_criteria, eos_token_id=eos_token_id,
-                            attention_mask=kwargs.get('attention_mask'), pad_token_id=kwargs.get('pad_token_id'),
-                            cache=kv)
+                            temperature=temperature, top_k=top_k, top_p=top_p, stopping_criteria=stopping_criteria,
+                            eos_token_id=eos_token_id, attention_mask=kwargs.get('attention_mask'),
+                            pad_token_id=kwargs.get('pad_token_id'), cache=kv, generator=kwargs.get('generator'))
 
     def initialize_vision_tokenizer(self, mm_use_im_start_end, tokenizer, device, tune_mm_mlp_adapter=False,
                                     pretrain_mm_mlp_adapter=None):

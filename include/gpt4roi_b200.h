@@ -286,6 +286,26 @@ int g4r_decode_attention_rows_bf16(const void* q, long long ldq, const void* kca
                                    void* out, long long ldo, int B, int H, int head_dim, int kv_bound,
                                    const int* pos_rows, int Lmax, float scale, void* stream);
 
+/* ---- next-token selection (the decode loop's last kernel) ------------------------------------
+ * logits: 16-bit [B, V] rows, row pitch ld elements.  Writes out_ids[b] (int64, like the decode step's ids buffer).
+ * greedy != 0: the arg-max of each row, first index among equal values -- replaces the `argmax` of transformers'
+ *   GenerationMixin._sample (and torch.argmax in general; NaN counts as the largest value).
+ * greedy == 0: a draw from the processed softmax, in transformers' order (logits_process.py), on the logits widened to
+ *   fp32 as HF's `.float()` does: TemperatureLogitsWarper (s = x / temperature, a division), then TopKLogitsWarper when
+ *   0 < top_k < V (keep s >= the k-th largest s, duplicates counted), then TopPLogitsWarper when top_p < 1
+ *   (min_tokens_to_keep = 1; keep each value whose strictly larger survivors hold less than top_p of the survivors'
+ *   softmax mass -- a group of equal values at the boundary is kept whole, where HF's unstable sort may split it),
+ *   then the softmax + multinomial of GenerationMixin._sample, by inverse CDF over (value descending, index ascending).
+ *   The uniform is Philox4x32-10 with key = seed and counter = (*rng_step, b, 0): (word0 >> 8) * 2^-24.  The result
+ *   is a function of the logits, seed and *rng_step alone (no float atomics), so a CUDA graph that captured this call
+ *   draws afresh on every replay once the caller advances *rng_step.  Needs V < 65536.
+ * eos_id >= 0 and pad_id >= 0 and finished (device int32 [B]) non-NULL: transformers' eos -> pad rule -- a row with
+ *   finished[b] set gets pad_id, a row that emits eos_id sets finished[b].
+ * Capturable: every per-step value is read from device memory. */
+int g4r_sample_tokens_bf16(const void* logits, long long ld, int B, int V, float temperature, int top_k, float top_p,
+                           int greedy, unsigned long long seed, const long long* rng_step, int eos_id, int pad_id,
+                           int* finished, long long* out_ids, void* stream);
+
 /*
  * NHWC convolution as an implicit GEMM (stride 1, pad (ksize-1)/2, ksize 1 or 3):
  *   Y[n,y,x,co] = act( sum_{ky,kx,ci} X[n,y+ky-1,x+kx-1,ci] * Wt[co,(ky*ks+kx)*Cin+ci] + bias[co] )
@@ -643,6 +663,9 @@ int g4r_decode_attention_rows_f16(const void* q, long long ldq, const void* kcac
 int g4r_attention_cached_f16(const void* q, long long ldq, const void* kcache, const void* vcache, int lmax,
                              void* out, long long ldo, int B, int H, int Lc, int head_dim, float scale,
                              const int* start, const int* qlen, void* stream);
+int g4r_sample_tokens_f16(const void* logits, long long ld, int B, int V, float temperature, int top_k, float top_p,
+                          int greedy, unsigned long long seed, const long long* rng_step, int eos_id, int pad_id,
+                          int* finished, long long* out_ids, void* stream);
 
 #ifdef __cplusplus
 }
