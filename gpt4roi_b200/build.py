@@ -24,7 +24,7 @@ EXTRA = {
 # The inference kernels are built twice: bf16 as written, and an fp16 twin (-DG4R_ACT_HALF, csrc/act_type.cuh) for the
 # demo's dtype (gpt4roi/app.py:74-98: model.half()).  Both land in the one shared library.
 FP16_TWINS = ('gemm_wgmma.cu', 'attention_wgmma.cu', 'attention.cu', 'elementwise.cu', 'gemm_skinny.cu', 'decode.cu',
-              'sample.cu')
+              'sample.cu', 'beam.cu')
 
 
 def nvcc():

@@ -1,9 +1,10 @@
 // act_type.cuh -- the 16-bit activation / weight type of the inference kernels.
 //
 // The demo serves the model in fp16 (gpt4roi/app.py:74-98,271: `model.half()`, `images.half()`, `bboxes.half()`), the
-// training scripts and everything else in bf16 (train_stage*.sh --bf16 True).  The seven inference sources
-// (gemm_wgmma.cu, attention_wgmma.cu, attention.cu, elementwise.cu, gemm_skinny.cu, decode.cu, sample.cu) are therefore built
-// twice: as written (bf16), and with -DG4R_ACT_HALF, where this header -- included AFTER common.cuh / ptx.cuh --
+// training scripts and everything else in bf16 (train_stage*.sh --bf16 True).  The eight inference sources
+// (gemm_wgmma.cu, attention_wgmma.cu, attention.cu, elementwise.cu, gemm_skinny.cu, decode.cu, sample.cu, beam.cu) are
+// therefore built twice: as written (bf16), and with -DG4R_ACT_HALF, where this header -- included AFTER common.cuh /
+// ptx.cuh --
 // retargets the type, its conversion intrinsics, the tensor-core operand format and the exported names to fp16:
 //   * every kernel keeps fp32 accumulation and the same rounding points ("round to the storage type" is now fp16);
 //   * wgmma and mma.sync switch their .bf16 operand qualifier to .f16 (G4R_ACT_PTX); TMA tensor maps carry the
@@ -57,6 +58,8 @@
 #define g4r_decode_attention_rows_bf16 g4r_decode_attention_rows_f16
 #define g4r_attention_cached_bf16 g4r_attention_cached_f16
 #define g4r_sample_tokens_bf16 g4r_sample_tokens_f16
+#define g4r_decode_attention_beam_bf16 g4r_decode_attention_beam_f16
+#define g4r_beam_step_bf16 g4r_beam_step_f16
 
 #else
 #define G4R_NS g4r

@@ -44,11 +44,15 @@ kv_append_bf16(const __nv_bfloat16* __restrict__ qkv, long long ld, __nv_bfloat1
 // still come from the host's bound kv_len (>= every row's length); each row slices its own keys into S parts, so a CTA
 // of a short row may own no key at all -- it still joins every cluster barrier and contributes -inf to the max and 0 to
 // the sum and to the output.  All rows equal: the slicing, and so the result, is the scalar kernel's.
-template <int D>
+// BEAM (beam search, pos_rows given): the caches are shared by every row, and key / value p of row b is read from cache
+// row anc[b, p] (anc: int32 [rows, Lmax]) instead of row b.  A half-warp still loads one 256-byte row per key; the
+// 16 lanes read the same anc entry.  Without BEAM `anc` is unused and the code is the non-beam kernel's.
+template <int D, bool BEAM = false>
 __global__ void __launch_bounds__(256)
 decode_attention_bf16(const __nv_bfloat16* q, long long ldq, const __nv_bfloat16* kc, const __nv_bfloat16* vc,
                       __nv_bfloat16* out, long long ldo, int H, int kv_len, const int* __restrict__ pos_dev,
-                      const int* __restrict__ pos_rows, int Lmax, float scale, int per_max) {
+                      const int* __restrict__ pos_rows, int Lmax, float scale, int per_max,
+                      const int* __restrict__ anc) {
   // Programmatic dependent launch (common.cuh): q and the newest K/V row come from the q|k|v GEMM that precedes this
   // kernel in the decode step, so there is nothing to fetch ahead; the launch itself and the prologue overlap its tail.
   // q / kc / vc carry no __restrict__: their loads must stay on the coherent path.
@@ -87,14 +91,21 @@ decode_attention_bf16(const __nv_bfloat16* q, long long ldq, const __nv_bfloat16
     }
   }
   // ---- phase 1: scores of the slice
-  const __nv_bfloat16* kb = kc + ((long long)b * Lmax + k0) * HD + (long long)h * D + sub * 8;
+  // row offset of local key `key` (BEAM: the cache row its ancestry table names)
+  const long long kv0 = BEAM ? (long long)k0 * HD : ((long long)b * Lmax + k0) * HD;
+  const int* arow = BEAM ? anc + (long long)b * Lmax + k0 : nullptr;
+  auto key_off = [&](int key) -> long long {
+    if constexpr (BEAM) return ((long long)arow[key] * Lmax + key) * HD;
+    else return (long long)key * HD;
+  };
+  const __nv_bfloat16* kb = kc + kv0 + (long long)h * D + sub * 8;
   float mx = -INFINITY;
   for (int base = 0; base < n_loc; base += GROUPS * 4) {
     uint4 raw[4];
 #pragma unroll
     for (int u = 0; u < 4; u++) {
       const int key = base + u * GROUPS + grp;
-      raw[u] = key < n_loc ? *reinterpret_cast<const uint4*>(kb + (long long)key * HD) : make_uint4(0, 0, 0, 0);
+      raw[u] = key < n_loc ? *reinterpret_cast<const uint4*>(kb + key_off(key)) : make_uint4(0, 0, 0, 0);
     }
 #pragma unroll
     for (int u = 0; u < 4; u++) {
@@ -148,7 +159,7 @@ decode_attention_bf16(const __nv_bfloat16* q, long long ldq, const __nv_bfloat16
   for (int r = 0; r < S; r++) gsum += *cluster.map_shared_rank(&cl_sum, r);
   const float inv = 1.f / gsum;
   // ---- phase 2: partial P.V of the slice (probabilities rounded to bf16 like P.to(q.dtype))
-  const __nv_bfloat16* vb = vc + ((long long)b * Lmax + k0) * HD + (long long)h * D + sub * 8;
+  const __nv_bfloat16* vb = vc + kv0 + (long long)h * D + sub * 8;
   float o8[8];
 #pragma unroll
   for (int j = 0; j < 8; j++) o8[j] = 0.f;
@@ -159,7 +170,7 @@ decode_attention_bf16(const __nv_bfloat16* q, long long ldq, const __nv_bfloat16
     for (int u = 0; u < 4; u++) {
       const int key = base + u * GROUPS + grp;
       const bool ok = key < n_loc;
-      raw[u] = ok ? *reinterpret_cast<const uint4*>(vb + (long long)key * HD) : make_uint4(0, 0, 0, 0);
+      raw[u] = ok ? *reinterpret_cast<const uint4*>(vb + key_off(key)) : make_uint4(0, 0, 0, 0);
       pk[u] = ok ? __bfloat162float(__float2bfloat16_rn(sc[key] * inv)) : 0.f;
     }
 #pragma unroll
@@ -222,10 +233,10 @@ extern "C" int g4r_kv_append_rows_bf16(const void* qkv, long long ld, void* kcac
   return launch_kv_append(qkv, ld, kcache, vcache, B, Ln, 0, nullptr, pos_rows, Lmax, HD, (cudaStream_t)stream);
 }
 
-template <int D>
+template <int D, bool BEAM>
 static int launch_decode_attention(const void* q, long long ldq, const void* kcache, const void* vcache, void* out,
                                    long long ldo, int B, int H, int kv_len, const int* pos_dev, const int* pos_rows,
-                                   int Lmax, float scale, cudaStream_t st) {
+                                   const int* anc, int Lmax, float scale, cudaStream_t st) {
   // split-KV factor: enough CTAs for >= 2 per SM, slices of >= 64 keys, cluster size <= 8 (portable)
   int S = 1;
   while (S < 8 && H * B * S < 2 * num_sms() && kv_len / (2 * S) >= 64) S *= 2;
@@ -235,37 +246,55 @@ static int launch_decode_attention(const void* q, long long ldq, const void* kca
   G4R_REQUIRE(smem <= 200 * 1024, "decode_attention: kv_len %d too long for the shared-memory score buffer", kv_len);
   static bool set = false;
   if (!set) {
-    G4R_CUDA(cudaFuncSetAttribute(decode_attention_bf16<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    G4R_CUDA(cudaFuncSetAttribute(decode_attention_bf16<D, BEAM>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     set = true;
   }
-  G4R_CUDA(launch_pdl(decode_attention_bf16<D>, dim3(H, B, S), dim3(256), smem, st, dim3(1, 1, S),
+  G4R_CUDA(launch_pdl(decode_attention_bf16<D, BEAM>, dim3(H, B, S), dim3(256), smem, st, dim3(1, 1, S),
                       (const __nv_bfloat16*)q, ldq, (const __nv_bfloat16*)kcache, (const __nv_bfloat16*)vcache,
-                      (__nv_bfloat16*)out, ldo, H, kv_len, pos_dev, pos_rows, Lmax, scale, per_max));
+                      (__nv_bfloat16*)out, ldo, H, kv_len, pos_dev, pos_rows, Lmax, scale, per_max, anc));
   return G4R_OK;
 }
 
 static int decode_attention(const void* q, long long ldq, const void* kcache, const void* vcache, void* out,
                             long long ldo, int B, int H, int head_dim, int kv_len, const int* pos_dev,
-                            const int* pos_rows, int Lmax, float scale, void* stream) {
+                            const int* pos_rows, const int* anc, int Lmax, float scale, void* stream) {
   G4R_REQUIRE(q && kcache && vcache && out && B > 0 && H > 0 && kv_len > 0 && kv_len <= Lmax, "decode_attention: bad arguments");
   G4R_REQUIRE(head_dim == 64 || head_dim == 128, "decode_attention: head_dim %d", head_dim);
   G4R_REQUIRE(ldq % 8 == 0 && ((uintptr_t)q & 15) == 0, "decode_attention: q rows must be 16-byte aligned");
   cudaStream_t st = (cudaStream_t)stream;
+  if (anc) {
+    if (head_dim == 128)
+      return launch_decode_attention<128, true>(q, ldq, kcache, vcache, out, ldo, B, H, kv_len, pos_dev, pos_rows, anc,
+                                                Lmax, scale, st);
+    return launch_decode_attention<64, true>(q, ldq, kcache, vcache, out, ldo, B, H, kv_len, pos_dev, pos_rows, anc,
+                                             Lmax, scale, st);
+  }
   if (head_dim == 128)
-    return launch_decode_attention<128>(q, ldq, kcache, vcache, out, ldo, B, H, kv_len, pos_dev, pos_rows, Lmax, scale, st);
-  return launch_decode_attention<64>(q, ldq, kcache, vcache, out, ldo, B, H, kv_len, pos_dev, pos_rows, Lmax, scale, st);
+    return launch_decode_attention<128, false>(q, ldq, kcache, vcache, out, ldo, B, H, kv_len, pos_dev, pos_rows, nullptr,
+                                               Lmax, scale, st);
+  return launch_decode_attention<64, false>(q, ldq, kcache, vcache, out, ldo, B, H, kv_len, pos_dev, pos_rows, nullptr,
+                                            Lmax, scale, st);
 }
 
 extern "C" int g4r_decode_attention_bf16(const void* q, long long ldq, const void* kcache, const void* vcache,
                                          void* out, long long ldo, int B, int H, int head_dim, int kv_len,
                                          const int* pos_dev, int Lmax, float scale, void* stream) {
-  return decode_attention(q, ldq, kcache, vcache, out, ldo, B, H, head_dim, kv_len, pos_dev, nullptr, Lmax, scale, stream);
+  return decode_attention(q, ldq, kcache, vcache, out, ldo, B, H, head_dim, kv_len, pos_dev, nullptr, nullptr, Lmax, scale,
+                          stream);
 }
 
 extern "C" int g4r_decode_attention_rows_bf16(const void* q, long long ldq, const void* kcache, const void* vcache,
                                               void* out, long long ldo, int B, int H, int head_dim, int kv_bound,
                                               const int* pos_rows, int Lmax, float scale, void* stream) {
   G4R_REQUIRE(pos_rows != nullptr, "decode_attention_rows: pos_rows is NULL");
-  return decode_attention(q, ldq, kcache, vcache, out, ldo, B, H, head_dim, kv_bound, nullptr, pos_rows, Lmax, scale,
+  return decode_attention(q, ldq, kcache, vcache, out, ldo, B, H, head_dim, kv_bound, nullptr, pos_rows, nullptr, Lmax,
+                          scale, stream);
+}
+
+extern "C" int g4r_decode_attention_beam_bf16(const void* q, long long ldq, const void* kcache, const void* vcache,
+                                              void* out, long long ldo, int R, int H, int head_dim, int kv_bound,
+                                              const int* pos_rows, const int* anc, int Lmax, float scale, void* stream) {
+  G4R_REQUIRE(pos_rows != nullptr && anc != nullptr, "decode_attention_beam: pos_rows and anc are required");
+  return decode_attention(q, ldq, kcache, vcache, out, ldo, R, H, head_dim, kv_bound, nullptr, pos_rows, anc, Lmax, scale,
                           stream);
 }

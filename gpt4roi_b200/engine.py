@@ -567,12 +567,17 @@ class KVCache:
     The K/V tensors are zero-filled, and grow() zero-fills the new space: the chunk attention (kernels.attention_cached)
     reads cache rows past each row's valid length, up to the next multiple of 64, and needs them finite."""
 
-    def __init__(self, cfg, B, max_len, device):
+    def __init__(self, cfg, B, max_len, device, kv=None):
+        """kv: optional (k, v) lists of per-layer [B, max_len, HD] tensors to use instead of allocating (BeamCache's
+        prompt rows)."""
         hd = cfg.n_heads * cfg.head_dim
         dt = cfg.torch_dtype
         self.cfg = cfg
-        self.k = [torch.zeros((B, max_len, hd), dtype=dt, device=device) for _ in range(cfg.n_layers)]
-        self.v = [torch.zeros((B, max_len, hd), dtype=dt, device=device) for _ in range(cfg.n_layers)]
+        if kv is not None:
+            self.k, self.v = list(kv[0]), list(kv[1])
+        else:
+            self.k = [torch.zeros((B, max_len, hd), dtype=dt, device=device) for _ in range(cfg.n_layers)]
+            self.v = [torch.zeros((B, max_len, hd), dtype=dt, device=device) for _ in range(cfg.n_layers)]
         self.ids = torch.full((B, max_len), -1, dtype=torch.int64, device=device)
         self.B, self.max_len, self.length = B, max_len, 0
         self.lens = None
@@ -688,6 +693,7 @@ def _decode_step_chain(self, token_ids, cache, pos_dev):
     pos = cache.length
     kv_len = cache.max_len if pos_dev is not None else pos + 1   # sizes the score buffer when device-driven
     rows = cache.lens        # per-sample positions (<= pos): these override pos / pos_dev in every kernel
+    anc = getattr(cache, 'anc', None)   # a BeamCache: attention through its ancestry table, positions set by beam_step
     x = splice_region_tokens(token_ids, self.embed, None, None, 0, c.im_patch_token, c.im_start_token,
                              c.im_end_token, c.bbox_token, validate=False).view(B, c.hidden)
     cos, sin = self._rope_span(cache.max_len)
@@ -701,8 +707,7 @@ def _decode_step_chain(self, token_ids, cache, pos_dev):
             h = kernels.rmsnorm(x, w['ln_in'], c.rms_eps)
             qkv = dense.decode_gemm(h, w['wqkv'], rope=(cos, sin, 2 * c.hidden, pos, pos_dev), kv=(cache.k[li], cache.v[li]),
                                     pos_rows=rows)
-            a = kernels.decode_attention(qkv, cache.k[li], cache.v[li], B, c.n_heads, c.head_dim, kv_len, scale, pos_dev,
-                                         pos_rows=rows)
+            a = _decode_attention(cache, li, qkv, kv_len, scale, pos_dev, rows, anc)
             x = dense.linear(a, w['wo'], residual=x)
             h = kernels.rmsnorm(x, w['ln_post'], c.rms_eps)
             f = dense.decode_gemm(h, w['wgu'], act='swiglu')
@@ -719,19 +724,27 @@ def _decode_step_chain(self, token_ids, cache, pos_dev):
             qkv = dense.linear(h, w['wqkv'])
             kernels.rope_inplace(qkv, cos[pos:pos + 1].contiguous(), sin[pos:pos + 1].contiguous(), 1, 2 * c.n_heads, c.head_dim)
         kernels.kv_append(qkv, cache.k[li], cache.v[li], B, 1, pos, pos_dev, pos_rows=rows)
-        a = kernels.decode_attention(qkv, cache.k[li], cache.v[li], B, c.n_heads, c.head_dim, kv_len, scale, pos_dev,
-                                     pos_rows=rows)
+        a = _decode_attention(cache, li, qkv, kv_len, scale, pos_dev, rows, anc)
         x = dense.linear(a, w['wo'], residual=x)
         h = kernels.rmsnorm(x, w['ln_post'], c.rms_eps)
         f = dense.linear(h, w['wgu'], act='swiglu')
         x = dense.linear(f, w['wdown'], residual=x)
     cache.length = pos + 1
-    if rows is not None and pos_dev is None:
+    if rows is not None and pos_dev is None and anc is None:
         rows.add_(1)
     x = kernels.rmsnorm(x, self.norm_w, c.rms_eps)
     buf = torch.empty((B, self.vocab_pad), dtype=self.dt, device=self.dev)
     dense.linear(x, self.lm_head, out=buf[:, :c.vocab])
     return buf[:, None, :c.vocab]
+
+
+def _decode_attention(cache, li, qkv, kv_len, scale, pos_dev, rows, anc):
+    c = cache.cfg
+    if anc is None:
+        return kernels.decode_attention(qkv, cache.k[li], cache.v[li], qkv.shape[0], c.n_heads, c.head_dim, kv_len, scale,
+                                        pos_dev, pos_rows=rows)
+    return kernels.decode_attention_beam(qkv, cache.full_k[li], cache.full_v[li], qkv.shape[0], c.n_heads, c.head_dim,
+                                         kv_len, scale, rows, anc)
 
 
 class Sampler:
@@ -786,7 +799,8 @@ def sampling_seed(generator=None):
 @torch.no_grad()
 def _generate(self, input_ids, images, bboxes, max_new_tokens=32, do_sample=False, temperature=1.0,
               stopping_criteria=None, eos_token_id=None, generator=None, use_graph=True, attention_mask=None,
-              pad_token_id=None, cache=None, top_k=None, top_p=None):
+              pad_token_id=None, cache=None, top_k=None, top_p=None, num_beams=1, length_penalty=1.0,
+              early_stopping=False, num_return_sequences=1):
     """Prefill + greedy / sampled decode (gpt4roi/app.py:286-300 calls
     model.generate(input_ids, images=..., do_sample=True, temperature=0.2, max_new_tokens=1024,
     stopping_criteria=[...]) with the boxes bound to forward).  Returns ids [B, L + new]: the prompt as given,
@@ -803,7 +817,21 @@ def _generate(self, input_ids, images, bboxes, max_new_tokens=32, do_sample=Fals
     cache: a KVCache to generate into -- a conversation's earlier turns (gpt4roi/app.py re-submits the whole
     conversation every turn): the prefix it already holds is reused and only the rest is prefilled (prefill_cached);
     afterwards it holds the conversation including this turn's answer (the last new token excepted), ready for the next.
-    Rows that finished with pad_token_id keep those pads in the recorded ids, so the next turn's reuse stops there."""
+    Rows that finished with pad_token_id keep those pads in the recorded ids, so the next turn's reuse stops there.
+    num_beams > 1: deterministic beam search (transformers' GenerationMixin._beam_search, do_sample=False) with
+    length_penalty, early_stopping (True, False or "never") and num_return_sequences <= num_beams; eos_token_id may be
+    a list.  The prompt is prefilled once per sample and the beams share its KV cache (BeamCache).  Returns
+    [B * num_return_sequences, L + n] as HF crops it."""
+    if num_beams > 1:
+        if do_sample:
+            raise NotImplementedError('beam search with do_sample runs on the HF loop only: pass use_hf_loop=True')
+        if stopping_criteria is not None:
+            raise NotImplementedError('beam search with stopping_criteria runs on the HF loop only: pass use_hf_loop=True')
+        if cache is not None:
+            raise NotImplementedError('beam search on a conversation cache (cache=) runs on the HF loop only: pass '
+                                      'use_hf_loop=True')
+        return _generate_beams(self, input_ids, images, bboxes, max_new_tokens, num_beams, eos_token_id, pad_token_id,
+                               attention_mask, length_penalty, early_stopping, num_return_sequences, use_graph)
     B, L = input_ids.shape
     ids = input_ids.to(self.dev)
     if cache is not None:
@@ -904,6 +932,160 @@ class GraphedDecode:
         if self.sampler is not None:
             self.sampler.advance()
         return self.logits
+
+
+class BeamCache:
+    """KV cache and device state of beam search over B samples of N beams.  Per layer one [B + B*N, Lmax, HD] tensor
+    (full_k / full_v): rows 0..B-1 hold the prompts (the B-row prefill writes them through `prompt`, a KVCache whose
+    k / v are the views [:B]), rows B.. the beams (the decode step writes beam row r's new K/V at pos_rows[r] through
+    the views k / v = [B:]).  A cell is written once and never moved: `anc` (int32 [B*N, Lmax]) names the cache row
+    that holds position p of beam row r -- its sample's prompt row below lens[b], else the beam row that wrote it --
+    and the beam step permutes its generated columns when the beams are reordered.  The rest is the state of
+    transformers' _beam_search that kernels.beam_step keeps on the device (see g4r_beam_step_bf16)."""
+
+    def __init__(self, cfg, B, N, prompt_len, max_new_tokens, device, eos=(), length_penalty=1.0, early_stopping=False,
+                 fill=-1):
+        hd = cfg.n_heads * cfg.head_dim
+        dt = cfg.torch_dtype
+        dev = torch.device(device)
+        R = B * N
+        Lmax = prompt_len + max_new_tokens
+        self.cfg, self.B, self.N, self.prompt_len = cfg, R, N, prompt_len
+        self.n_samples = B
+        self.full_k = [torch.zeros((B + R, Lmax, hd), dtype=dt, device=dev) for _ in range(cfg.n_layers)]
+        self.full_v = [torch.zeros((B + R, Lmax, hd), dtype=dt, device=dev) for _ in range(cfg.n_layers)]
+        self.prompt = KVCache(cfg, B, Lmax, dev, kv=([t[:B] for t in self.full_k], [t[:B] for t in self.full_v]))
+        self.k = [t[B:] for t in self.full_k]
+        self.v = [t[B:] for t in self.full_v]
+        self.max_len = self.Lmax = Lmax
+        self.length = 0
+        self.G = max_new_tokens
+        self.max_length = prompt_len + max_new_tokens
+        eos = [int(e) for e in eos]
+        self.n_eos = len(eos)
+        self.K = max(2, 1 + len(eos)) * N            # beams_to_keep
+        self.eos = torch.tensor(eos, dtype=torch.int32, device=dev) if eos else None
+        self.length_penalty = float(length_penalty)
+        if early_stopping not in (True, False, 'never'):
+            raise ValueError('early_stopping must be True, False or "never", got %r' % (early_stopping,))
+        self.early = 2 if early_stopping == 'never' else int(bool(early_stopping))
+        self.fill = int(fill)
+        self.lens = torch.zeros(R, dtype=torch.int32, device=dev)          # pos_rows of the decode step
+        self.pos_rows = self.lens
+        self.prompt_lens = torch.full((B,), prompt_len, dtype=torch.int32, device=dev)
+        self.anc = torch.zeros((R, Lmax), dtype=torch.int32, device=dev)
+        self.ids = torch.zeros((R, 1), dtype=torch.int64, device=dev)     # the graph's own input
+        self.state = torch.zeros(4 * B + 2, dtype=torch.int32, device=dev)
+        self.state[1:4 * B:4] = 1                                           # early-stop heuristic unsatisfied
+        self.run_score = torch.zeros((B, N), dtype=torch.float32, device=dev)
+        self.run_score[:, 1:] = -1e9
+        self.run_score = self.run_score.view(R)
+        self.cand_score = torch.empty(R * self.K, dtype=torch.float32, device=dev)
+        self.cand_tok = torch.empty(R * self.K, dtype=torch.int32, device=dev)
+        self.run_seq = torch.full((2, B, N, self.G), self.fill, dtype=torch.int64, device=dev)
+        self.fin_seq = torch.full((2, B, N, self.G), self.fill, dtype=torch.int64, device=dev)
+        self.fin_score = torch.full((B, N), -1e9, dtype=torch.float32, device=dev)
+        self.fin_state = torch.zeros((B, N, 2), dtype=torch.int32, device=dev)
+
+    def start(self, lens):
+        """After the prefill: lens (device int32 [B]) each sample's prompt length; every beam row's prompt positions
+        point at its sample's prompt row."""
+        B = self.n_samples
+        self.prompt_lens = lens.to(torch.int32).contiguous()
+        self.anc.copy_(torch.arange(B, dtype=torch.int32, device=self.anc.device).repeat_interleave(self.N)[:, None]
+                       .expand(self.anc.shape))
+        self.length = self.prompt_len
+
+    def step(self, logits, first=False):
+        """The beam step on this step's logits (first: the prefill's [B, V] rows, shared by each sample's beams)."""
+        kernels.beam_step(logits, self.N if first else 1, self)
+
+    def done(self):
+        """Whether the search has ended (transformers' _beam_search_has_unfinished_sequences is False): one word."""
+        return bool(self.state[4 * self.n_samples + 1])
+
+    def result(self, num_return_sequences, prompt_ids):
+        """[B * num_return_sequences, L + n]: each sample's best finished beams after the prompt as given, cropped to the
+        longest returned one (HF's "prepare outputs")."""
+        B, N = self.n_samples, self.N
+        g = int(self.state[0])
+        seqs = self.fin_seq[g & 1][:, :num_return_sequences].reshape(B * num_return_sequences, self.G)
+        n = int(self.fin_state[:, :num_return_sequences, 1].max())
+        prompt = prompt_ids.to(seqs.device).repeat_interleave(num_return_sequences, 0)
+        return torch.cat([prompt, seqs[:, :n]], 1)
+
+
+class GraphedBeamDecode:
+    """CUDA-graph replay of one beam-search step: the decode step over the B*N beam rows of a BeamCache (attention
+    through its ancestry table) followed by the beam step, which writes the next ids into cache.ids -- the graph's own
+    input -- and the beam rows' positions and ancestry, so step() takes nothing from the host.  Build it after the
+    first beam step (from the prefill logits) has run."""
+
+    def __init__(self, engine, cache):
+        self.eng, self.cache = engine, cache
+        dev = engine.dev
+        self.pos = torch.tensor([cache.length], dtype=torch.int32, device=dev)   # sizes the step by max_len
+        start = cache.length
+        side = torch.cuda.Stream(device=dev)
+        side.wait_stream(torch.cuda.current_stream(dev))
+        with torch.cuda.stream(side):
+            for _ in range(2):  # warm-up (writes each beam row's current position, rewritten by the first real step)
+                engine.decode_step(cache.ids, cache, self.pos)
+                cache.length = start
+        torch.cuda.current_stream(dev).wait_stream(side)
+        torch.cuda.synchronize(dev)
+        self.graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(self.graph):
+            self.logits = engine.decode_step(cache.ids, cache, self.pos)
+            cache.step(self.logits)
+        cache.length = start
+
+    def step(self):
+        if self.cache.length + 1 > self.cache.max_len:
+            raise RuntimeError('KV cache is full (%d)' % self.cache.max_len)
+        self.graph.replay()
+        self.cache.length += 1
+        return self.logits
+
+
+@torch.no_grad()
+def _generate_beams(self, input_ids, images, bboxes, max_new_tokens, num_beams, eos_token_id, pad_token_id,
+                    attention_mask, length_penalty, early_stopping, num_return_sequences, use_graph):
+    B, L = input_ids.shape
+    N = int(num_beams)
+    if not 1 <= num_return_sequences <= N:
+        raise ValueError('num_return_sequences (%d) must be between 1 and num_beams (%d)' % (num_return_sequences, N))
+    if max_new_tokens < 1:
+        raise ValueError('max_new_tokens must be >= 1')
+    eos = [] if eos_token_id is None else [int(e) for e in (eos_token_id if isinstance(eos_token_id, (list, tuple))
+                                                               else [eos_token_id])]
+    fill = (pad_token_id or eos[0]) if eos else -1        # HF's output_fill_value
+    ids = input_ids.to(self.dev)
+    cache = BeamCache(self.cfg, B, N, L, max_new_tokens, self.dev, eos, length_penalty, early_stopping, fill)
+    plan = self.plan_boxes(bboxes)
+    run_ids, seqlens = ids, None
+    lens = torch.full((B,), L, dtype=torch.int32, device=self.dev)
+    if attention_mask is not None:
+        lens, shift = right_pad_layout(attention_mask.to(self.dev))
+        if bool(shift.any()):
+            run_ids = to_right_padded(ids, shift).contiguous()
+        if not bool((lens == L).all()):
+            seqlens = lens.to(torch.int32).contiguous()
+    logits = self.forward_device(run_ids.contiguous(), None if images is None else images.to(self.dev, self.dt), plan,
+                                 validate=True, last_only=True, seqlens=seqlens, cache=cache.prompt)
+    cache.start(lens)
+    cache.step(logits, first=True)
+    stepper = None
+    if use_graph and max_new_tokens > 4 and self.cfg.head_dim == 128:
+        stepper = GraphedBeamDecode(self, cache)
+    for _ in range(max_new_tokens):      # the max-length criterion ends the search by then
+        if cache.done():
+            break
+        if stepper is not None:
+            stepper.step()
+        else:
+            cache.step(self.decode_step(cache.ids, cache))
+    return cache.result(num_return_sequences, ids)
 
 
 PrefillEngine.decode_step = _decode_step

@@ -263,3 +263,35 @@ def decode_attention(qkv, kcache, vcache, B, n_heads, head_dim, kv_len, scale, p
           _L.ptr(out), out.stride(0), B, n_heads, head_dim, int(kv_len), _L.ptr(pos_dev), kcache.shape[1], float(scale),
           act=act)
     return out
+
+
+def decode_attention_beam(qkv, kcache, vcache, R, n_heads, head_dim, kv_bound, scale, pos_rows, anc):
+    """Beam-search decode attention: qkv [R, 3*HD] (one new token per beam row); caches [rows, Lmax, HD] shared by all
+    R rows; row r attends over positions 0..pos_rows[r], reading position p from cache row anc[r, p] (anc: device int32
+    [R, Lmax]).  kv_bound (>= every pos_rows[r] + 1) sizes the split and the score buffer.  Returns [R, HD]."""
+    act = _bf16(qkv, kcache, vcache)
+    Lmax = kcache.shape[1]
+    if anc.dtype != torch.int32 or tuple(anc.shape) != (R, Lmax) or not anc.is_contiguous():
+        raise RuntimeError('decode_attention_beam: anc must be a contiguous device int32 [%d, %d] table' % (R, Lmax))
+    out = torch.empty((R, n_heads * head_dim), dtype=act, device=qkv.device)
+    _call('g4r_decode_attention_beam_bf16', qkv.device, _L.ptr(qkv), qkv.stride(0), _L.ptr(kcache), _L.ptr(vcache),
+          _L.ptr(out), out.stride(0), R, n_heads, head_dim, int(kv_bound), _L.ptr(_pos_rows(pos_rows, R)), _L.ptr(anc),
+          Lmax, float(scale), act=act)
+    return out
+
+
+def beam_step(logits, row_div, st):
+    """One beam-search step (csrc/beam.cu) on 16-bit logits [rows, V] (or [rows, 1, V]; unit column stride) with the
+    device state of st (engine.BeamCache): B*N rows, or B with row_div = N (the first step, from the prefill)."""
+    rows = logits.reshape(logits.shape[0], logits.shape[-1]) if logits.dim() == 3 else logits
+    act = _bf16(rows)
+    V = rows.shape[1]
+    B, N = st.n_samples, st.N
+    if rows.stride(1) != 1 or rows.shape[0] * row_div != B * N:
+        raise RuntimeError('beam_step: logits must be [%d, V] rows with unit column stride' % (B * N // row_div))
+    _L.require_cuda_same_device([('logits', rows), ('state', st.state), ('anc', st.anc)])
+    _call('g4r_beam_step_bf16', rows.device, _L.ptr(rows), rows.stride(0), int(row_div), B, N, V, st.K,
+          _L.ptr(st.eos), st.n_eos, st.prompt_len, st.max_length, float(st.length_penalty), st.early, st.G, st.Lmax,
+          _L.ptr(st.prompt_lens), _L.ptr(st.state), _L.ptr(st.run_score), _L.ptr(st.cand_score), _L.ptr(st.cand_tok),
+          _L.ptr(st.run_seq), _L.ptr(st.fin_seq), _L.ptr(st.fin_score), _L.ptr(st.fin_state), _L.ptr(st.ids),
+          _L.ptr(st.pos_rows), _L.ptr(st.anc), act=act)

@@ -258,6 +258,22 @@ class G4RCache:
     def __bool__(self):
         return True
 
+    def reorder_cache(self, beam_idx):
+        """transformers' beam search (GenerationMixin._beam_search) after every step: row i of the cache becomes row
+        beam_idx[i] -- every layer's K/V, the recorded ids, lengths, images and boxes.  In place, so a CUDA graph
+        captured on the cache (the stepper) stays valid."""
+        kv = self.kv
+        idx = beam_idx.to(kv.ids.device, torch.long)
+        for t in kv.k + kv.v:
+            t.copy_(t.index_select(0, idx.to(t.device)))
+        kv.ids.copy_(kv.ids.index_select(0, idx))
+        if kv.lens is not None:
+            kv.lens.copy_(kv.lens.index_select(0, idx.to(kv.lens.device)))
+        if kv.images is not None:
+            kv.images.copy_(kv.images.index_select(0, idx.to(kv.images.device)))
+        if kv.boxes is not None:
+            kv.boxes = [kv.boxes[i] for i in idx.tolist()]
+
 
 def _find_cache(past_key_values):
     """Our cache, whether handed back directly or riding on the (otherwise unused) HF Cache object that
@@ -510,6 +526,47 @@ def resolve_sampling(model, input_len, do_sample=None, temperature=None, **kwarg
             float(gc.top_p if gc.top_p is not None else 1.0))
 
 
+def resolve_beam_search(model, input_len, max_new_tokens, do_sample=None, **kwargs):
+    """The engine loop's beam search for a generate call, resolved as transformers resolves it (explicit kwargs, then
+    `generation_config=`, then model.generation_config, then HF's defaults: GenerationMixin._prepare_generation_config).
+    Returns None when the resolved num_beams is 1, else a dict of num_beams, length_penalty, early_stopping,
+    num_return_sequences, eos_token_id (a list), pad_token_id and max_length.  Beam search with do_sample, with any
+    logits processor, or with output_scores / return_dict_in_generate raises NotImplementedError: the HF loop
+    (use_hf_loop=True) runs those."""
+    from transformers.utils import logging as hf_logging
+    given = {k: v for k, v in dict(kwargs, do_sample=do_sample, max_new_tokens=max_new_tokens).items() if v is not None}
+    verbosity = hf_logging.get_verbosity()
+    hf_logging.set_verbosity_error()
+    try:
+        gc, _ = model._prepare_generation_config(given.pop('generation_config', None), **given)
+        model._prepare_special_tokens(gc, True, 'cpu')
+    finally:
+        hf_logging.set_verbosity(verbosity)
+    N = gc.num_beams or 1
+    if N <= 1:
+        return None
+    hf = 'runs on the HF loop only: pass use_hf_loop=True'
+    if gc.do_sample:
+        raise NotImplementedError('beam search with do_sample (beam sampling) ' + hf)
+    if gc.output_scores or gc.output_logits or gc.return_dict_in_generate:
+        raise NotImplementedError('beam search with output_scores / return_dict_in_generate ' + hf)
+    procs = model._get_logits_processor(gc, input_ids_seq_length=input_len, device='cpu', model_kwargs={},
+                                        logits_processor=kwargs.get('logits_processor'))
+    if len(procs):
+        raise NotImplementedError('the engine loop applies no logits processor to beam search; %s %s'
+                                  % (', '.join(type(p).__name__ for p in procs), hf))
+    nrs = gc.num_return_sequences or 1
+    if nrs > N:
+        raise ValueError('num_return_sequences (%d) must be <= num_beams (%d)' % (nrs, N))
+    eos = gc._eos_token_tensor
+    pad = gc._pad_token_tensor
+    return dict(num_beams=int(N), length_penalty=float(gc.length_penalty if gc.length_penalty is not None else 1.0),
+                early_stopping=gc.early_stopping if gc.early_stopping is not None else False,
+                num_return_sequences=int(nrs), eos_token_id=None if eos is None else eos.flatten().tolist(),
+                pad_token_id=None if pad is None else int(pad),
+                max_length=int(input_len + gc.max_new_tokens if gc.max_new_tokens is not None else gc.max_length))
+
+
 class SPILlavaMPTForCausalLM(LlamaForCausalLM, _EngineHost):
     """Drop-in for gpt4roi.models.spi_llava.SPILlavaMPTForCausalLM (spi_llava.py:215-306)."""
     config_class = LlavaConfig
@@ -671,6 +728,20 @@ class SPILlavaMPTForCausalLM(LlamaForCausalLM, _EngineHost):
             model_inputs['is_first_iteration'] = True
         return model_inputs
 
+    @staticmethod
+    def _expand_inputs_for_generation(expand_size=1, is_encoder_decoder=False, input_ids=None, **model_kwargs):
+        """HF's expansion (beam search, num_return_sequences) repeats tensors only; the per-sample python lists of
+        `bboxes` and `images` are repeated the same way (row i -> rows i*expand_size ..), so every expanded row keeps
+        its own boxes."""
+        input_ids, model_kwargs = LlamaForCausalLM._expand_inputs_for_generation(
+            expand_size=expand_size, is_encoder_decoder=is_encoder_decoder, input_ids=input_ids, **model_kwargs)
+        if expand_size > 1:
+            for key in ('bboxes', 'images'):
+                v = model_kwargs.get(key)
+                if isinstance(v, (list, tuple)):
+                    model_kwargs[key] = [x for x in v for _ in range(expand_size)]
+        return input_ids, model_kwargs
+
     @torch.no_grad()
     def generate(self, input_ids=None, images=None, bboxes=None, max_new_tokens=32, do_sample=None,
                  temperature=None, stopping_criteria=None, eos_token_id=None, use_hf_loop=False, **kwargs):
@@ -684,7 +755,11 @@ class SPILlavaMPTForCausalLM(LlamaForCausalLM, _EngineHost):
         Sampling on the engine loop follows HF's resolution of do_sample / temperature / top_k / top_p /
         generation_config (resolve_sampling: the demo's call samples from the top 50 at T = 0.2, as on the HF loop);
         the draws are keyed by torch's default generator (or `generator=`), so torch.manual_seed makes them
-        reproducible.  Other logits processors and beam search raise NotImplementedError there."""
+        reproducible.  Other logits processors raise NotImplementedError there.
+        num_beams > 1 (do_sample false) runs beam search on the engine loop (resolve_beam_search: length_penalty,
+        early_stopping, num_return_sequences, eos / max length as HF resolves them): the prompt is prefilled once per
+        sample and the beams share its KV cache; beam sampling, logits processors, stopping_criteria, output_scores /
+        return_dict_in_generate and past_key_values raise NotImplementedError there, and run with use_hf_loop=True."""
         if bboxes is None:
             bboxes = getattr(getattr(self, 'forward', None), 'keywords', {}).get('bboxes')
         if use_hf_loop:
@@ -701,6 +776,21 @@ class SPILlavaMPTForCausalLM(LlamaForCausalLM, _EngineHost):
                                     do_sample=bool(do_sample), use_cache=True, **kw)
         gen = {k: v for k, v in kwargs.items() if k not in ('attention_mask', 'pad_token_id', 'past_key_values',
                                                              'generator')}
+        beam = resolve_beam_search(self, input_ids.shape[1], max_new_tokens, do_sample, eos_token_id=eos_token_id,
+                                   pad_token_id=kwargs.get('pad_token_id'), **gen)
+        if beam is not None:
+            if stopping_criteria is not None:
+                raise NotImplementedError('beam search with stopping_criteria runs on the HF loop only: pass '
+                                          'use_hf_loop=True')
+            if kwargs.get('past_key_values') is not None:
+                raise NotImplementedError('beam search on a conversation cache (past_key_values) runs on the HF loop '
+                                          'only: pass use_hf_loop=True')
+            eng = self._get_engine(input_ids.device)
+            return eng.generate(input_ids, images, bboxes, max_new_tokens=beam['max_length'] - input_ids.shape[1],
+                                num_beams=beam['num_beams'], length_penalty=beam['length_penalty'],
+                                early_stopping=beam['early_stopping'], num_return_sequences=beam['num_return_sequences'],
+                                eos_token_id=beam['eos_token_id'], pad_token_id=beam['pad_token_id'],
+                                attention_mask=kwargs.get('attention_mask'))
         do_sample, temperature, top_k, top_p = resolve_sampling(self, input_ids.shape[1], do_sample, temperature, **gen)
         eng = self._get_engine(input_ids.device)
         kv = None

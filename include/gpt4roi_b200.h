@@ -285,6 +285,29 @@ int g4r_kv_append_rows_bf16(const void* qkv, long long ld, void* kcache, void* v
 int g4r_decode_attention_rows_bf16(const void* q, long long ldq, const void* kcache, const void* vcache,
                                    void* out, long long ldo, int B, int H, int head_dim, int kv_bound,
                                    const int* pos_rows, int Lmax, float scale, void* stream);
+/* g4r_decode_attention_rows_bf16 for beam search: the caches are shared by all R rows, and key / value p of row r is
+ * read from cache row anc[r * Lmax + p] (device int32 [R, Lmax], the ancestry table) instead of row r. */
+int g4r_decode_attention_beam_bf16(const void* q, long long ldq, const void* kcache, const void* vcache,
+                                   void* out, long long ldo, int R, int H, int head_dim, int kv_bound,
+                                   const int* pos_rows, const int* anc, int Lmax, float scale, void* stream);
+
+/* ---- beam search step (the beam decode loop's last two kernels) -----------------------------
+ * One step of transformers' GenerationMixin._beam_search with do_sample=False for B samples of N beams, on logits
+ * (16-bit rows, pitch ld: B*N rows; row_div = N reads sample b's single row for all its beams, the first step
+ * from the prefill logits, else 1).  K = beams_to_keep = max(2, 1 + n_eos) * N; eos_ids: device int32 [n_eos].
+ * prompt_len: the padded prompt length, max_length = prompt_len + max_new_tokens, early_stopping 0 (False), 1 (True)
+ * or 2 ("never").  G: generated columns of run_seq / fin_seq (int64 [2, B, N, G], double-buffered by the parity of the
+ * step).  state: int32 [4B + 2] (per sample: tokens generated, early-stop heuristic unsatisfied, flags; then a ticket
+ * and the batch's done word); run_score: fp32 [B*N]; cand_score / cand_tok: [B*N*K] scratch; fin_score: fp32 [B, N];
+ * fin_state: int32 [B, N, 2] (finished, generated length).  Writes the next ids (int64 [B*N]), each beam row's
+ * position pos_rows = lens[b] + g and the ancestry table anc (int32 [B*N, Lmax]: generated columns permuted to the new
+ * parents, the new position pointing at cache row B + r).  Ties in score go to the lower flat index beam * V + token.
+ * Capturable: every per-step value is read from device memory. */
+int g4r_beam_step_bf16(const void* logits, long long ld, int row_div, int B, int N, int V, int K, const int* eos_ids,
+                       int n_eos, int prompt_len, int max_length, double length_penalty, int early_stopping, int G,
+                       int Lmax, const int* lens, int* state, float* run_score, float* cand_score, int* cand_tok,
+                       long long* run_seq, long long* fin_seq, float* fin_score, int* fin_state, long long* ids,
+                       int* pos_rows, int* anc, void* stream);
 
 /* ---- next-token selection (the decode loop's last kernel) ------------------------------------
  * logits: 16-bit [B, V] rows, row pitch ld elements.  Writes out_ids[b] (int64, like the decode step's ids buffer).
@@ -666,6 +689,14 @@ int g4r_attention_cached_f16(const void* q, long long ldq, const void* kcache, c
 int g4r_sample_tokens_f16(const void* logits, long long ld, int B, int V, float temperature, int top_k, float top_p,
                           int greedy, unsigned long long seed, const long long* rng_step, int eos_id, int pad_id,
                           int* finished, long long* out_ids, void* stream);
+int g4r_decode_attention_beam_f16(const void* q, long long ldq, const void* kcache, const void* vcache,
+                                  void* out, long long ldo, int R, int H, int head_dim, int kv_bound,
+                                  const int* pos_rows, const int* anc, int Lmax, float scale, void* stream);
+int g4r_beam_step_f16(const void* logits, long long ld, int row_div, int B, int N, int V, int K, const int* eos_ids,
+                      int n_eos, int prompt_len, int max_length, double length_penalty, int early_stopping, int G,
+                      int Lmax, const int* lens, int* state, float* run_score, float* cand_score, int* cand_tok,
+                      long long* run_seq, long long* fin_seq, float* fin_score, int* fin_state, long long* ids,
+                      int* pos_rows, int* anc, void* stream);
 
 #ifdef __cplusplus
 }
