@@ -129,12 +129,6 @@ def matmul_t(a, b, a_mn=False, b_mn=False, out_dtype=torch.bfloat16, out=None):
     return out
 
 
-def _pos_rows(pos_rows, n):
-    if pos_rows.dtype != torch.int32 or tuple(pos_rows.shape) != (n,) or not pos_rows.is_contiguous():
-        raise RuntimeError('pos_rows must be a contiguous device int32 [%d] vector' % n)
-    return pos_rows
-
-
 def qkv_rope(x, wqkv, cos, sin, L, rope_cols, pos0=0, pos_dev=None, pos_rows=None):
     """Fused LLaMA q/k/v projection + rotary embedding: x [M,K] bf16, wqkv [N,K] (q|k|v rows), cos/sin
     bf16 [L,128]; columns [0,rope_cols) (q and k heads, head_dim 128) are rotated at position row % L.
@@ -149,7 +143,7 @@ def qkv_rope(x, wqkv, cos, sin, L, rope_cols, pos0=0, pos_dev=None, pos_rows=Non
         if pos_rows is not None:
             _L.check(getattr(_L.load(), _L.sym('g4r_gemm_qkv_rope_rows_bf16', a16))(
                 _L.ptr(x), x.stride(0), _L.ptr(wqkv), wqkv.stride(0), _L.ptr(out), N, M, N, K, _L.ptr(cos), _L.ptr(sin),
-                int(rope_cols), int(L), _L.ptr(_pos_rows(pos_rows, M // L)), _L.stream_ptr(dev)))
+                int(rope_cols), int(L), _L.ptr(_L.require_pos_rows(pos_rows, M // L)), _L.stream_ptr(dev)))
         else:
             _L.check(getattr(_L.load(), _L.sym('g4r_gemm_qkv_rope_bf16', a16))(
                 _L.ptr(x), x.stride(0), _L.ptr(wqkv), wqkv.stride(0), _L.ptr(out), N, M, N, K, _L.ptr(cos), _L.ptr(sin),
@@ -230,8 +224,8 @@ def decode_gemm(x, weight, act=None, residual=None, rope=None, kv=None, pos_rows
             _L.check(getattr(_L.load(), _L.sym('g4r_decode_gemm_rows_bf16', a16))(
                 _L.ptr(x), x.stride(0), _L.ptr(weight), weight.stride(0), _L.ptr(out), out.stride(0), M, N, K,
                 ACT[act], _L.ptr(residual), residual.stride(0) if residual is not None else 0,
-                _L.ptr(cos), _L.ptr(sin), int(rope_cols), _L.ptr(_pos_rows(pos_rows, M)), _L.ptr(kc), _L.ptr(vc), int(lmax),
-                int(hd), _L.stream_ptr(dev)))
+                _L.ptr(cos), _L.ptr(sin), int(rope_cols), _L.ptr(_L.require_pos_rows(pos_rows, M)), _L.ptr(kc), _L.ptr(vc),
+                int(lmax), int(hd), _L.stream_ptr(dev)))
             _prof_end(dev, _ps, 'gemm', 2.0 * M * N * K)
             return out
         _L.check(getattr(_L.load(), _L.sym('g4r_decode_gemm_bf16', a16))(

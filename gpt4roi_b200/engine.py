@@ -16,10 +16,11 @@ from (c,ph,pw) to (ph,pw,c)).  Numerics: bf16 storage, fp32 accumulation, roundi
 reference under bf16 autocast.
 """
 import math
+import os
 
 import torch
 
-from . import dense, kernels
+from . import dense, kernels, lib
 from .roi_align import roi_align_mlvl
 from .splice import splice_region_tokens
 
@@ -40,7 +41,6 @@ class EngineConfig:
         when the model was cast to bf16, the BASELINE "7B bf16 prefill" mode) or 'fp32' (what the reference has
         whenever its parameters are fp32 under autocast; closer to the fp32 anchor at 32 layers, somewhat slower:
         tests/test_parity_7b_gpu.py).  Env G4R_LLAMA_STREAM overrides the default."""
-        import os
         if llama_stream is None:
             llama_stream = os.environ.get('G4R_LLAMA_STREAM', 'bf16')
         if llama_stream not in ('fp32', 'bf16'):
@@ -50,7 +50,6 @@ class EngineConfig:
         if dtype not in ('bf16', 'fp16'):
             raise ValueError("dtype must be 'bf16' or 'fp16'")
         self.__dict__.update(locals())
-        del self.__dict__['os']
         del self.__dict__['self']
         self.torch_dtype = torch.bfloat16 if dtype == 'bf16' else torch.float16
         self.grid = image_size // patch_size
@@ -340,6 +339,18 @@ class PrefillEngine:
             bidx = torch.zeros((0,), dtype=torch.float32, device=self.dev)
         return dict(K=K, boxes=boxes, bidx=bidx, offs=offs)
 
+    def _region(self, plan, taps):
+        """The splice's region argument for a box plan: (region-token rows, per-sample offsets), or None without a plan.
+        taps: the ViT hidden states the rows are computed from; None, or a plan without boxes: one zero row."""
+        if plan is None:
+            return None
+        if plan['K'] > 0 and taps is not None:
+            maps, ss = self.fuse_maps(taps)
+            rows = self.region_tokens(maps, ss, plan['boxes'], plan['bidx'])
+        else:
+            rows = torch.zeros((1, self.cfg.hidden), dtype=self.dt, device=self.dev)
+        return rows, plan['offs']
+
     def forward_device(self, input_ids, images, plan, validate=True, last_only=False, seqlens=None, cache=None,
                        hidden_taps=None, want='logits', stage_taps=None):
         """Device-only forward (capturable): input_ids int64 [B,L], images bf16 [B,3,S,S] on the GPU.
@@ -347,27 +358,17 @@ class PrefillEngine:
         stage_taps: optional dict filled with 'vit_taps', 'region', 'embeds' (parity tests)."""
         c = self.cfg
         B, L = input_ids.shape
-        if images is None:
-            embeds = splice_region_tokens(input_ids, self.embed, None, None, 0, c.im_patch_token, c.im_start_token,
-                                          c.im_end_token, c.bbox_token, validate=False)
-            if cache is not None:
-                cache.start(L, seqlens, input_ids)
-            return self.llama(embeds, B, L, last_only=last_only, seqlens=seqlens, cache=cache,
-                              hidden_taps=hidden_taps, want=want)
-        taps = self.vit(images)
-        feat = kernels.cast_tokens_f32_bf16(taps[c.select_index], dtype=self.dt)  # spi_llava.py:68-73 (+ autocast cast, CLS dropped)
-        img_rows = dense.linear(feat, self.proj_w, self.proj_b).view(B, c.num_patches, c.hidden)
-        region = None
-        if plan is not None:
-            if plan['K'] > 0:
-                maps, ss = self.fuse_maps(taps)
-                rows = self.region_tokens(maps, ss, plan['boxes'], plan['bidx'])
-            else:
-                rows = torch.zeros((1, c.hidden), dtype=self.dt, device=self.dev)
-            region = (rows, plan['offs'])
-        embeds = splice_region_tokens(input_ids, self.embed, img_rows, region, c.num_patches, c.im_patch_token,
-                                      c.im_start_token, c.im_end_token, c.bbox_token, validate=validate)
-        if stage_taps is not None:
+        vision = images is not None
+        img_rows = region = None
+        if vision:
+            taps = self.vit(images)
+            feat = kernels.cast_tokens_f32_bf16(taps[c.select_index], dtype=self.dt)  # spi_llava.py:68-73 (+ autocast cast, CLS dropped)
+            img_rows = dense.linear(feat, self.proj_w, self.proj_b).view(B, c.num_patches, c.hidden)
+            region = self._region(plan, taps)
+        embeds = splice_region_tokens(input_ids, self.embed, img_rows, region, c.num_patches if vision else 0,
+                                      c.im_patch_token, c.im_start_token, c.im_end_token, c.bbox_token,
+                                      validate=validate and vision)
+        if stage_taps is not None and vision:
             stage_taps['vit_taps'] = [taps[l][:, 1:] for l in c.level_layers]
             stage_taps['region'] = region[0] if (region is not None and plan['K'] > 0) else None
             stage_taps['embeds'] = embeds
@@ -387,18 +388,11 @@ class PrefillEngine:
         hidden_taps / stage_taps / the cache hold the right-padded layout; the cache also records the token ids, images
         and boxes it was computed from (a later turn reuses it: generate(cache=))."""
         plan = self.plan_boxes(bboxes)
-        seqlens = None
-        input_ids = input_ids.to(self.dev, non_blocking=True)
-        shift = None
-        if attention_mask is not None:
-            lens, shift = right_pad_layout(attention_mask.to(self.dev))
-            seqlens = lens.to(torch.int32).contiguous()
-            if bool(shift.any()):
-                input_ids = to_right_padded(input_ids, shift)
-            else:
-                shift = None
+        input_ids, lens, shift = _right_padded(input_ids.to(self.dev, non_blocking=True), attention_mask)
+        # a mask, even an all-ones one, gives the cache per-row lengths
+        seqlens = None if attention_mask is None else lens.to(torch.int32)
         images = None if images is None else images.to(self.dev, self.dt, non_blocking=True).contiguous()
-        out = self.forward_device(input_ids.contiguous(), images, plan, validate, last_only, seqlens, cache=cache,
+        out = self.forward_device(input_ids, images, plan, validate, last_only, seqlens, cache=cache,
                                   hidden_taps=hidden_taps, want=want, stage_taps=stage_taps)
         if cache is not None:
             cache.set_source(images, bboxes)
@@ -420,29 +414,21 @@ class PrefillEngine:
         c = self.cfg
         if c.head_dim != 128:
             raise NotImplementedError('continuing a cached sequence needs the fused-RoPE QKV GEMM (head_dim 128)')
-        ids = input_ids.to(self.dev).contiguous()
+        ids, lens, shift = _right_padded(input_ids.to(self.dev), attention_mask)
+        if shift is not None:
+            raise NotImplementedError('extend takes right-padded chunks')
         B, Lc = ids.shape
-        valid = torch.full((B,), Lc, dtype=torch.int32, device=self.dev)
-        qlen = None
-        if attention_mask is not None:
-            lens, shift = right_pad_layout(attention_mask.to(self.dev))
-            if bool(shift.any()):
-                raise NotImplementedError('extend takes right-padded chunks')
-            valid = lens.to(torch.int32).contiguous()
-            qlen = None if bool((valid == Lc).all()) else valid
+        valid = lens.to(torch.int32)
+        qlen = _seqlens(lens, Lc)
         start = cache.row_lens().clone()
         start_h = start.cpu()
         cache.grow(int(start_h.max()) + Lc)   # every row appends all Lc chunk rows, its padding included
-        region = None
         plan = self.plan_boxes(bboxes)
-        if plan is not None:   # the splice checks each row's <bbox> count against its boxes (status 3)
-            if plan['K'] > 0 and bool((ids == c.bbox_token).any()):
-                images = images.to(self.dev, self.dt).contiguous()
-                maps, ss = self.fuse_maps(self.vit(images))
-                rows = self.region_tokens(maps, ss, plan['boxes'], plan['bidx'])
-            else:
-                rows = torch.zeros((1, c.hidden), dtype=self.dt, device=self.dev)
-            region = (rows, plan['offs'])
+        taps = None
+        if plan is not None and plan['K'] > 0 and bool((ids == c.bbox_token).any()):
+            images = images.to(self.dev, self.dt).contiguous()
+            taps = self.vit(images)
+        region = self._region(plan, taps)   # the splice checks each row's <bbox> count against its boxes (status 3)
         embeds = splice_region_tokens(ids, self.embed, None, region, 0, c.im_patch_token, c.im_start_token,
                                       c.im_end_token, c.bbox_token, validate=True, continuation=True)
         logits = self.llama(embeds, B, Lc, last_only=last_only, seqlens=qlen, cache=cache, start=start)
@@ -452,8 +438,8 @@ class PrefillEngine:
         for b in range(B):
             n_old = int((rec[b, :int(start_h[b])] == c.bbox_token).sum())
             old = cache.boxes[b] if cache.boxes is not None and cache.boxes[b] is not None else torch.zeros(0, 4)
-            new = _row_boxes(bboxes, b)
-            new = torch.zeros(0, 4) if new is None else new.detach().to('cpu', torch.float32)
+            new = _row_boxes(bboxes, b, host=True)
+            new = torch.zeros(0, 4) if new is None else new
             boxes.append(torch.cat([old[:n_old], new], 0))
         cache.record_ids(ids, start)
         cache.lens = (start + valid).to(torch.int32)
@@ -474,13 +460,7 @@ class PrefillEngine:
         B, L = input_ids.shape
         if B != cache.B:
             raise ValueError('the cache holds %d rows, the prompt has %d' % (cache.B, B))
-        ids = input_ids.to(self.dev)
-        lens = torch.full((B,), L, dtype=torch.int64, device=self.dev)
-        if attention_mask is not None:
-            lens, shift = right_pad_layout(attention_mask.to(self.dev))
-            if bool(shift.any()):
-                ids = to_right_padded(ids, shift)
-        ids = ids.contiguous()
+        ids, lens, _ = _right_padded(input_ids.to(self.dev), attention_mask)
         cache.grow(L + new_tokens)
         reuse = cache.reusable(input_ids, images, bboxes, attention_mask)
         ids_h, lens_h = ids.cpu(), lens.cpu()
@@ -490,10 +470,9 @@ class PrefillEngine:
             span = image_tok[b, :int(lens_h[b])].nonzero()
             covered = covered and (len(span) == 0 or int(span.max()) < int(reuse[b]))
         if not covered:
-            seqlens = None if bool((lens_h == L).all()) else lens.to(torch.int32).contiguous()
             images = None if images is None else images.to(self.dev, self.dt).contiguous()
             logits = self.forward_device(ids, images, self.plan_boxes(bboxes), validate=True, last_only=True,
-                                         seqlens=seqlens, cache=cache)
+                                         seqlens=_seqlens(lens, L), cache=cache)
             cache.set_source(images, bboxes)
             return logits
         tl = lens_h - reuse
@@ -512,9 +491,11 @@ class PrefillEngine:
         return self.extend(cache, tail, images, tail_boxes, attention_mask=mask)
 
 
-def _row_boxes(bboxes, b):
-    """Row b's boxes of a per-row box list, or None (bboxes None or empty, as plan_boxes takes them: no boxes)."""
-    return None if bboxes is None or len(bboxes) == 0 else bboxes[b]
+def _row_boxes(bboxes, b, host=False):
+    """Row b's boxes of a per-row box list, or None (bboxes None or empty, as plan_boxes takes them: no boxes).
+    host: as a host fp32 tensor of its own."""
+    row = None if bboxes is None or len(bboxes) == 0 else bboxes[b]
+    return row.detach().to('cpu', torch.float32, copy=True) if host and row is not None else row
 
 
 def right_pad_layout(attention_mask):
@@ -534,6 +515,24 @@ def right_pad_layout(attention_mask):
     return lens, shift
 
 
+def _right_padded(x, attention_mask):
+    """x [B, L, ...] with its 0/1 attention_mask [B, L] (None: every row has L entries) -> (x in the right-padded
+    layout the engine runs on, on x's device and contiguous; lens int64 [B]; shift as right_pad_layout gives it, None
+    when no row is left-padded and x is as given)."""
+    B, L = x.shape[:2]
+    if attention_mask is None:
+        return x.contiguous(), torch.full((B,), L, dtype=torch.int64, device=x.device), None
+    lens, shift = right_pad_layout(attention_mask.to(x.device))
+    if not bool(shift.any()):
+        return x.contiguous(), lens, None
+    return to_right_padded(x, shift), lens, shift
+
+
+def _seqlens(lens, L):
+    """lens int64 [B] -> the int32 seqlens of a prefill, None when every row has all L entries."""
+    return None if bool((lens == L).all()) else lens.to(torch.int32)
+
+
 def _rotate(x, shift):
     B, L = x.shape[:2]
     idx = (torch.arange(L, device=x.device)[None] + shift.to(x.device)[:, None]) % L
@@ -550,7 +549,7 @@ def from_right_padded(x, shift):
     return _rotate(x, (x.shape[1] - shift) % x.shape[1])
 
 
-_DECODE_FUSED = int(__import__('os').environ.get('G4R_DECODE_FUSED', '1'))
+_DECODE_FUSED = int(os.environ.get('G4R_DECODE_FUSED', '1'))
 
 
 class KVCache:
@@ -597,8 +596,7 @@ class KVCache:
     def set_source(self, images, bboxes):
         """Record the images [B, 3, S, S] (None: text-only) and per-row box lists the cached K/V were computed from."""
         self.images = None if images is None else images.detach().clone()
-        self.boxes = [None if _row_boxes(bboxes, b) is None else bboxes[b].detach().to('cpu', torch.float32).clone()
-                      for b in range(self.B)]
+        self.boxes = [_row_boxes(bboxes, b, host=True) for b in range(self.B)]
         self.source_known = True
 
     def row_lens(self):
@@ -638,28 +636,23 @@ class KVCache:
         prefix of the row's tokens (unpadded: attention_mask rows right- or left-padded) equal to the recorded ids,
         cut at the first <bbox> whose box differs from the recorded one, 0 when the row's image differs, and at most
         len - 1 so that at least the last token is computed and gives logits."""
-        B, L = input_ids.shape
+        B = input_ids.shape[0]
         out = torch.zeros(B, dtype=torch.int64)
         if B != self.B or not self.source_known:
             return out
-        ids = input_ids.cpu()
-        if attention_mask is not None:
-            lens, shift = right_pad_layout(attention_mask.cpu())
-        else:
-            lens, shift = torch.full((B,), L, dtype=torch.int64), torch.zeros(B, dtype=torch.int64)
+        ids, lens, _ = _right_padded(input_ids.cpu(), attention_mask)
         held = self.row_lens().cpu()
         rec = self.ids.cpu()
         for b in range(B):
             if not self._same_image(b, images):
                 continue
-            n, s = int(lens[b]), int(shift[b])
-            row = ids[b, s:s + n]
+            n = int(lens[b])
+            row = ids[b, :n]
             m = min(n - 1, int(held[b]))
             diff = (row[:m] != rec[b, :m]).nonzero()
             p = int(diff[0]) if len(diff) else m
             old = self.boxes[b]
-            new = _row_boxes(bboxes, b)
-            new = None if new is None else new.detach().to('cpu', torch.float32)
+            new = _row_boxes(bboxes, b, host=True)
             for k, t in enumerate((row[:p] == self.cfg.bbox_token).nonzero().flatten().tolist()):
                 if old is None or new is None or k >= old.shape[0] or k >= new.shape[0] or not torch.equal(old[k], new[k]):
                     p = t
@@ -675,7 +668,6 @@ def _decode_step(self, token_ids, cache, pos_dev=None):
     position from memory instead of from a launch argument).
     On a cache with per-sample lengths (cache.lens) every kernel takes sample b's position from cache.lens[b], which
     the step advances on the device -- except under graph capture (pos_dev given), where GraphedDecode.step does."""
-    from . import lib
     if cache.length + 1 > cache.max_len:
         raise RuntimeError('KV cache is full (%d)' % cache.max_len)
     # every kernel of the step only READS weights: let each one start in its predecessor's tail and fetch its first
@@ -702,19 +694,13 @@ def _decode_step_chain(self, token_ids, cache, pos_dev):
     # KV-cache append folded into the q|k|v GEMM's RoPE epilogue (7 launches per layer instead of 8).
     # G4R_DECODE_FUSED=0: the unfused sequence, which B > 16 and head_dim != 128 run anyway.
     fuse_step = fused and B <= 16 and c.hidden % 256 == 0 and _DECODE_FUSED > 0
+    swiglu_gemm = dense.decode_gemm if fuse_step else dense.linear
     for li, w in enumerate(self.layers):
+        h = kernels.rmsnorm(x, w['ln_in'], c.rms_eps)
         if fuse_step:
-            h = kernels.rmsnorm(x, w['ln_in'], c.rms_eps)
             qkv = dense.decode_gemm(h, w['wqkv'], rope=(cos, sin, 2 * c.hidden, pos, pos_dev), kv=(cache.k[li], cache.v[li]),
                                     pos_rows=rows)
-            a = _decode_attention(cache, li, qkv, kv_len, scale, pos_dev, rows, anc)
-            x = dense.linear(a, w['wo'], residual=x)
-            h = kernels.rmsnorm(x, w['ln_post'], c.rms_eps)
-            f = dense.decode_gemm(h, w['wgu'], act='swiglu')
-            x = dense.linear(f, w['wdown'], residual=x)
-            continue
-        h = kernels.rmsnorm(x, w['ln_in'], c.rms_eps)
-        if fused:
+        elif fused:
             qkv = dense.qkv_rope(h, w['wqkv'], cos, sin, 1, 2 * c.hidden, pos0=pos, pos_dev=pos_dev, pos_rows=rows)
         else:
             if pos_dev is not None:
@@ -723,11 +709,12 @@ def _decode_step_chain(self, token_ids, cache, pos_dev):
                 raise NotImplementedError('prompts of different lengths need the fused-RoPE QKV GEMM (head_dim 128)')
             qkv = dense.linear(h, w['wqkv'])
             kernels.rope_inplace(qkv, cos[pos:pos + 1].contiguous(), sin[pos:pos + 1].contiguous(), 1, 2 * c.n_heads, c.head_dim)
-        kernels.kv_append(qkv, cache.k[li], cache.v[li], B, 1, pos, pos_dev, pos_rows=rows)
+        if not fuse_step:
+            kernels.kv_append(qkv, cache.k[li], cache.v[li], B, 1, pos, pos_dev, pos_rows=rows)
         a = _decode_attention(cache, li, qkv, kv_len, scale, pos_dev, rows, anc)
         x = dense.linear(a, w['wo'], residual=x)
         h = kernels.rmsnorm(x, w['ln_post'], c.rms_eps)
-        f = dense.linear(h, w['wgu'], act='swiglu')
+        f = swiglu_gemm(h, w['wgu'], act='swiglu')
         x = dense.linear(f, w['wdown'], residual=x)
     cache.length = pos + 1
     if rows is not None and pos_dev is None and anc is None:
@@ -839,16 +826,9 @@ def _generate(self, input_ids, images, bboxes, max_new_tokens=32, do_sample=Fals
         pos0 = cache.row_lens().clone()
     else:
         cache = KVCache(self.cfg, B, L + max_new_tokens, self.dev)
-        plan = self.plan_boxes(bboxes)
-        run_ids, seqlens = ids, None
-        if attention_mask is not None:
-            lens, shift = right_pad_layout(attention_mask.to(self.dev))
-            if bool(shift.any()):
-                run_ids = to_right_padded(ids, shift).contiguous()
-            if not bool((lens == L).all()):
-                seqlens = lens.to(torch.int32).contiguous()
-        logits = self.forward_device(run_ids, images.to(self.dev, self.dt), plan, validate=True, last_only=True,
-                                     seqlens=seqlens, cache=cache)
+        run_ids, lens, _ = _right_padded(ids, attention_mask)
+        logits = self.forward_device(run_ids, images.to(self.dev, self.dt), self.plan_boxes(bboxes), validate=True,
+                                     last_only=True, seqlens=_seqlens(lens, L), cache=cache)
         pos0 = None
     greedy = not (do_sample and temperature > 0)
     rule = pad_token_id is not None and eos_token_id is not None
@@ -887,6 +867,21 @@ def _generate(self, input_ids, images, bboxes, max_new_tokens=32, do_sample=Fals
     return out
 
 
+def _capture(dev, warm, body):
+    """Run warm() on a side stream, wait for the device, then capture body() into a CUDA graph on the current stream.
+    Returns (graph, what body returned: the graph's static outputs)."""
+    side = torch.cuda.Stream(device=dev)
+    side.wait_stream(torch.cuda.current_stream(dev))
+    with torch.cuda.stream(side):
+        warm()
+    torch.cuda.current_stream(dev).wait_stream(side)
+    torch.cuda.synchronize(dev)
+    graph = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(graph):
+        out = body()
+    return graph, out
+
+
 class GraphedDecode:
     """CUDA-graph replay of one decode step: ~260 launches become one.  The current length lives in a
     device int32 that the QKV-RoPE epilogue, kv_append and decode_attention read; `step` bumps it (and the
@@ -901,21 +896,20 @@ class GraphedDecode:
         self.ids = torch.zeros((cache.B, 1), dtype=torch.int64, device=dev)
         self.pos = torch.tensor([cache.length], dtype=torch.int32, device=dev)
         start = cache.length
-        side = torch.cuda.Stream(device=dev)
-        side.wait_stream(torch.cuda.current_stream(dev))
-        with torch.cuda.stream(side):
-            for _ in range(2):  # warm-up (writes slot `start`, overwritten by the first real step)
+
+        def warm():
+            for _ in range(2):  # writes slot `start`, overwritten by the first real step
                 logits = engine.decode_step(self.ids, cache, self.pos)
                 cache.length = start
             if sampler is not None:   # into a scratch buffer, `finished` untouched
                 sampler(logits, torch.empty_like(self.ids), update=False)
-        torch.cuda.current_stream(dev).wait_stream(side)
-        torch.cuda.synchronize(dev)
-        self.graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(self.graph):
-            self.logits = engine.decode_step(self.ids, cache, self.pos)
+
+        def body():
+            logits = engine.decode_step(self.ids, cache, self.pos)
             if sampler is not None:
-                sampler(self.logits, self.ids)
+                sampler(logits, self.ids)
+            return logits
+        self.graph, self.logits = _capture(dev, warm, body)
         cache.length = start
 
     def step(self, token_ids=None):
@@ -1026,18 +1020,17 @@ class GraphedBeamDecode:
         dev = engine.dev
         self.pos = torch.tensor([cache.length], dtype=torch.int32, device=dev)   # sizes the step by max_len
         start = cache.length
-        side = torch.cuda.Stream(device=dev)
-        side.wait_stream(torch.cuda.current_stream(dev))
-        with torch.cuda.stream(side):
-            for _ in range(2):  # warm-up (writes each beam row's current position, rewritten by the first real step)
+
+        def warm():
+            for _ in range(2):  # writes each beam row's current position, rewritten by the first real step
                 engine.decode_step(cache.ids, cache, self.pos)
                 cache.length = start
-        torch.cuda.current_stream(dev).wait_stream(side)
-        torch.cuda.synchronize(dev)
-        self.graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(self.graph):
-            self.logits = engine.decode_step(cache.ids, cache, self.pos)
-            cache.step(self.logits)
+
+        def body():
+            logits = engine.decode_step(cache.ids, cache, self.pos)
+            cache.step(logits)
+            return logits
+        self.graph, self.logits = _capture(dev, warm, body)
         cache.length = start
 
     def step(self):
@@ -1062,17 +1055,10 @@ def _generate_beams(self, input_ids, images, bboxes, max_new_tokens, num_beams, 
     fill = (pad_token_id or eos[0]) if eos else -1        # HF's output_fill_value
     ids = input_ids.to(self.dev)
     cache = BeamCache(self.cfg, B, N, L, max_new_tokens, self.dev, eos, length_penalty, early_stopping, fill)
-    plan = self.plan_boxes(bboxes)
-    run_ids, seqlens = ids, None
-    lens = torch.full((B,), L, dtype=torch.int32, device=self.dev)
-    if attention_mask is not None:
-        lens, shift = right_pad_layout(attention_mask.to(self.dev))
-        if bool(shift.any()):
-            run_ids = to_right_padded(ids, shift).contiguous()
-        if not bool((lens == L).all()):
-            seqlens = lens.to(torch.int32).contiguous()
-    logits = self.forward_device(run_ids.contiguous(), None if images is None else images.to(self.dev, self.dt), plan,
-                                 validate=True, last_only=True, seqlens=seqlens, cache=cache.prompt)
+    run_ids, lens, _ = _right_padded(ids, attention_mask)
+    logits = self.forward_device(run_ids, None if images is None else images.to(self.dev, self.dt),
+                                 self.plan_boxes(bboxes), validate=True, last_only=True, seqlens=_seqlens(lens, L),
+                                 cache=cache.prompt)
     cache.start(lens)
     cache.step(logits, first=True)
     stepper = None
@@ -1104,16 +1090,14 @@ class GraphedPrefill:
         self.images = images.to(dev, engine.dt).clone()
         self.plan = engine.plan_boxes(bboxes)
         self.counts = None if bboxes is None else [0 if b is None else int(b.shape[0]) for b in bboxes]
-        side = torch.cuda.Stream(device=dev)
-        side.wait_stream(torch.cuda.current_stream(dev))
-        with torch.cuda.stream(side):
-            engine.forward_device(self.ids, self.images, self.plan, validate=True, last_only=last_only)  # warm-up + validation
-            engine.forward_device(self.ids, self.images, self.plan, validate=False, last_only=last_only)
-        torch.cuda.current_stream(dev).wait_stream(side)
-        torch.cuda.synchronize(dev)
-        self.graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(self.graph):
-            self.out = engine.forward_device(self.ids, self.images, self.plan, validate=False, last_only=last_only)
+
+        def body(validate=False):
+            return engine.forward_device(self.ids, self.images, self.plan, validate=validate, last_only=last_only)
+
+        def warm():
+            body(validate=True)   # validation runs here only: it reads a status word back, which a capture cannot
+            body()
+        self.graph, self.out = _capture(dev, warm, body)
 
     def run(self, input_ids, images, bboxes):
         self.ids.copy_(input_ids, non_blocking=True)

@@ -1,5 +1,8 @@
 """Torch-tensor front-ends of the elementwise / attention entry points of the C ABI
 (csrc/elementwise.cu, csrc/attention.cu).  No computation happens in Python."""
+import ctypes
+import os
+
 import torch
 
 from . import lib as _L
@@ -52,7 +55,6 @@ def cast_tokens_f32_bf16(hidden, skip_first=1, dtype=torch.bfloat16):
     """hidden fp32 [B,T,C] -> dense 16-bit [B*(T-skip_first), C] (drops the CLS row)."""
     B, T, C = hidden.shape
     out = torch.empty((B * (T - skip_first), C), dtype=dtype, device=hidden.device)
-    import ctypes
     src = ctypes.c_void_p(hidden.data_ptr() + skip_first * C * 4)
     _call('g4r_cast_f32_bf16', hidden.device, src, C, T * C, _L.ptr(out), B, T - skip_first, C, act=dtype)
     return out
@@ -79,7 +81,7 @@ def rope_inplace(qkv, cos, sin, L, n_heads_qk, head_dim):
     return qkv
 
 
-ATTN_IMPL = __import__('os').environ.get('G4R_ATTN', 'tc')  # 'tc' = wgmma kernel, 'mma' = mma.sync kernel
+ATTN_IMPL = os.environ.get('G4R_ATTN', 'tc')  # 'tc' = wgmma kernel, 'mma' = mma.sync kernel
 
 
 def attention(qkv, B, L, n_heads, head_dim, causal, scale, out=None, seqlens=None, impl=None):
@@ -91,7 +93,6 @@ def attention(qkv, B, L, n_heads, head_dim, causal, scale, out=None, seqlens=Non
     ld = qkv.stride(0)
     esz = 2
     base = qkv.data_ptr()
-    import ctypes
     q, k, v = (ctypes.c_void_p(base + i * hd * esz) for i in range(3))
     fn = 'g4r_attention_tc_bf16' if (impl or ATTN_IMPL) == 'tc' else 'g4r_attention_bf16'
     _call(fn, qkv.device, q, k, v, _L.ptr(out), ld, L * ld, out.stride(0), L * out.stride(0),
@@ -109,7 +110,7 @@ def attention_cached(qkv, kcache, vcache, B, n_heads, head_dim, Lc, scale, start
     out = torch.empty((B * Lc, hd), dtype=act, device=qkv.device)
     _call('g4r_attention_cached_bf16', qkv.device, _L.ptr(qkv), qkv.stride(0), _L.ptr(kcache), _L.ptr(vcache),
           kcache.shape[1], _L.ptr(out), out.stride(0), B, n_heads, Lc, head_dim, float(scale),
-          _L.ptr(_pos_rows(start, B)), None if qlen is None else _L.ptr(_pos_rows(qlen, B)), act=act)
+          _L.ptr(_L.require_pos_rows(start, B)), None if qlen is None else _L.ptr(_L.require_pos_rows(qlen, B)), act=act)
     return out
 
 
@@ -140,7 +141,6 @@ def upsample_tokens_coords(hidden, G, Ho, cpad, has_cls=True, dtype=None):
                            % (G * G + skip, tuple(hidden.shape), hidden.dtype))
     act = hidden.dtype if hidden.dtype != torch.float32 else (dtype or torch.bfloat16)
     out = torch.empty((B, Ho, Ho, cpad), dtype=act, device=hidden.device)
-    import ctypes
     f32 = hidden.dtype == torch.float32
     tok = ctypes.c_void_p(hidden.data_ptr() + skip * C * (4 if f32 else 2))  # skip CLS
     _call('g4r_upsample_tokens_coords_f32' if f32 else 'g4r_upsample_tokens_coords_bf16', hidden.device, tok, C,
@@ -204,6 +204,14 @@ def add_bias_pos_cast(acc, bias, pos):
     return out
 
 
+def _logit_rows(name, logits):
+    """16-bit logits [rows, V] or [rows, 1, V] -> ([rows, V] with unit column stride, their 16-bit type)."""
+    rows = logits.reshape(logits.shape[0], logits.shape[-1]) if logits.dim() == 3 else logits
+    if rows.stride(1) != 1:
+        raise RuntimeError('%s: logits rows must have unit column stride' % name)
+    return rows, _bf16(rows)
+
+
 def sample_tokens(logits, out, greedy, temperature=1.0, top_k=0, top_p=1.0, seed=0, rng_step=None, eos_id=-1,
                   pad_id=-1, finished=None):
     """Next token of every row of 16-bit logits [B, V] (or [B, 1, V]; unit column stride) into out (int64, B contiguous
@@ -211,11 +219,8 @@ def sample_tokens(logits, out, greedy, temperature=1.0, top_k=0, top_p=1.0, seed
     top-k / top-p processed softmax with Philox key `seed` and counter (*rng_step, row) -- rng_step: device int64 [1].
     top_k 0 / top_p 1 switch that filter off.  finished (device int32 [B]) with eos_id, pad_id >= 0: transformers'
     eos -> pad rule, updated in place."""
-    rows = logits.reshape(logits.shape[0], logits.shape[-1]) if logits.dim() == 3 else logits
-    act = _bf16(rows)
+    rows, act = _logit_rows('sample_tokens', logits)
     B, V = rows.shape
-    if rows.stride(1) != 1:
-        raise RuntimeError('sample_tokens: logits rows must have unit column stride')
     if out.dtype != torch.int64 or out.numel() != B or not out.is_contiguous():
         raise RuntimeError('sample_tokens: out must be a contiguous int64 tensor of %d elements' % B)
     if rng_step is not None and (rng_step.dtype != torch.int64 or rng_step.numel() != 1):
@@ -229,12 +234,6 @@ def sample_tokens(logits, out, greedy, temperature=1.0, top_k=0, top_p=1.0, seed
     return out
 
 
-def _pos_rows(pos_rows, B):
-    if pos_rows.dtype != torch.int32 or tuple(pos_rows.shape) != (B,) or not pos_rows.is_contiguous():
-        raise RuntimeError('pos_rows must be a contiguous device int32 [%d] vector' % B)
-    return pos_rows
-
-
 def kv_append(qkv, kcache, vcache, B, Ln, pos0, pos_dev=None, pos_rows=None):
     """Copy the k|v parts of packed qkv rows [B*Ln, 3*HD] into caches [B, Lmax, HD] at pos0..pos0+Ln-1.
     pos_rows: device int32 [B] -- sample b's rows go to pos_rows[b]..pos_rows[b]+Ln-1 instead (pos0 / pos_dev unused)."""
@@ -242,7 +241,7 @@ def kv_append(qkv, kcache, vcache, B, Ln, pos0, pos_dev=None, pos_rows=None):
     act = _bf16(qkv, kcache, vcache)
     if pos_rows is not None:
         _call('g4r_kv_append_rows_bf16', qkv.device, _L.ptr(qkv), qkv.stride(0), _L.ptr(kcache), _L.ptr(vcache), B, Ln,
-              _L.ptr(_pos_rows(pos_rows, B)), kcache.shape[1], HD, act=act)
+              _L.ptr(_L.require_pos_rows(pos_rows, B)), kcache.shape[1], HD, act=act)
         return
     _call('g4r_kv_append_bf16', qkv.device, _L.ptr(qkv), qkv.stride(0), _L.ptr(kcache), _L.ptr(vcache), B, Ln,
           int(pos0), _L.ptr(pos_dev), kcache.shape[1], HD, act=act)
@@ -256,7 +255,7 @@ def decode_attention(qkv, kcache, vcache, B, n_heads, head_dim, kv_len, scale, p
     out = torch.empty((B, n_heads * head_dim), dtype=act, device=qkv.device)
     if pos_rows is not None:
         _call('g4r_decode_attention_rows_bf16', qkv.device, _L.ptr(qkv), qkv.stride(0), _L.ptr(kcache), _L.ptr(vcache),
-              _L.ptr(out), out.stride(0), B, n_heads, head_dim, int(kv_len), _L.ptr(_pos_rows(pos_rows, B)),
+              _L.ptr(out), out.stride(0), B, n_heads, head_dim, int(kv_len), _L.ptr(_L.require_pos_rows(pos_rows, B)),
               kcache.shape[1], float(scale), act=act)
         return out
     _call('g4r_decode_attention_bf16', qkv.device, _L.ptr(qkv), qkv.stride(0), _L.ptr(kcache), _L.ptr(vcache),
@@ -275,20 +274,19 @@ def decode_attention_beam(qkv, kcache, vcache, R, n_heads, head_dim, kv_bound, s
         raise RuntimeError('decode_attention_beam: anc must be a contiguous device int32 [%d, %d] table' % (R, Lmax))
     out = torch.empty((R, n_heads * head_dim), dtype=act, device=qkv.device)
     _call('g4r_decode_attention_beam_bf16', qkv.device, _L.ptr(qkv), qkv.stride(0), _L.ptr(kcache), _L.ptr(vcache),
-          _L.ptr(out), out.stride(0), R, n_heads, head_dim, int(kv_bound), _L.ptr(_pos_rows(pos_rows, R)), _L.ptr(anc),
-          Lmax, float(scale), act=act)
+          _L.ptr(out), out.stride(0), R, n_heads, head_dim, int(kv_bound), _L.ptr(_L.require_pos_rows(pos_rows, R)),
+          _L.ptr(anc), Lmax, float(scale), act=act)
     return out
 
 
 def beam_step(logits, row_div, st):
     """One beam-search step (csrc/beam.cu) on 16-bit logits [rows, V] (or [rows, 1, V]; unit column stride) with the
     device state of st (engine.BeamCache): B*N rows, or B with row_div = N (the first step, from the prefill)."""
-    rows = logits.reshape(logits.shape[0], logits.shape[-1]) if logits.dim() == 3 else logits
-    act = _bf16(rows)
+    rows, act = _logit_rows('beam_step', logits)
     V = rows.shape[1]
     B, N = st.n_samples, st.N
-    if rows.stride(1) != 1 or rows.shape[0] * row_div != B * N:
-        raise RuntimeError('beam_step: logits must be [%d, V] rows with unit column stride' % (B * N // row_div))
+    if rows.shape[0] * row_div != B * N:
+        raise RuntimeError('beam_step: logits must be [%d, V] rows' % (B * N // row_div))
     _L.require_cuda_same_device([('logits', rows), ('state', st.state), ('anc', st.anc)])
     _call('g4r_beam_step_bf16', rows.device, _L.ptr(rows), rows.stride(0), int(row_div), B, N, V, st.K,
           _L.ptr(st.eos), st.n_eos, st.prompt_len, st.max_length, float(st.length_penalty), st.early, st.G, st.Lmax,

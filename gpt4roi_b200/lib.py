@@ -236,6 +236,13 @@ def require_contiguous(named):
                                'data_ptr memory, roi_align_cuda.cu:21-23)' % name)
 
 
+def require_pos_rows(pos_rows, n):
+    """Per-sample positions (or lengths) as the `_rows` entry points read them: a contiguous int32 [n] vector."""
+    if pos_rows.dtype != torch.int32 or tuple(pos_rows.shape) != (n,) or not pos_rows.is_contiguous():
+        raise RuntimeError('pos_rows must be a contiguous device int32 [%d] vector' % n)
+    return pos_rows
+
+
 def ptr(t):
     return None if t is None else ctypes.c_void_p(t.data_ptr())
 

@@ -35,8 +35,7 @@ import torch.nn as nn
 from transformers import LlamaConfig, LlamaForCausalLM, LlamaModel
 from transformers.modeling_outputs import BaseModelOutputWithPast, CausalLMOutputWithPast
 
-from .engine import (BF16, EngineConfig, KVCache, PrefillEngine, from_right_padded, right_pad_layout,
-                     to_right_padded)
+from .engine import BF16, EngineConfig, KVCache, PrefillEngine, _right_padded, from_right_padded, right_pad_layout
 from .roi_align import RoIAlign
 
 DEFAULT_IMAGE_PATCH_TOKEN = '<im_patch>'
@@ -451,15 +450,10 @@ def _run_engine(eng, input_ids, images, bboxes, attention_mask, past_key_values,
         B, L = inputs_embeds.shape[:2]
         x = inputs_embeds.to(eng.dev, eng.dt)
         seqlens = _seqlens(eng, attention_mask, L)
-        shift = None
-        if seqlens is not None:
-            _, shift = right_pad_layout(attention_mask.to(eng.dev))
-            shift = shift if bool(shift.any()) else None
-            if shift is not None:
-                x = to_right_padded(x, shift)
+        x, _, shift = _right_padded(x, attention_mask if seqlens is not None else None)
         if kv is not None:
             kv.start(L, seqlens)
-        out = eng.llama(x.contiguous(), B, L, seqlens=seqlens, cache=kv, want=want, last_only=last_only)
+        out = eng.llama(x, B, L, seqlens=seqlens, cache=kv, want=want, last_only=last_only)
         if shift is not None and not last_only:
             out = from_right_padded(out, shift)
         return out, new_cache
