@@ -15,6 +15,7 @@ ONCE at load time (fused QKV, interleaved gate/up, NHWC conv filters, flatten_li
 from (c,ph,pw) to (ph,pw,c)).  Numerics: bf16 storage, fp32 accumulation, rounding points of the
 reference under bf16 autocast.
 """
+import collections
 import math
 import os
 
@@ -734,14 +735,154 @@ def _decode_attention(cache, li, qkv, kv_len, scale, pos_dev, rows, anc):
                                          kv_len, scale, rows, anc)
 
 
+STOP_TABLE_MAX_BYTES = 64 << 20
+_STOP_TABLES = collections.OrderedDict()   # (token strings, stop strings, stop token ids) -> host table; the last 8 used
+
+
+def _stop_lookup(table, tokens, state):
+    """kernels.stop_step's lookup with torch indexing: tokens, state int64 [n] -> (new state int64 [n], hit bool [n])."""
+    V = table.shape[0] - 1
+    e = table[torch.where((tokens < 0) | (tokens > V), V, tokens), state].to(torch.int64)
+    return e & 0x7FFF, e < 0
+
+
+class StopStrings:
+    """The stop strings of a generate call as a lookup table (transformers' StopStringCriteria as a state machine): a
+    row stops at the first generated token in which an occurrence of a stop string ends, in the concatenation of the
+    tokens' strings -- the occurrence may begin in earlier tokens and the last token may run past its end.
+
+    token_strings: the string every token id stands for (StopStringCriteria.clean_tokenizer_vocab), a list indexed by
+    id, None for ids the vocabulary does not hold.  stop_token_ids: ids that stop a row by themselves
+    (KeywordsStoppingCriteria.keyword_ids).
+
+    The matcher is the Aho-Corasick automaton of the stop strings over their own characters plus one class for every
+    other character: states = trie nodes (S <= 1 + sum of the lengths), failure links and output sets folded into a
+    dense transition table.  `table` (host int16 [V_tok + 1, S]) composes it with the tokens: entry (t, s) is the
+    state after token t's string is fed from state s, bit 15 set when an accepting state was entered on the way.  An id
+    the vocabulary does not hold, and the last row (where ids >= V_tok go), sends every state to the root without a hit,
+    as HF's matcher breaks a match there.  An empty string leaves the state as it is, as HF's does -- with one
+    difference: HF looks at the last max(len(stop)) tokens only, so a match that empty-string tokens stretch over more
+    tokens than that is found here and missed there.
+    kernels.stop_step walks the table on the device (Sampler); initial_states() gives each row's state after its
+    prompt."""
+
+    def __init__(self, token_strings, stop_strings, stop_token_ids=()):
+        stops = (stop_strings,) if isinstance(stop_strings, str) else tuple(stop_strings)
+        if not stops:
+            raise ValueError('stop_strings: no stop string given')
+        if not all(isinstance(s, str) and s for s in stops):
+            raise ValueError('stop_strings: every stop string must be a non-empty str, got %r' % (stops,))
+        self.stop_strings = stops
+        self.max_len = max(len(s) for s in stops)
+        self.V_tok = len(token_strings)
+        key = (tuple(token_strings), stops, tuple(int(t) for t in stop_token_ids))
+        if key in _STOP_TABLES:
+            _STOP_TABLES.move_to_end(key)
+        else:
+            _STOP_TABLES[key] = self._build(*key)
+            if len(_STOP_TABLES) > 8:
+                _STOP_TABLES.popitem(last=False)
+        self.table = _STOP_TABLES[key]
+        self.S = self.table.shape[1]
+        self._device = {}
+
+    @staticmethod
+    def _automaton(stops):
+        """-> (delta int64 [S, A], accept bool [S], code: character -> column of delta; column 0: any other character)."""
+        code = {ch: i + 1 for i, ch in enumerate(sorted(set(''.join(stops))))}
+        goto, accept = [{}], [False]
+        for s in stops:
+            n = 0
+            for ch in s:
+                if code[ch] not in goto[n]:
+                    goto[n][code[ch]] = len(goto)
+                    goto.append({})
+                    accept.append(False)
+                n = goto[n][code[ch]]
+            accept[n] = True
+        S, A = len(goto), len(code) + 1
+        delta = torch.zeros((S, A), dtype=torch.int64)
+        fail = [0] * S
+        order = [0]
+        for n in order:                          # breadth first: a node's failure state is finished before the node
+            accept[n] = accept[n] or accept[fail[n]]
+            delta[n] = delta[fail[n]] if n else 0
+            for c, m in goto[n].items():
+                fail[m] = int(delta[fail[n], c]) if n else 0
+                delta[n, c] = m
+                order.append(m)
+        return delta, torch.tensor(accept), code
+
+    @classmethod
+    def _build(cls, token_strings, stops, stop_token_ids):
+        V = len(token_strings)
+        delta, accept, code = cls._automaton(stops)
+        S = delta.shape[0]
+        if V == 0 or S > 32767 or S * (V + 1) * 2 > STOP_TABLE_MAX_BYTES:
+            raise ValueError('stop_strings: %d matcher states x %d tokens need a %d-byte table; the limit is %d bytes '
+                             'and 32767 states' % (S, V, S * (V + 1) * 2, STOP_TABLE_MAX_BYTES))
+        known = torch.tensor([t is not None for t in token_strings])
+        lens = torch.tensor([len(t or '') for t in token_strings])
+        chars = torch.zeros((V, max(int(lens.max()), 1)), dtype=torch.int64)
+        for i, t in enumerate(token_strings):
+            if t and any(ch in code for ch in t):
+                chars[i, :len(t)] = torch.tensor([code.get(ch, 0) for ch in t])
+        cur = torch.arange(S).repeat(V, 1)
+        hit = torch.zeros((V, S), dtype=torch.bool)
+        for p in range(chars.shape[1]):          # all (token, state) pairs at once, one character position per pass
+            live = (lens > p)[:, None]
+            nxt = delta[cur, chars[:, p, None]]
+            cur = torch.where(live, nxt, cur)
+            hit |= live & accept[nxt]
+        if not bool(hit.any()):                  # StopStringCriteria refuses the same
+            raise ValueError('stop_strings: no token of the vocabulary can end any of %r (characters the vocabulary '
+                             'does not hold?)' % (stops,))
+        cur[~known] = 0
+        for t in stop_token_ids:
+            if not 0 <= t < V:
+                raise ValueError('stop_token_ids: %d is outside the vocabulary (%d tokens)' % (t, V))
+            cur[t], hit[t] = 0, True
+        table = torch.zeros((V + 1, S), dtype=torch.int16)
+        table[:V] = (cur - 32768 * hit.to(torch.int64)).to(torch.int16)
+        return table
+
+    def on(self, device):
+        """The table on `device` (copied once per device)."""
+        device = torch.device(device)
+        if device.type == 'cpu':
+            return self.table
+        if device not in self._device:
+            self._device[device] = self.table.to(device)
+        return self._device[device]
+
+    def advance(self, tokens, state):
+        """One lookup on the host: tokens, state int64 [n] -> (new state int64 [n], hit bool [n])."""
+        return _stop_lookup(self.table, tokens, state)
+
+    def initial_states(self, ids, lens):
+        """Each row's state after its prompt, int32 [B] on the host: the table walked (hits ignored) over the last
+        max(len(stop)) of the row's lens[b] tokens, ids[b, :lens[b]] -- which is what lets a stop string begin in the
+        prompt and end in the answer."""
+        ids, lens = ids.cpu(), lens.cpu().to(torch.int64)
+        state = torch.zeros(ids.shape[0], dtype=torch.int64)
+        for k in range(self.max_len, 0, -1):
+            col = lens - k
+            new, _ = self.advance(ids.gather(1, col.clamp(min=0)[:, None])[:, 0], state)
+            state = torch.where(col >= 0, new, state)
+        return state.to(torch.int32)
+
+
 class Sampler:
     """Next-token selection of the decode loop (kernels.sample_tokens): arg-max, or a draw from the temperature /
     top-k / top-p processed softmax, with transformers' eos -> pad rule when eos_id and pad_id are both given.
     Its per-step state lives on the device, so a CUDA graph can capture the call: `rng_step` (int64 [1], the Philox
-    counter, advanced once per selected token) and `finished` (int32 [B], the rows that have emitted eos_id)."""
+    counter, advanced once per selected token) and `finished` (int32 [B], the rows that have emitted eos_id).
+    stops (a StopStrings, with stop_state: each row's state after its prompt, int32 [B]): every call then ends with
+    kernels.stop_step on the tokens just selected, which keeps the rows' matcher states in `stop_state` and sets
+    `finished` for a row whose token ends a stop string."""
 
     def __init__(self, B, device, greedy=True, temperature=1.0, top_k=None, top_p=None, seed=0, eos_id=None,
-                 pad_id=None):
+                 pad_id=None, stops=None, stop_state=None):
         self.greedy = bool(greedy)
         self.temperature = float(temperature)
         self.top_k = 0 if top_k is None else int(top_k)
@@ -751,13 +892,21 @@ class Sampler:
         self.eos_id, self.pad_id = (int(eos_id), int(pad_id)) if rule else (-1, -1)
         self.rng_step = torch.zeros(1, dtype=torch.int64, device=device)
         self.finished = torch.zeros(B, dtype=torch.int32, device=device)
+        self.stop_table = None if stops is None else stops.on(device)
+        if stops is not None:
+            self.stop_state = torch.zeros_like(self.finished) if stop_state is None else stop_state.to(device, torch.int32)
 
     def __call__(self, logits, out, update=True):
-        """Select from logits [B, 1, V] into out (int64 [B, 1]).  update=False leaves `finished` alone (warm-up)."""
+        """Select from logits [B, 1, V] into out (int64 [B, 1]).  update=False leaves `finished` and `stop_state` alone
+        (warm-up: the stop-string lookup then runs on copies, so that a graph capture is not its first launch)."""
         if not logits.is_cuda:
             return self._host(logits, out, update)
-        return kernels.sample_tokens(logits, out, self.greedy, self.temperature, self.top_k, self.top_p, self.seed,
-                                     self.rng_step, self.eos_id, self.pad_id, self.finished if update else None)
+        kernels.sample_tokens(logits, out, self.greedy, self.temperature, self.top_k, self.top_p, self.seed,
+                              self.rng_step, self.eos_id, self.pad_id, self.finished if update else None)
+        if self.stop_table is not None:
+            state, finished = (self.stop_state, self.finished) if update else (self.stop_state.clone(), self.finished.clone())
+            kernels.stop_step(out, self.stop_table, state, finished)
+        return out
 
     def _host(self, logits, out, update):
         """Host tensors come only from CPU stand-ins of the engine (the loop's host-side tests): the arg-max and the
@@ -769,6 +918,11 @@ class Sampler:
         if update and self.eos_id >= 0:
             tok = torch.where(self.finished.bool(), torch.full_like(tok, self.pad_id), tok)
             self.finished |= (tok == self.eos_id).to(torch.int32)
+        if update and self.stop_table is not None:
+            live = self.finished == 0
+            state, hit = _stop_lookup(self.stop_table, tok, self.stop_state.to(torch.int64))
+            self.stop_state = torch.where(live, state.to(torch.int32), self.stop_state)
+            self.finished |= (live & hit).to(torch.int32)
         out.copy_(tok.view(out.shape))
         return out
 
@@ -787,7 +941,7 @@ def sampling_seed(generator=None):
 def _generate(self, input_ids, images, bboxes, max_new_tokens=32, do_sample=False, temperature=1.0,
               stopping_criteria=None, eos_token_id=None, generator=None, use_graph=True, attention_mask=None,
               pad_token_id=None, cache=None, top_k=None, top_p=None, num_beams=1, length_penalty=1.0,
-              early_stopping=False, num_return_sequences=1):
+              early_stopping=False, num_return_sequences=1, stop_strings=None):
     """Prefill + greedy / sampled decode (gpt4roi/app.py:286-300 calls
     model.generate(input_ids, images=..., do_sample=True, temperature=0.2, max_new_tokens=1024,
     stopping_criteria=[...]) with the boxes bound to forward).  Returns ids [B, L + new]: the prompt as given,
@@ -805,6 +959,11 @@ def _generate(self, input_ids, images, bboxes, max_new_tokens=32, do_sample=Fals
     conversation every turn): the prefix it already holds is reused and only the rest is prefilled (prefill_cached);
     afterwards it holds the conversation including this turn's answer (the last new token excepted), ready for the next.
     Rows that finished with pad_token_id keep those pads in the recorded ids, so the next turn's reuse stops there.
+    stop_strings: a StopStrings -- transformers' generate(stop_strings=...), matched on the device per row: a row is
+    finished at the first new token in which a stop string ends (it may begin in the row's prompt), that token is part
+    of the output, and the loop ends once every row is finished.  As in HF, finished rows are filled with pad_token_id
+    only when eos_token_id and pad_token_id are both given; otherwise they keep generating until the last row stops.
+    Host stopping_criteria callbacks may be given as well.
     num_beams > 1: deterministic beam search (transformers' GenerationMixin._beam_search, do_sample=False) with
     length_penalty, early_stopping (True, False or "never") and num_return_sequences <= num_beams; eos_token_id may be
     a list.  The prompt is prefilled once per sample and the beams share its KV cache (BeamCache).  Returns
@@ -814,6 +973,8 @@ def _generate(self, input_ids, images, bboxes, max_new_tokens=32, do_sample=Fals
             raise NotImplementedError('beam search with do_sample runs on the HF loop only: pass use_hf_loop=True')
         if stopping_criteria is not None:
             raise NotImplementedError('beam search with stopping_criteria runs on the HF loop only: pass use_hf_loop=True')
+        if stop_strings is not None:
+            raise NotImplementedError('beam search with stop_strings runs on the HF loop only: pass use_hf_loop=True')
         if cache is not None:
             raise NotImplementedError('beam search on a conversation cache (cache=) runs on the HF loop only: pass '
                                       'use_hf_loop=True')
@@ -832,8 +993,11 @@ def _generate(self, input_ids, images, bboxes, max_new_tokens=32, do_sample=Fals
         pos0 = None
     greedy = not (do_sample and temperature > 0)
     rule = pad_token_id is not None and eos_token_id is not None
+    stop_state = None
+    if stop_strings is not None:     # the submitted prompt's tokens, also on a conversation cache
+        stop_state = stop_strings.initial_states(*_right_padded(input_ids.cpu(), attention_mask)[:2])
     sampler = Sampler(B, self.dev, greedy, temperature, top_k, top_p, seed=0 if greedy else sampling_seed(generator),
-                      eos_id=eos_token_id, pad_id=pad_token_id)
+                      eos_id=eos_token_id, pad_id=pad_token_id, stops=stop_strings, stop_state=stop_state)
     out = torch.empty((B, L + max_new_tokens), dtype=torch.int64, device=self.dev)
     out[:, :L] = ids
     stepper = None
@@ -846,10 +1010,9 @@ def _generate(self, input_ids, images, bboxes, max_new_tokens=32, do_sample=Fals
     for step in range(max_new_tokens):
         out[:, L + step:L + step + 1].copy_(tok)
         n = step + 1
-        if rule:
-            if bool(sampler.finished.all()):
-                break
-        elif eos_token_id is not None and bool((tok == eos_token_id).all()):
+        if (rule or stop_strings is not None) and bool(sampler.finished.all()):
+            break
+        if not rule and eos_token_id is not None and bool((tok == eos_token_id).all()):
             break
         if stopping_criteria is not None and any(bool(torch.as_tensor(sc(out[:, :L + n], logits[:, -1].float())).all())
                                                  for sc in stopping_criteria):

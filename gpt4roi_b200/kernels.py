@@ -234,6 +234,25 @@ def sample_tokens(logits, out, greedy, temperature=1.0, top_k=0, top_p=1.0, seed
     return out
 
 
+def stop_step(ids, table, state, finished):
+    """Stop strings, one step: every row b with finished[b] == 0 advances its matcher state by the token ids[b] through
+    table (int16 [V_tok + 1, S], engine.StopStrings) and sets finished[b] when an occurrence of a stop string ended in
+    that token.  ids: int64, B contiguous elements (the decode step's ids buffer, after sample_tokens); state, finished:
+    contiguous device int32 [B], updated in place."""
+    B = ids.numel()
+    if ids.dtype != torch.int64 or not ids.is_contiguous():
+        raise RuntimeError('stop_step: ids must be a contiguous int64 tensor')
+    if table.dtype != torch.int16 or table.dim() != 2 or table.stride(1) != 1 or table.shape[0] < 2:
+        raise RuntimeError('stop_step: table must be an int16 [V_tok + 1, S] tensor with unit column stride')
+    for name, t in (('state', state), ('finished', finished)):
+        if t.dtype != torch.int32 or t.numel() != B or not t.is_contiguous():
+            raise RuntimeError('stop_step: %s must be a contiguous device int32 [%d] vector' % (name, B))
+    _L.require_cuda_same_device([('ids', ids), ('table', table), ('state', state), ('finished', finished)])
+    _call('g4r_stop_step', ids.device, _L.ptr(ids), _L.ptr(table), table.stride(0), table.shape[0] - 1, table.shape[1],
+          B, _L.ptr(state), _L.ptr(finished))
+    return finished
+
+
 def kv_append(qkv, kcache, vcache, B, Ln, pos0, pos_dev=None, pos_rows=None):
     """Copy the k|v parts of packed qkv rows [B*Ln, 3*HD] into caches [B, Lmax, HD] at pos0..pos0+Ln-1.
     pos_rows: device int32 [B] -- sample b's rows go to pos_rows[b]..pos_rows[b]+Ln-1 instead (pos0 / pos_dev unused)."""

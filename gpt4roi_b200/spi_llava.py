@@ -27,6 +27,7 @@ id changes) which launches the hand-written kernels.
 
 Anything outside this (output_attentions, left padding, list-of-images) raises instead of falling back.
 """
+import collections
 import weakref
 from typing import List, Optional
 
@@ -35,7 +36,8 @@ import torch.nn as nn
 from transformers import LlamaConfig, LlamaForCausalLM, LlamaModel
 from transformers.modeling_outputs import BaseModelOutputWithPast, CausalLMOutputWithPast
 
-from .engine import BF16, EngineConfig, KVCache, PrefillEngine, _right_padded, from_right_padded, right_pad_layout
+from .engine import (BF16, EngineConfig, KVCache, PrefillEngine, StopStrings, _right_padded, from_right_padded,
+                     right_pad_layout)
 from .roi_align import RoIAlign
 
 DEFAULT_IMAGE_PATCH_TOKEN = '<im_patch>'
@@ -486,6 +488,22 @@ class _TrainStepFn(torch.autograd.Function):
         return (None,) * 6 + out
 
 
+def _generation_config(model, given):
+    """The generation config of a generate call as transformers resolves it (GenerationMixin._prepare_generation_config:
+    the explicit kwargs `given`, then its `generation_config` entry, then model.generation_config, then HF's defaults),
+    special tokens prepared."""
+    from transformers.utils import logging as hf_logging
+    given = dict(given)
+    verbosity = hf_logging.get_verbosity()
+    hf_logging.set_verbosity_error()     # HF's notes on flags and pad tokens belong to its own loop
+    try:
+        gc, _ = model._prepare_generation_config(given.pop('generation_config', None), **given)
+        model._prepare_special_tokens(gc, True, 'cpu')
+    finally:
+        hf_logging.set_verbosity(verbosity)
+    return gc
+
+
 def resolve_sampling(model, input_len, do_sample=None, temperature=None, **kwargs):
     """The engine loop's selection rule for a generate call, resolved as transformers resolves it: explicit kwargs, then
     `generation_config=`, then model.generation_config, then HF's global defaults (GenerationMixin.
@@ -495,15 +513,8 @@ def resolve_sampling(model, input_len, do_sample=None, temperature=None, **kwarg
     min_p, typical_p, no_repeat_ngram_size, a caller's logits_processor, ...), or run beam search, raises
     NotImplementedError: the engine loop does not implement it, the HF loop (use_hf_loop=True) does."""
     from transformers.generation.logits_process import TemperatureLogitsWarper, TopKLogitsWarper, TopPLogitsWarper
-    from transformers.utils import logging as hf_logging
     given = {k: v for k, v in dict(kwargs, do_sample=do_sample, temperature=temperature).items() if v is not None}
-    verbosity = hf_logging.get_verbosity()
-    hf_logging.set_verbosity_error()     # HF's notes on flags and pad tokens belong to its own loop
-    try:
-        gc, _ = model._prepare_generation_config(given.pop('generation_config', None), **given)
-        model._prepare_special_tokens(gc, True, 'cpu')
-    finally:
-        hf_logging.set_verbosity(verbosity)
+    gc = _generation_config(model, given)
     if (gc.num_beams or 1) > 1:
         raise NotImplementedError('beam search (num_beams=%d) runs on the HF loop only: pass use_hf_loop=True'
                                   % gc.num_beams)
@@ -527,15 +538,8 @@ def resolve_beam_search(model, input_len, max_new_tokens, do_sample=None, **kwar
     num_return_sequences, eos_token_id (a list), pad_token_id and max_length.  Beam search with do_sample, with any
     logits processor, or with output_scores / return_dict_in_generate raises NotImplementedError: the HF loop
     (use_hf_loop=True) runs those."""
-    from transformers.utils import logging as hf_logging
     given = {k: v for k, v in dict(kwargs, do_sample=do_sample, max_new_tokens=max_new_tokens).items() if v is not None}
-    verbosity = hf_logging.get_verbosity()
-    hf_logging.set_verbosity_error()
-    try:
-        gc, _ = model._prepare_generation_config(given.pop('generation_config', None), **given)
-        model._prepare_special_tokens(gc, True, 'cpu')
-    finally:
-        hf_logging.set_verbosity(verbosity)
+    gc = _generation_config(model, given)
     N = gc.num_beams or 1
     if N <= 1:
         return None
@@ -559,6 +563,44 @@ def resolve_beam_search(model, input_len, max_new_tokens, do_sample=None, **kwar
                 num_return_sequences=int(nrs), eos_token_id=None if eos is None else eos.flatten().tolist(),
                 pad_token_id=None if pad is None else int(pad),
                 max_length=int(input_len + gc.max_new_tokens if gc.max_new_tokens is not None else gc.max_length))
+
+
+_STOP_STRINGS = collections.OrderedDict()   # (vocabulary, stop strings) -> StopStrings; the last 8 used
+
+
+def stop_strings_from_tokenizer(tokenizer, stop_strings):
+    """The engine's StopStrings table for `tokenizer`: its token strings are what transformers' matcher uses
+    (StopStringCriteria.clean_tokenizer_vocab).  Kept per (vocabulary, stop strings), as HF keeps its own tables."""
+    from transformers.generation.stopping_criteria import StopStringCriteria
+    stops = (stop_strings,) if isinstance(stop_strings, str) else tuple(stop_strings)
+    key = (tuple(sorted(tokenizer.get_vocab().items())), stops)     # sorted: a fast tokenizer lists it in no fixed order
+    if key not in _STOP_STRINGS:
+        strings, ids = StopStringCriteria.clean_tokenizer_vocab(tokenizer)
+        by_id = [None] * (max(ids) + 1)
+        for s, i in zip(strings, ids):
+            by_id[i] = s
+        _STOP_STRINGS[key] = StopStrings(by_id, stops)
+        if len(_STOP_STRINGS) > 8:
+            _STOP_STRINGS.popitem(last=False)
+    _STOP_STRINGS.move_to_end(key)
+    return _STOP_STRINGS[key]
+
+
+def resolve_stop_strings(model, tokenizer=None, stop_strings=None, generation_config=None):
+    """The stop strings of a generate call, resolved as transformers resolves them (the explicit kwarg, then
+    `generation_config=`, then model.generation_config): a tuple, or None when there are none.  Stop strings without a
+    tokenizer raise the ValueError transformers raises (GenerationMixin._get_stopping_criteria)."""
+    given = dict(generation_config=generation_config)
+    if stop_strings is not None:
+        given['stop_strings'] = stop_strings
+    stops = _generation_config(model, given).stop_strings
+    if stops is None:
+        return None
+    if tokenizer is None:
+        raise ValueError("There are one or more stop strings, either in the arguments to `generate` or in the model's "
+                         "generation config, but we could not locate a tokenizer. When generating with stop strings, "
+                         "you must pass the model's tokenizer to the `tokenizer` argument of `generate`.")
+    return (stops,) if isinstance(stops, str) else tuple(stops)
 
 
 class SPILlavaMPTForCausalLM(LlamaForCausalLM, _EngineHost):
@@ -750,9 +792,13 @@ class SPILlavaMPTForCausalLM(LlamaForCausalLM, _EngineHost):
         generation_config (resolve_sampling: the demo's call samples from the top 50 at T = 0.2, as on the HF loop);
         the draws are keyed by torch's default generator (or `generator=`), so torch.manual_seed makes them
         reproducible.  Other logits processors raise NotImplementedError there.
+        stop_strings (with tokenizer=, as transformers' generate takes them; resolve_stop_strings) are matched on the
+        device, per row, inside the decode step (engine.StopStrings): a row that has produced a stop string is finished
+        and, when eos_token_id and pad_token_id are given, filled with pad_token_id, as on the HF loop.  Host
+        stopping_criteria (KeywordsStoppingCriteria) keep running as callbacks after every token.
         num_beams > 1 (do_sample false) runs beam search on the engine loop (resolve_beam_search: length_penalty,
         early_stopping, num_return_sequences, eos / max length as HF resolves them): the prompt is prefilled once per
-        sample and the beams share its KV cache; beam sampling, logits processors, stopping_criteria, output_scores /
+        sample and the beams share its KV cache; beam sampling, logits processors, stopping_criteria, stop_strings, output_scores /
         return_dict_in_generate and past_key_values raise NotImplementedError there, and run with use_hf_loop=True."""
         if bboxes is None:
             bboxes = getattr(getattr(self, 'forward', None), 'keywords', {}).get('bboxes')
@@ -769,12 +815,17 @@ class SPILlavaMPTForCausalLM(LlamaForCausalLM, _EngineHost):
             return super().generate(input_ids, images=images, bboxes=bboxes, max_new_tokens=max_new_tokens,
                                     do_sample=bool(do_sample), use_cache=True, **kw)
         gen = {k: v for k, v in kwargs.items() if k not in ('attention_mask', 'pad_token_id', 'past_key_values',
-                                                             'generator')}
+                                                             'generator', 'tokenizer')}
+        stops = resolve_stop_strings(self, kwargs.get('tokenizer'), kwargs.get('stop_strings'),
+                                     kwargs.get('generation_config'))
         beam = resolve_beam_search(self, input_ids.shape[1], max_new_tokens, do_sample, eos_token_id=eos_token_id,
                                    pad_token_id=kwargs.get('pad_token_id'), **gen)
         if beam is not None:
             if stopping_criteria is not None:
                 raise NotImplementedError('beam search with stopping_criteria runs on the HF loop only: pass '
+                                          'use_hf_loop=True')
+            if stops is not None:
+                raise NotImplementedError('beam search with stop_strings runs on the HF loop only: pass '
                                           'use_hf_loop=True')
             if kwargs.get('past_key_values') is not None:
                 raise NotImplementedError('beam search on a conversation cache (past_key_values) runs on the HF loop '
@@ -799,7 +850,8 @@ class SPILlavaMPTForCausalLM(LlamaForCausalLM, _EngineHost):
         return eng.generate(input_ids, images, bboxes, max_new_tokens=max_new_tokens, do_sample=do_sample,
                             temperature=temperature, top_k=top_k, top_p=top_p, stopping_criteria=stopping_criteria,
                             eos_token_id=eos_token_id, attention_mask=kwargs.get('attention_mask'),
-                            pad_token_id=kwargs.get('pad_token_id'), cache=kv, generator=kwargs.get('generator'))
+                            pad_token_id=kwargs.get('pad_token_id'), cache=kv, generator=kwargs.get('generator'),
+                            stop_strings=None if stops is None else stop_strings_from_tokenizer(kwargs['tokenizer'], stops))
 
     def initialize_vision_tokenizer(self, mm_use_im_start_end, tokenizer, device, tune_mm_mlp_adapter=False,
                                     pretrain_mm_mlp_adapter=None):

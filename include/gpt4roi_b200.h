@@ -329,6 +329,19 @@ int g4r_sample_tokens_bf16(const void* logits, long long ld, int B, int V, float
                            int greedy, unsigned long long seed, const long long* rng_step, int eos_id, int pad_id,
                            int* finished, long long* out_ids, void* stream);
 
+/* ---- stop strings (after the next-token selection, once per decode step) ---------------------
+ * Replaces transformers.generation.stopping_criteria.StopStringCriteria.__call__ (and, per row, the reference's
+ * KeywordsStoppingCriteria, llava/model/utils.py:26-46) for the decode loop: a row stops at the first generated token
+ * in which an occurrence of a stop string ends.  The matcher is a table built once on the host:
+ * step: int16 [V_tok + 1, S], row pitch ld elements; entry (t, s) = the matcher's state after token t is fed from state
+ * s (low 15 bits), bit 15 set when an occurrence ended inside token t.  Row V_tok is the reset row.
+ * For every row b with finished[b] == 0:  e = step[t][state[b]], t = ids[b] if 0 <= ids[b] < V_tok else V_tok;
+ * state[b] = e & 0x7FFF; finished[b] = 1 if e < 0.  Rows with finished[b] != 0 are left untouched.
+ * ids: int64 [B] (what g4r_sample_tokens wrote); state, finished: int32 [B].  S in 1..32767.
+ * Capturable: every per-step value is read from device memory. */
+int g4r_stop_step(const long long* ids, const short* step, long long ld, int V_tok, int S, int B, int* state,
+                  int* finished, void* stream);
+
 /*
  * NHWC convolution as an implicit GEMM (stride 1, pad (ksize-1)/2, ksize 1 or 3):
  *   Y[n,y,x,co] = act( sum_{ky,kx,ci} X[n,y+ky-1,x+kx-1,ci] * Wt[co,(ky*ks+kx)*Cin+ci] + bias[co] )
