@@ -203,6 +203,176 @@ decode_attention_bf16(const __nv_bfloat16* q, long long ldq, const __nv_bfloat16
   cluster.sync();   // keep every CTA's shared memory alive until rank 0 has read it
 }
 
+// Shared-prefix ("cascade") decode attention for several sampled answers per prompt (generate(num_return_sequences=N,
+// do_sample=True), engine.SampleCache).  Cache layout [B + B*N, Lmax, HD]: rows 0..B-1 hold the prompts, row B + r the
+// generated positions of query row r = b*N + i.  Row r attends over positions 0..prompt_lens[b]-1 of prompt row b and
+// prompt_lens[b]..pos_rows[r] of its own row.  Grid (H, B, S), a cluster of S CTAs along z as in decode_attention_bf16:
+// CTA (h, b, rank) owns slice `rank` of prompt b's keys and slice `rank` of each of the N rows' own keys, so every
+// prompt key / value row is fetched from HBM by one CTA and used there by all N queries (the N reads hit L1 / L2).
+// 16 lane groups of 16 lanes (a lane holds 8 of the 128 features, as above); lane group g serves query g / KS and
+// every KS-th key of that query's local keys (KS = 16 / N): QK^T and P.V on the CUDA cores, q and the partial output
+// in registers.  One max and one sum per query over all its keys; the statistics and partial outputs combine across
+// the cluster through distributed shared memory in rank order.  No atomics: bitwise repeatable.
+// An empty slice (a prompt shorter than S keys, a row with no generated key yet) still joins every barrier.
+constexpr int GROUP_MAX_N = 16;
+
+__global__ void __launch_bounds__(256)
+decode_attention_group_bf16(const __nv_bfloat16* q, long long ldq, const __nv_bfloat16* kc, const __nv_bfloat16* vc,
+                            __nv_bfloat16* out, long long ldo, int H, int N, const int* __restrict__ prompt_lens,
+                            const int* __restrict__ pos_rows, int Lmax, float scale, int per_max, int gper_max) {
+  pdl_sync();
+  constexpr int D = 128, LPR = 16, GROUPS = 16;
+  namespace cg = cooperative_groups;
+  cg::cluster_group cluster = cg::this_cluster();
+  const int S = (int)cluster.num_blocks(), rank = (int)cluster.block_rank();
+  const int h = blockIdx.x, b = blockIdx.y, B = gridDim.y;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int sub = lane % LPR, grp = warp * 2 + lane / LPR;
+  const int HD = H * D;
+  const int KS = GROUPS / N;                 // lane groups per query
+  const int qi = grp / KS, part = grp % KS;  // this group's query and its share of the query's keys
+  const bool active = qi < N;
+  const int r = b * N + (active ? qi : 0);
+  const int P = prompt_lens[b];
+  const int per = (P + S - 1) / S;
+  const int k0 = rank * per;
+  const int n_loc = max(0, min(P, k0 + per) - k0);            // prompt keys of this CTA, shared by the N queries
+  const int g = active ? max(0, pos_rows[r] + 1 - P) : 0;     // the row's own keys
+  const int gper = (g + S - 1) / S;
+  const int g0 = rank * gper;
+  const int n_gen = max(0, min(g, g0 + gper) - g0);
+  const int n_all = active ? n_loc + n_gen : 0;               // local keys of the query: prompt slice, then own slice
+  // both lane groups of a warp run the same trip count (the reductions shuffle across the whole warp)
+  const int n_warp = max(n_all, __shfl_xor_sync(0xffffffffu, n_all, 16));
+  const int ld_sc = per_max + gper_max;
+  extern __shared__ float sm[];
+  float* sc = sm;                              // [N][ld_sc] scores / probabilities of the local keys
+  float* part_o = sm + N * ld_sc;              // [GROUPS][D] partial outputs of the lane groups
+  float* tot = part_o + GROUPS * D;            // [N][D] CTA totals, read by rank 0
+  __shared__ float red[GROUPS];
+  __shared__ float cl_max[GROUP_MAX_N], cl_sum[GROUP_MAX_N];
+
+  float qf[8];
+  {
+    uint4 raw = make_uint4(0, 0, 0, 0);
+    if (active) raw = *reinterpret_cast<const uint4*>(q + (long long)r * ldq + (long long)h * D + sub * 8);
+    const __nv_bfloat162* hh = reinterpret_cast<const __nv_bfloat162*>(&raw);
+#pragma unroll
+    for (int j = 0; j < 4; j++) {
+      const float2 f = __bfloat1622float2(hh[j]);
+      qf[2 * j] = f.x * scale;
+      qf[2 * j + 1] = f.y * scale;
+    }
+  }
+  // local key j of the query: prompt row b at k0 + j, or its own row B + r at P + g0 + (j - n_loc)
+  const long long prompt_off = ((long long)b * Lmax + k0) * HD + (long long)h * D + sub * 8;
+  const long long own_off = ((long long)(B + r) * Lmax + P + g0 - n_loc) * HD + (long long)h * D + sub * 8;
+  auto off = [&](int j) -> long long { return (j < n_loc ? prompt_off : own_off) + (long long)j * HD; };
+  float* srow = sc + (active ? qi : 0) * ld_sc;
+  const int step = 4 * KS;
+  // ---- phase 1: scores of the local keys
+  float mx = -INFINITY;
+  for (int base = part; base - part < n_warp; base += step) {
+    uint4 raw[4];
+#pragma unroll
+    for (int u = 0; u < 4; u++) {
+      const int j = base + u * KS;
+      raw[u] = j < n_all ? *reinterpret_cast<const uint4*>(kc + off(j)) : make_uint4(0, 0, 0, 0);
+    }
+#pragma unroll
+    for (int u = 0; u < 4; u++) {
+      const __nv_bfloat162* hh = reinterpret_cast<const __nv_bfloat162*>(&raw[u]);
+      float acc = 0.f;
+#pragma unroll
+      for (int j = 0; j < 4; j++) {
+        const float2 f = __bfloat1622float2(hh[j]);
+        acc += f.x * qf[2 * j] + f.y * qf[2 * j + 1];
+      }
+#pragma unroll
+      for (int o = LPR / 2; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+      const int j = base + u * KS;
+      if (j < n_all) {
+        if (sub == 0) srow[j] = acc;
+        mx = fmaxf(mx, acc);
+      }
+    }
+  }
+  if (sub == 0) red[grp] = mx;
+  __syncthreads();
+  if (tid < N) {
+    float m = red[tid * KS];
+    for (int p = 1; p < KS; p++) m = fmaxf(m, red[tid * KS + p]);
+    cl_max[tid] = m;
+  }
+  cluster.sync();
+  float gmax = -INFINITY;
+  if (active)
+    for (int c = 0; c < S; c++) gmax = fmaxf(gmax, *cluster.map_shared_rank(&cl_max[qi], c));
+  float sum = 0.f;
+  for (int j = part + sub * KS; j < n_all; j += LPR * KS) {
+    const float p = __expf(srow[j] - gmax);
+    srow[j] = p;
+    sum += p;
+  }
+#pragma unroll
+  for (int o = LPR / 2; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+  if (sub == 0) red[grp] = sum;   // the max's reads of red[] finished before the cluster barrier
+  __syncthreads();
+  if (tid < N) {
+    float t = 0.f;
+    for (int p = 0; p < KS; p++) t += red[tid * KS + p];
+    cl_sum[tid] = t;
+  }
+  cluster.sync();
+  float gsum = 0.f;
+  if (active)
+    for (int c = 0; c < S; c++) gsum += *cluster.map_shared_rank(&cl_sum[qi], c);
+  const float inv = active ? 1.f / gsum : 0.f;
+  // ---- phase 2: partial P.V of the local keys (probabilities rounded to the 16-bit type, as P.to(q.dtype))
+  float o8[8];
+#pragma unroll
+  for (int j = 0; j < 8; j++) o8[j] = 0.f;
+  for (int base = part; base < n_all; base += step) {
+    uint4 raw[4];
+    float pk[4];
+#pragma unroll
+    for (int u = 0; u < 4; u++) {
+      const int j = base + u * KS;
+      const bool ok = j < n_all;
+      raw[u] = ok ? *reinterpret_cast<const uint4*>(vc + off(j)) : make_uint4(0, 0, 0, 0);
+      pk[u] = ok ? __bfloat162float(__float2bfloat16_rn(srow[j] * inv)) : 0.f;
+    }
+#pragma unroll
+    for (int u = 0; u < 4; u++) {
+      const __nv_bfloat162* hh = reinterpret_cast<const __nv_bfloat162*>(&raw[u]);
+#pragma unroll
+      for (int j = 0; j < 4; j++) {
+        const float2 f = __bfloat1622float2(hh[j]);
+        o8[2 * j] += pk[u] * f.x;
+        o8[2 * j + 1] += pk[u] * f.y;
+      }
+    }
+  }
+#pragma unroll
+  for (int j = 0; j < 8; j++) part_o[grp * D + sub * 8 + j] = o8[j];
+  __syncthreads();
+  for (int i = tid; i < N * D; i += 256) {
+    const int t = i / D, d = i % D;
+    float v = 0.f;
+    for (int p = 0; p < KS; p++) v += part_o[(t * KS + p) * D + d];
+    tot[i] = v;
+  }
+  cluster.sync();
+  if (rank == 0) {
+    for (int i = tid; i < N * D; i += 256) {
+      float v = 0.f;
+      for (int c = 0; c < S; c++) v += cluster.map_shared_rank(tot, c)[i];
+      out[(long long)(b * N + i / D) * ldo + (long long)h * D + i % D] = __float2bfloat16_rn(v);
+    }
+  }
+  cluster.sync();   // keep every CTA's shared memory alive until rank 0 has read it
+}
+
 }  // namespace g4r
 
 using namespace G4R_NS;
@@ -297,4 +467,34 @@ extern "C" int g4r_decode_attention_beam_bf16(const void* q, long long ldq, cons
   G4R_REQUIRE(pos_rows != nullptr && anc != nullptr, "decode_attention_beam: pos_rows and anc are required");
   return decode_attention(q, ldq, kcache, vcache, out, ldo, R, H, head_dim, kv_bound, nullptr, pos_rows, anc, Lmax, scale,
                           stream);
+}
+
+extern "C" int g4r_decode_attention_group_bf16(const void* q, long long ldq, const void* kcache, const void* vcache,
+                                               void* out, long long ldo, int B, int N, int H, int head_dim,
+                                               int prompt_bound, int gen_bound, const int* prompt_lens,
+                                               const int* pos_rows, int Lmax, float scale, void* stream) {
+  G4R_REQUIRE(q && kcache && vcache && out && prompt_lens && pos_rows, "decode_attention_group: NULL argument");
+  G4R_REQUIRE(N >= 1 && N <= GROUP_MAX_N, "decode_attention_group: N=%d rows per prompt; the kernel supports 1..%d", N,
+              GROUP_MAX_N);
+  G4R_REQUIRE(head_dim == 128, "decode_attention_group: head_dim %d (only 128 is built)", head_dim);
+  G4R_REQUIRE(B > 0 && H > 0 && prompt_bound > 0 && gen_bound >= 0 && prompt_bound + gen_bound <= Lmax,
+              "decode_attention_group: bad arguments (B=%d H=%d prompt_bound=%d gen_bound=%d Lmax=%d)", B, H,
+              prompt_bound, gen_bound, Lmax);
+  G4R_REQUIRE(ldq % 8 == 0 && ((uintptr_t)q & 15) == 0, "decode_attention_group: q rows must be 16-byte aligned");
+  // split-KV factor as decode_attention's, over the B prompts
+  int S = 1;
+  while (S < 8 && H * B * S < 2 * num_sms() && prompt_bound / (2 * S) >= 64) S *= 2;
+  const int per_max = (prompt_bound + S - 1) / S, gper_max = (gen_bound + S - 1) / S;
+  const size_t smem = ((size_t)N * (per_max + gper_max) + (size_t)(16 + N) * head_dim) * sizeof(float);
+  G4R_REQUIRE(smem <= 200 * 1024, "decode_attention_group: N=%d rows x (%d prompt + %d generated) keys per CTA exceed "
+              "the shared-memory score buffer", N, per_max, gper_max);
+  static bool set = false;
+  if (!set) {
+    G4R_CUDA(cudaFuncSetAttribute(decode_attention_group_bf16, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    set = true;
+  }
+  G4R_CUDA(launch_pdl(decode_attention_group_bf16, dim3(H, B, S), dim3(256), smem, (cudaStream_t)stream, dim3(1, 1, S),
+                      (const __nv_bfloat16*)q, ldq, (const __nv_bfloat16*)kcache, (const __nv_bfloat16*)vcache,
+                      (__nv_bfloat16*)out, ldo, H, N, prompt_lens, pos_rows, Lmax, scale, per_max, gper_max));
+  return G4R_OK;
 }

@@ -728,6 +728,10 @@ def _decode_step_chain(self, token_ids, cache, pos_dev):
 
 def _decode_attention(cache, li, qkv, kv_len, scale, pos_dev, rows, anc):
     c = cache.cfg
+    if isinstance(cache, SampleCache):   # N rows per prompt: the prompt's keys read once for all of them
+        return kernels.decode_attention_group(qkv, cache.full_k[li], cache.full_v[li], cache.n_samples, cache.N,
+                                              c.n_heads, c.head_dim, cache.prompt_len, cache.G, scale,
+                                              cache.prompt_lens, rows)
     if anc is None:
         return kernels.decode_attention(qkv, cache.k[li], cache.v[li], qkv.shape[0], c.n_heads, c.head_dim, kv_len, scale,
                                         pos_dev, pos_rows=rows)
@@ -967,7 +971,15 @@ def _generate(self, input_ids, images, bboxes, max_new_tokens=32, do_sample=Fals
     num_beams > 1: deterministic beam search (transformers' GenerationMixin._beam_search, do_sample=False) with
     length_penalty, early_stopping (True, False or "never") and num_return_sequences <= num_beams; eos_token_id may be
     a list.  The prompt is prefilled once per sample and the beams share its KV cache (BeamCache).  Returns
-    [B * num_return_sequences, L + n] as HF crops it."""
+    [B * num_return_sequences, L + n] as HF crops it.
+    num_return_sequences = N > 1 with sampling (num_beams 1): N independent answers per prompt, as HF's _sample
+    returns them after expanding the inputs -- [B * N, L + n], row b*N + i is sample i of prompt b, each row with its
+    own tokens, eos -> pad rule, stop-string state and finished flag; host stopping_criteria see all B * N rows.  Row r
+    draws with Philox counter (step, r), so the result is that of this loop on input_ids.repeat_interleave(N, 0) with
+    the same seed, up to the attention's summation order.  The prompts are prefilled once, at batch B, and the N rows
+    of a prompt share its KV cache (SampleCache), whose keys the decode attention reads once per step for all N.
+    Greedy selection with N > 1 raises ValueError, as HF does; a conversation cache (cache=) with N > 1 raises
+    NotImplementedError."""
     if num_beams > 1:
         if do_sample:
             raise NotImplementedError('beam search with do_sample runs on the HF loop only: pass use_hf_loop=True')
@@ -981,29 +993,51 @@ def _generate(self, input_ids, images, bboxes, max_new_tokens=32, do_sample=Fals
         return _generate_beams(self, input_ids, images, bboxes, max_new_tokens, num_beams, eos_token_id, pad_token_id,
                                attention_mask, length_penalty, early_stopping, num_return_sequences, use_graph)
     B, L = input_ids.shape
+    N = int(num_return_sequences)
+    greedy = not (do_sample and temperature > 0)
+    if N != 1:
+        if N < 1:
+            raise ValueError('num_return_sequences must be >= 1, got %d' % N)
+        if greedy:
+            raise ValueError('Greedy methods without beam search do not support `num_return_sequences` different than 1 '
+                             '(got %d).' % N)
+        if cache is not None:
+            raise NotImplementedError('several sampled answers per prompt (num_return_sequences=%d) on a conversation '
+                                      'cache (cache=) run on the HF loop only: pass use_hf_loop=True' % N)
     ids = input_ids.to(self.dev)
     if cache is not None:
         logits = self.prefill_cached(cache, input_ids, images, bboxes, attention_mask, new_tokens=max_new_tokens)
         pos0 = cache.row_lens().clone()
+    elif N > 1:   # the B prompts prefilled once; each prompt's N rows share its K/V
+        cache = SampleCache(self.cfg, B, N, L, max_new_tokens, self.dev)
+        run_ids, lens, _ = _right_padded(ids, attention_mask)
+        logits = self.forward_device(run_ids, None if images is None else images.to(self.dev, self.dt),
+                                     self.plan_boxes(bboxes), validate=True, last_only=True, seqlens=_seqlens(lens, L),
+                                     cache=cache.prompt)
+        cache.start(lens)
+        logits = logits.repeat_interleave(N, 0)   # every row's first token is drawn from its prompt's logits
+        pos0 = None
     else:
         cache = KVCache(self.cfg, B, L + max_new_tokens, self.dev)
         run_ids, lens, _ = _right_padded(ids, attention_mask)
         logits = self.forward_device(run_ids, images.to(self.dev, self.dt), self.plan_boxes(bboxes), validate=True,
                                      last_only=True, seqlens=_seqlens(lens, L), cache=cache)
         pos0 = None
-    greedy = not (do_sample and temperature > 0)
+    R = B * N
     rule = pad_token_id is not None and eos_token_id is not None
     stop_state = None
     if stop_strings is not None:     # the submitted prompt's tokens, also on a conversation cache
         stop_state = stop_strings.initial_states(*_right_padded(input_ids.cpu(), attention_mask)[:2])
-    sampler = Sampler(B, self.dev, greedy, temperature, top_k, top_p, seed=0 if greedy else sampling_seed(generator),
+        if N > 1:
+            stop_state = stop_state.repeat_interleave(N)
+    sampler = Sampler(R, self.dev, greedy, temperature, top_k, top_p, seed=0 if greedy else sampling_seed(generator),
                       eos_id=eos_token_id, pad_id=pad_token_id, stops=stop_strings, stop_state=stop_state)
-    out = torch.empty((B, L + max_new_tokens), dtype=torch.int64, device=self.dev)
-    out[:, :L] = ids
+    out = torch.empty((R, L + max_new_tokens), dtype=torch.int64, device=self.dev)
+    out[:, :L] = ids if N == 1 else ids.repeat_interleave(N, 0)
     stepper = None
     if use_graph and max_new_tokens > 4 and self.cfg.head_dim == 128:
         stepper = GraphedDecode(self, cache, sampler=sampler)   # each replay also selects the next token into its ids
-    tok = stepper.ids if stepper is not None else torch.empty((B, 1), dtype=torch.int64, device=self.dev)
+    tok = stepper.ids if stepper is not None else torch.empty((R, 1), dtype=torch.int64, device=self.dev)
     sampler(logits, tok)              # the first new token, from the prefill logits
     sampler.advance()
     n = 0
@@ -1091,17 +1125,14 @@ class GraphedDecode:
         return self.logits
 
 
-class BeamCache:
-    """KV cache and device state of beam search over B samples of N beams.  Per layer one [B + B*N, Lmax, HD] tensor
-    (full_k / full_v): rows 0..B-1 hold the prompts (the B-row prefill writes them through `prompt`, a KVCache whose
-    k / v are the views [:B]), rows B.. the beams (the decode step writes beam row r's new K/V at pos_rows[r] through
-    the views k / v = [B:]).  A cell is written once and never moved: `anc` (int32 [B*N, Lmax]) names the cache row
-    that holds position p of beam row r -- its sample's prompt row below lens[b], else the beam row that wrote it --
-    and the beam step permutes its generated columns when the beams are reordered.  The rest is the state of
-    transformers' _beam_search that kernels.beam_step keeps on the device (see g4r_beam_step_bf16)."""
+class _SharedPromptCache:
+    """KV layout of N decode rows per prompt that share the prompt's K/V (beam search, several sampled answers).  Per
+    layer one [B + B*N, Lmax, HD] tensor (full_k / full_v): rows 0..B-1 hold the B prompts (n_samples; the B-row
+    prefill writes them through `prompt`, a KVCache whose k / v are the views [:B]), row B + r the positions decode row
+    r generates (the decode step writes row r's new K/V at pos_rows[r] = lens[r] through the views k / v = [B:]).
+    prompt_lens: each prompt's length, device int32 [B]."""
 
-    def __init__(self, cfg, B, N, prompt_len, max_new_tokens, device, eos=(), length_penalty=1.0, early_stopping=False,
-                 fill=-1):
+    def __init__(self, cfg, B, N, prompt_len, max_new_tokens, device):
         hd = cfg.n_heads * cfg.head_dim
         dt = cfg.torch_dtype
         dev = torch.device(device)
@@ -1117,6 +1148,43 @@ class BeamCache:
         self.max_len = self.Lmax = Lmax
         self.length = 0
         self.G = max_new_tokens
+        self.lens = torch.zeros(R, dtype=torch.int32, device=dev)          # pos_rows of the decode step
+        self.prompt_lens = torch.full((B,), prompt_len, dtype=torch.int32, device=dev)
+
+
+class SampleCache(_SharedPromptCache):
+    """KV cache of N sampled answers per prompt (generate(num_return_sequences=N, do_sample=True)): the shared-prompt
+    layout with sample row r = b*N + i in cache row B + r.  Rows never reorder, so there is no ancestry table: position p
+    of row r lies in prompt row b below prompt_lens[b], else in row B + r.  The decode attention
+    (kernels.decode_attention_group) reads each prompt's keys once per step for all N of its rows."""
+
+    def __init__(self, cfg, B, N, prompt_len, max_new_tokens, device):
+        if not 1 <= N <= kernels.GROUP_MAX_N:
+            raise ValueError('num_return_sequences=%d: the engine loop samples 1..%d answers per prompt; pass '
+                             'use_hf_loop=True for more' % (N, kernels.GROUP_MAX_N))
+        super().__init__(cfg, B, N, prompt_len, max_new_tokens, device)
+
+    def start(self, lens):
+        """After the prefill: lens (int64 or int32 [B]) each prompt's length; every sample row's first new token goes
+        to its prompt's length."""
+        self.prompt_lens.copy_(lens.to(torch.int32))
+        self.lens.copy_(self.prompt_lens.repeat_interleave(self.N))
+        self.length = self.prompt_len
+
+
+class BeamCache(_SharedPromptCache):
+    """KV cache and device state of beam search over B samples of N beams, in the shared-prompt layout (beam row r in
+    cache row B + r).  A cell is written once and never moved: `anc` (int32 [B*N, Lmax]) names the cache row
+    that holds position p of beam row r -- its sample's prompt row below lens[b], else the beam row that wrote it --
+    and the beam step permutes its generated columns when the beams are reordered.  The rest is the state of
+    transformers' _beam_search that kernels.beam_step keeps on the device (see g4r_beam_step_bf16)."""
+
+    def __init__(self, cfg, B, N, prompt_len, max_new_tokens, device, eos=(), length_penalty=1.0, early_stopping=False,
+                 fill=-1):
+        super().__init__(cfg, B, N, prompt_len, max_new_tokens, device)
+        dev = torch.device(device)
+        R = B * N
+        Lmax = self.Lmax
         self.max_length = prompt_len + max_new_tokens
         eos = [int(e) for e in eos]
         self.n_eos = len(eos)
@@ -1127,9 +1195,7 @@ class BeamCache:
             raise ValueError('early_stopping must be True, False or "never", got %r' % (early_stopping,))
         self.early = 2 if early_stopping == 'never' else int(bool(early_stopping))
         self.fill = int(fill)
-        self.lens = torch.zeros(R, dtype=torch.int32, device=dev)          # pos_rows of the decode step
         self.pos_rows = self.lens
-        self.prompt_lens = torch.full((B,), prompt_len, dtype=torch.int32, device=dev)
         self.anc = torch.zeros((R, Lmax), dtype=torch.int32, device=dev)
         self.ids = torch.zeros((R, 1), dtype=torch.int64, device=dev)     # the graph's own input
         self.state = torch.zeros(4 * B + 2, dtype=torch.int32, device=dev)

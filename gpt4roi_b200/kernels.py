@@ -298,6 +298,29 @@ def decode_attention_beam(qkv, kcache, vcache, R, n_heads, head_dim, kv_bound, s
     return out
 
 
+GROUP_MAX_N = 16   # rows per prompt the shared-prefix decode attention supports (csrc/decode.cu)
+
+
+def decode_attention_group(qkv, kcache, vcache, B, N, n_heads, head_dim, prompt_bound, gen_bound, scale, prompt_lens,
+                           pos_rows):
+    """Decode attention for N sampled rows per prompt sharing the prompt's keys: qkv [B*N, 3*HD] (row r = b*N + i);
+    caches [B + B*N, Lmax, HD] -- rows 0..B-1 the prompts, row B + r row r's own generated positions.  Row r attends
+    over positions 0..prompt_lens[b]-1 of cache row b and prompt_lens[b]..pos_rows[r] of cache row B + r (prompt_lens:
+    device int32 [B], pos_rows: device int32 [B*N]).  prompt_bound / gen_bound (>= every prompt length / every row's
+    count of own keys) size the split and the score buffer.  1 <= N <= 16 and head_dim 128.  Returns [B*N, HD]."""
+    if not 1 <= N <= GROUP_MAX_N:
+        raise ValueError('decode_attention_group: %d rows per prompt; the kernel supports 1..%d' % (N, GROUP_MAX_N))
+    act = _bf16(qkv, kcache, vcache)
+    if kcache.shape[0] != B + B * N or tuple(vcache.shape) != tuple(kcache.shape):
+        raise RuntimeError('decode_attention_group: caches must hold %d rows (B prompts + B*N sample rows)' % (B + B * N))
+    out = torch.empty((B * N, n_heads * head_dim), dtype=act, device=qkv.device)
+    _call('g4r_decode_attention_group_bf16', qkv.device, _L.ptr(qkv), qkv.stride(0), _L.ptr(kcache), _L.ptr(vcache),
+          _L.ptr(out), out.stride(0), int(B), int(N), n_heads, head_dim, int(prompt_bound), int(gen_bound),
+          _L.ptr(_L.require_pos_rows(prompt_lens, B)), _L.ptr(_L.require_pos_rows(pos_rows, B * N)), kcache.shape[1],
+          float(scale), act=act)
+    return out
+
+
 def beam_step(logits, row_div, st):
     """One beam-search step (csrc/beam.cu) on 16-bit logits [rows, V] (or [rows, 1, V]; unit column stride) with the
     device state of st (engine.BeamCache): B*N rows, or B with row_div = N (the first step, from the prefill)."""

@@ -105,6 +105,7 @@ SIGNATURES = {
     'g4r_stop_step': (_i, [_vp, _vp, _ll, _i, _i, _i, _vp, _vp, _vp]),
     'g4r_decode_attention_beam_bf16': (_i, [_vp, _ll, _vp, _vp, _vp, _ll, _i, _i, _i, _i, _vp, _vp, _i, _f, _vp]),
     'g4r_beam_step_bf16': (_i, [_vp, _ll] + [_i] * 5 + [_vp] + [_i] * 3 + [_c.c_double] + [_i] * 3 + [_vp] * 13),
+    'g4r_decode_attention_group_bf16': (_i, [_vp, _ll, _vp, _vp, _vp, _ll] + [_i] * 6 + [_vp, _vp, _i, _f, _vp]),
 }
 
 # fp16 twins of the inference entry points (include/gpt4roi_b200.h, last section; csrc/act_type.cuh): same signatures.
@@ -141,6 +142,7 @@ F16_TWINS = {
     'g4r_sample_tokens_bf16': 'g4r_sample_tokens_f16',
     'g4r_decode_attention_beam_bf16': 'g4r_decode_attention_beam_f16',
     'g4r_beam_step_bf16': 'g4r_beam_step_f16',
+    'g4r_decode_attention_group_bf16': 'g4r_decode_attention_group_f16',
 }
 SIGNATURES.update({twin: SIGNATURES[name] for name, twin in F16_TWINS.items()})
 

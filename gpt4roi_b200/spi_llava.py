@@ -531,6 +531,15 @@ def resolve_sampling(model, input_len, do_sample=None, temperature=None, **kwarg
             float(gc.top_p if gc.top_p is not None else 1.0))
 
 
+def resolve_num_return_sequences(model, do_sample=None, temperature=None, **kwargs):
+    """How many answers per prompt a generate call without beam search returns, resolved as transformers resolves it:
+    the explicit kwarg, then `generation_config=`, then model.generation_config (GenerationMixin.
+    _prepare_generation_config).  Greedy selection with more than one raises HF's own ValueError from the config's
+    validation."""
+    given = {k: v for k, v in dict(kwargs, do_sample=do_sample, temperature=temperature).items() if v is not None}
+    return int(_generation_config(model, given).num_return_sequences or 1)
+
+
 def resolve_beam_search(model, input_len, max_new_tokens, do_sample=None, **kwargs):
     """The engine loop's beam search for a generate call, resolved as transformers resolves it (explicit kwargs, then
     `generation_config=`, then model.generation_config, then HF's defaults: GenerationMixin._prepare_generation_config).
@@ -799,7 +808,11 @@ class SPILlavaMPTForCausalLM(LlamaForCausalLM, _EngineHost):
         num_beams > 1 (do_sample false) runs beam search on the engine loop (resolve_beam_search: length_penalty,
         early_stopping, num_return_sequences, eos / max length as HF resolves them): the prompt is prefilled once per
         sample and the beams share its KV cache; beam sampling, logits processors, stopping_criteria, stop_strings, output_scores /
-        return_dict_in_generate and past_key_values raise NotImplementedError there, and run with use_hf_loop=True."""
+        return_dict_in_generate and past_key_values raise NotImplementedError there, and run with use_hf_loop=True.
+        do_sample with num_return_sequences = N > 1 (resolve_num_return_sequences) returns N independent samples per
+        prompt, [B * N, L + new] with row b*N + i sample i of prompt b, as HF does; the engine loop prefills each prompt
+        once and its N rows share the prompt's KV cache.  With past_key_values it raises NotImplementedError (run it
+        with use_hf_loop=True)."""
         if bboxes is None:
             bboxes = getattr(getattr(self, 'forward', None), 'keywords', {}).get('bboxes')
         if use_hf_loop:
@@ -836,10 +849,14 @@ class SPILlavaMPTForCausalLM(LlamaForCausalLM, _EngineHost):
                                 early_stopping=beam['early_stopping'], num_return_sequences=beam['num_return_sequences'],
                                 eos_token_id=beam['eos_token_id'], pad_token_id=beam['pad_token_id'],
                                 attention_mask=kwargs.get('attention_mask'))
+        nrs = resolve_num_return_sequences(self, do_sample, temperature, **gen)
         do_sample, temperature, top_k, top_p = resolve_sampling(self, input_ids.shape[1], do_sample, temperature, **gen)
+        pkv = kwargs.get('past_key_values')
+        if nrs > 1 and pkv is not None:
+            raise NotImplementedError('several sampled answers per prompt (num_return_sequences=%d) on a conversation '
+                                      'cache (past_key_values) run on the HF loop only: pass use_hf_loop=True' % nrs)
         eng = self._get_engine(input_ids.device)
         kv = None
-        pkv = kwargs.get('past_key_values')
         if pkv is not None:   # a conversation's cache: reused and left holding this turn too
             cache = _find_cache(pkv)
             if cache is None:
@@ -851,7 +868,8 @@ class SPILlavaMPTForCausalLM(LlamaForCausalLM, _EngineHost):
                             temperature=temperature, top_k=top_k, top_p=top_p, stopping_criteria=stopping_criteria,
                             eos_token_id=eos_token_id, attention_mask=kwargs.get('attention_mask'),
                             pad_token_id=kwargs.get('pad_token_id'), cache=kv, generator=kwargs.get('generator'),
-                            stop_strings=None if stops is None else stop_strings_from_tokenizer(kwargs['tokenizer'], stops))
+                            stop_strings=None if stops is None else stop_strings_from_tokenizer(kwargs['tokenizer'], stops),
+                            num_return_sequences=nrs)
 
     def initialize_vision_tokenizer(self, mm_use_im_start_end, tokenizer, device, tune_mm_mlp_adapter=False,
                                     pretrain_mm_mlp_adapter=None):

@@ -290,6 +290,18 @@ int g4r_decode_attention_rows_bf16(const void* q, long long ldq, const void* kca
 int g4r_decode_attention_beam_bf16(const void* q, long long ldq, const void* kcache, const void* vcache,
                                    void* out, long long ldo, int R, int H, int head_dim, int kv_bound,
                                    const int* pos_rows, const int* anc, int Lmax, float scale, void* stream);
+/* Decode attention for N sampled rows per prompt that share the prompt's keys (generate(num_return_sequences=N,
+ * do_sample=True)): caches [B + B*N, Lmax, H*head_dim], rows 0..B-1 the prompts, row B + r the generated positions of
+ * query row r = b*N + i (q: B*N rows of pitch ldq; out: B*N rows of pitch ldo).  Row r attends over positions
+ * 0..prompt_lens[b]-1 of cache row b and prompt_lens[b]..pos_rows[r] of cache row B + r (prompt_lens: device int32
+ * [B]; pos_rows: device int32 [B*N], pos_rows[r] >= prompt_lens[b] - 1).  Each prompt key / value row is read from HBM
+ * once per step for all N rows.  prompt_bound (>= every prompt_lens[b]) and gen_bound (>= every row's count of own
+ * keys, pos_rows[r] + 1 - prompt_lens[b]) size the split-KV factor and the score buffer.  1 <= N <= 16, head_dim 128;
+ * anything else is refused. */
+int g4r_decode_attention_group_bf16(const void* q, long long ldq, const void* kcache, const void* vcache,
+                                    void* out, long long ldo, int B, int N, int H, int head_dim, int prompt_bound,
+                                    int gen_bound, const int* prompt_lens, const int* pos_rows, int Lmax, float scale,
+                                    void* stream);
 
 /* ---- beam search step (the beam decode loop's last two kernels) -----------------------------
  * One step of transformers' GenerationMixin._beam_search with do_sample=False for B samples of N beams, on logits
@@ -705,6 +717,10 @@ int g4r_sample_tokens_f16(const void* logits, long long ld, int B, int V, float 
 int g4r_decode_attention_beam_f16(const void* q, long long ldq, const void* kcache, const void* vcache,
                                   void* out, long long ldo, int R, int H, int head_dim, int kv_bound,
                                   const int* pos_rows, const int* anc, int Lmax, float scale, void* stream);
+int g4r_decode_attention_group_f16(const void* q, long long ldq, const void* kcache, const void* vcache,
+                                   void* out, long long ldo, int B, int N, int H, int head_dim, int prompt_bound,
+                                   int gen_bound, const int* prompt_lens, const int* pos_rows, int Lmax, float scale,
+                                   void* stream);
 int g4r_beam_step_f16(const void* logits, long long ld, int row_div, int B, int N, int V, int K, const int* eos_ids,
                       int n_eos, int prompt_len, int max_length, double length_penalty, int early_stopping, int G,
                       int Lmax, const int* lens, int* state, float* run_score, float* cand_score, int* cand_tok,
