@@ -95,10 +95,370 @@ __device__ __forceinline__ void suffix_scan(T v, T* tot, T& incl, T& excl) {
   __syncthreads();   // tot is reused by the next scan
 }
 
+// ---- the processed variant (g4r_sample_tokens_proc_*): transformers' history-dependent logits processors first
+// (RepetitionPenaltyLogitsProcessor, NoRepeatNGramLogitsProcessor, MinLengthLogitsProcessor,
+// MinNewTokensLengthLogitsProcessor), then the selection above on the processed fp32 scores.  The row's history
+// h[0, L + *rng_step) becomes two bitmaps in shared memory: `pres` (ids present: the penalised ones) and `ban` (ids
+// set to -inf: the n-gram matches, and the eos ids while a minimum length is in force).  Greedy compares fp32 order
+// keys of the processed values.  Sampling keeps the 16-bit histogram for the untouched ids; the penalised ids are not
+// 16-bit values, so they form a list (fp32 order key << 32 | ~index) sorted descending, which every per-thread walk
+// merges into its bins: thread t owns the list entries whose value rounds down to one of its 64 keys, an entry strictly
+// above its bin comes before the bin, one equal to it joins the bin's group.  Thresholds are fp32 order keys, so equal
+// processed values form one group whichever set they come from.
+constexpr int PROC_LIST_MAX = 8192;   // penalised ids a sampled row may hold: 64 KB of shared memory
+
+struct SampleProc {
+  long long* hist;        // int64 [B, ld_h]: row b's history, L + *rng_step ids long
+  long long ld_h;
+  int L;
+  float penalty;          // 1: off
+  int ngram;              // 0: off
+  int min_length, min_new_tokens;
+  const int* eos_ids;     // the ids min_length / min_new_tokens suppress
+  int n_eos;
+  int append;             // write the selected token to h[b, L + *rng_step]
+};
+
+// Order key of an fp32 value: ascends with the value; -0 folded onto +0, every NaN onto the top key (torch.argmax).
+__device__ __forceinline__ unsigned f32_key(float y) {
+  if (y != y) return 0xFFFFFFFFu;
+  const unsigned u = __float_as_uint(y == 0.f ? 0.f : y);
+  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+__device__ __forceinline__ float f32_of_key(unsigned k) {
+  return __uint_as_float((k & 0x80000000u) ? (k & 0x7FFFFFFFu) : ~k);
+}
+// The largest 16-bit value <= y, as bits (rounding toward -inf).
+#ifdef G4R_ACT_HALF
+__device__ __forceinline__ unsigned bits_rd(float y) { return __half_as_ushort(__float2half_rd(y)); }
+#else
+__device__ __forceinline__ unsigned bits_rd(float y) {
+  const unsigned u = __float_as_uint(y);
+  return (u >> 16) + (((u & 0xFFFFu) && (u >> 31)) ? 1u : 0u);
+}
+#endif
+__device__ __forceinline__ bool bit_of(const unsigned* bm, int i) { return (bm[i >> 5] >> (i & 31)) & 1u; }
+
+// The processed units (distinct values, with counts) of thread `key0 >> 6`, from its top key down: f(order key,
+// value, count) returns false to stop.  list[n0, n1) is the thread's part of the sorted penalised list.
+template <typename F>
+__device__ __forceinline__ void walk_units(const unsigned* hist, const unsigned long long* list, int n0, int n1,
+                                           unsigned key0, F&& f) {
+  int n = n0;
+  for (int j = 63; j >= 0; j--) {
+    const unsigned key = key0 + j;
+    int c = (int)bin_count(hist, key);
+    if (n >= n1 && !c) continue;   // no list entry left and an empty bin: as cheap as the plain kernel's walk
+    while (n < n1) {   // penalised values strictly between this bin's value and the next bin's
+      const unsigned yk = (unsigned)(list[n] >> 32);
+      const float y = f32_of_key(yk);
+      const unsigned bits = bits_rd(y);
+      if (order_key(bits) != key || bits_value(bits) == y) break;
+      int cy = 1;
+      for (n++; n < n1 && (unsigned)(list[n] >> 32) == yk; n++) cy++;
+      if (!f(yk, y, cy)) return;
+    }
+    const float v = key_value(key);
+    const unsigned vk = f32_key(v);
+    for (; n < n1 && (unsigned)(list[n] >> 32) == vk; n++) c++;   // penalised values equal to this bin's
+    if (c && !f(vk, v, c)) return;
+  }
+}
+
+// Which thread's keys a list entry's value rounds down to.
+__device__ __forceinline__ int list_owner(unsigned long long e) {
+  return (int)(order_key(bits_rd(f32_of_key((unsigned)(e >> 32)))) >> 6);
+}
+
+__device__ void select_processed(const unsigned short* __restrict__ row, int V, float temperature, int top_k,
+                                 float top_p, int greedy, unsigned long long seed, const long long* __restrict__ rng_step,
+                                 const SampleProc& pr, unsigned* smem, int& s_tok) {
+  __shared__ unsigned long long s_best[32];
+  __shared__ int s_int[32];
+  __shared__ float s_flt[32];
+  __shared__ int s_P, s_find, s_low, s_j;
+  __shared__ unsigned s_maxk, s_kthr, s_pthr, s_sel;
+  __shared__ float s_zk;
+  const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int W = (V + 31) >> 5;
+  unsigned* hist = smem;
+  unsigned* pres = smem + (greedy ? 0 : SAMPLE_SMEM_WORDS);
+  unsigned* ban = pres + W;
+  unsigned long long* list = (unsigned long long*)(ban + W);
+  const long long step = *rng_step;
+  const long long* h = pr.hist + (long long)b * pr.ld_h;
+  const int Lh = (int)min((long long)pr.L + step, pr.ld_h);
+  const bool pen = pr.penalty != 1.f;
+  const float p = pr.penalty;
+
+  // ---- the bitmaps of the history
+  for (int i = tid; i < 2 * W; i += SAMPLE_THREADS) pres[i] = 0u;
+  if (tid == 0) s_tok = 0;
+  __syncthreads();
+  if (pen)
+    for (int j = tid; j < Lh; j += SAMPLE_THREADS) {
+      const long long t = h[j];
+      if (t >= 0 && t < V) atomicOr(&pres[t >> 5], 1u << (t & 31));
+    }
+  const int n = pr.ngram;
+  if (n > 0 && Lh + 1 >= n) {   // ban t when h[j, j + n) == (the last n - 1 ids of h, t)
+    const long long* tail = h + Lh - (n - 1);
+    for (int j = tid; j + n <= Lh; j += SAMPLE_THREADS) {
+      bool m = true;
+      for (int q = 0; q < n - 1 && m; q++) m = h[j + q] == tail[q];
+      const long long t = h[j + n - 1];
+      if (m && t >= 0 && t < V) atomicOr(&ban[t >> 5], 1u << (t & 31));
+    }
+  }
+  if (Lh < pr.min_length || step < pr.min_new_tokens)
+    for (int e = tid; e < pr.n_eos; e += SAMPLE_THREADS) {
+      const int t = pr.eos_ids[e];
+      if (t >= 0 && t < V) atomicOr(&ban[t >> 5], 1u << (t & 31));
+    }
+  __syncthreads();
+  // processed value of id i (false: banned, -inf)
+  auto value = [&](int i, float& y) -> bool {
+    if (bit_of(ban, i)) return false;
+    y = bits_value(row[i]);
+    if (pen && bit_of(pres, i)) y = y < 0.f ? __fmul_rn(y, p) : __fdiv_rn(y, p);
+    return true;
+  };
+
+  if (greedy) {
+    // arg-max of the processed fp32 scores, first index among equals
+    unsigned long long best = 0;
+    for (int i = tid; i < V; i += SAMPLE_THREADS) {
+      float y;
+      const unsigned k = value(i, y) ? f32_key(y) : f32_key(-INFINITY);
+      const unsigned long long q = ((unsigned long long)k << 32) | (0xFFFFFFFFu - (unsigned)i);
+      best = q > best ? q : best;
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const unsigned long long x = __shfl_xor_sync(0xffffffffu, best, o);
+      best = x > best ? x : best;
+    }
+    if (lane == 0) s_best[warp] = best;
+    __syncthreads();
+    if (tid == 0) {
+      for (int w = 1; w < 32; w++) best = s_best[w] > best ? s_best[w] : best;
+      s_tok = (int)(0xFFFFFFFFu - (unsigned)best);
+    }
+    return;
+  }
+
+  // ---- histogram of the untouched ids; the penalised ids listed in index order
+  for (int i = tid; i < SAMPLE_SMEM_WORDS; i += SAMPLE_THREADS) hist[i] = 0u;
+  if (tid == 0) {
+    s_P = 0;
+    s_maxk = 0u;
+    s_kthr = 0u;
+    s_find = -1;
+  }
+  __syncthreads();
+  for (int i = tid; i < V; i += SAMPLE_THREADS) {
+    if (bit_of(ban, i) || (pen && bit_of(pres, i))) continue;
+    const unsigned key = order_key(row[i]);
+    atomicAdd(&hist[hist_word(key)], 1u << ((key & 1) * 16));
+  }
+  __syncthreads();   // the counts land in other threads' bins: complete before any walk reads them
+  if (pen) {
+    for (int base = 0; base < W; base += SAMPLE_THREADS) {
+      const int w = base + SAMPLE_THREADS - 1 - tid;   // reversed, so the suffix scan gives index-order offsets
+      unsigned m = w < W ? pres[w] & ~ban[w] : 0u;
+      int c_incl, c_excl;
+      suffix_scan(__popc(m), s_int, c_incl, c_excl);
+      int at = s_P + c_excl;
+      for (; m; m &= m - 1) {
+        const int i = w * 32 + __ffs(m) - 1;
+        float y;
+        value(i, y);
+        if (at < PROC_LIST_MAX) list[at] = ((unsigned long long)f32_key(y) << 32) | (0xFFFFFFFFu - (unsigned)i);
+        at++;
+      }
+      __syncthreads();
+      if (tid == 0) s_P += c_incl;   // thread 0 holds the chunk total
+      __syncthreads();
+    }
+  }
+  const int P = min(s_P, PROC_LIST_MAX);
+  // ---- bitonic sort of the list, descending: (value desc, index asc); zero keys pad it to a power of two
+  int Pp = 1;
+  while (Pp < P) Pp <<= 1;
+  if (P > 1) {
+    for (int i = P + tid; i < Pp; i += SAMPLE_THREADS) list[i] = 0ull;
+    __syncthreads();
+    for (int size = 2; size <= Pp; size <<= 1)
+      for (int stride = size >> 1; stride > 0; stride >>= 1) {
+        for (int i = tid; i < (Pp >> 1); i += SAMPLE_THREADS) {
+          const int lo = 2 * i - (i & (stride - 1)), hi = lo + stride;
+          const unsigned long long x = list[lo], y = list[hi];
+          if ((x < y) == ((lo & size) == 0)) {
+            list[lo] = y;
+            list[hi] = x;
+          }
+        }
+        __syncthreads();
+      }
+  }
+  // ---- this thread's part of the list: the entries whose values round down to its keys
+  int n0 = 0, n1 = 0;
+  {
+    int lo = 0, hi = P;   // first entry owned by a thread <= tid
+    while (lo < hi) {
+      const int mid = (lo + hi) >> 1;
+      if (list_owner(list[mid]) <= tid) hi = mid; else lo = mid + 1;
+    }
+    n0 = lo;
+    hi = P;               // first entry owned by a thread < tid
+    while (lo < hi) {
+      const int mid = (lo + hi) >> 1;
+      if (list_owner(list[mid]) < tid) hi = mid; else lo = mid + 1;
+    }
+    n1 = lo;
+  }
+  const unsigned key0 = (unsigned)tid * 64;
+  // ---- counts; the top value
+  int cnt = 0, top_c = 0;
+  unsigned top_k32 = 0u;
+  walk_units(hist, list, n0, n1, key0, [&](unsigned k, float, int c) {
+    if (!top_c) {
+      top_k32 = k;
+      top_c = c;
+    }
+    cnt += c;
+    return true;
+  });
+  if (top_c) atomicMax(&s_maxk, top_k32);
+  int c_incl, c_excl;
+  suffix_scan(cnt, s_int, c_incl, c_excl);   // its barriers publish s_maxk
+  const unsigned maxk = s_maxk;
+  // ---- top-k: the k-th largest processed value, counting duplicates
+  if (top_k > 0 && top_k < V) {
+    if (c_incl >= top_k) atomicMax(&s_find, tid);
+    __syncthreads();
+    if (tid == s_find) {
+      int c0 = c_excl;
+      walk_units(hist, list, n0, n1, key0, [&](unsigned k, float, int c) {
+        c0 += c;
+        if (c0 >= top_k) s_kthr = k;
+        return c0 < top_k;
+      });
+    }
+    __syncthreads();
+  }
+  const unsigned kthr = s_kthr;
+  // ---- masses of the top-k survivors
+  const float smax = __fdiv_rn(f32_of_key(maxk), temperature);
+  float mass = 0.f;
+  walk_units(hist, list, n0, n1, key0, [&](unsigned k, float y, int c) {
+    if (k < kthr) return false;
+    mass += (float)c * expf(__fdiv_rn(y, temperature) - smax);
+    return true;
+  });
+  float m_incl, m_excl;
+  suffix_scan(mass, s_flt, m_incl, m_excl);
+  const float z = s_flt[0];
+  // ---- top-p over the processed groups
+  unsigned thr = kthr;
+  if (tid == 0) s_zk = z;
+  if (top_p < 1.f) {
+    const float pz = top_p * z;
+    __syncthreads();
+    if (tid == 0) {
+      s_find = SAMPLE_THREADS;
+      s_pthr = maxk;   // top_p <= 0: the top value alone
+    }
+    if (top_c && top_k32 == maxk) s_zk = (float)top_c * expf(__fdiv_rn(f32_of_key(maxk), temperature) - smax);
+    __syncthreads();
+    if (top_p > 0.f && m_excl < pz) atomicMin(&s_find, tid);
+    __syncthreads();
+    if (tid == s_find) {
+      float cum = m_excl;
+      walk_units(hist, list, n0, n1, key0, [&](unsigned k, float y, int c) {
+        if (k < kthr || !(cum < pz)) return false;
+        cum += (float)c * expf(__fdiv_rn(y, temperature) - smax);
+        s_pthr = k;
+        s_zk = cum;
+        return true;
+      });
+    }
+    __syncthreads();
+    thr = max(thr, s_pthr);
+  }
+  __syncthreads();
+  // ---- inverse CDF over the kept groups, from the top; a thread with kept groups takes it when rounding leaves the
+  // target past every thread's inclusive mass
+  const uint4 r = philox4x32_10(make_uint4((unsigned)step, (unsigned)((unsigned long long)step >> 32), (unsigned)b, 0u),
+                                make_uint2((unsigned)seed, (unsigned)(seed >> 32)));
+  const float target = (float)(r.x >> 8) * 0x1p-24f * s_zk;
+  if (tid == 0) {
+    s_find = -1;
+    s_low = SAMPLE_THREADS;
+    s_sel = 0u;   // no group at all (every id banned): no id matches, token 0
+    s_j = 0;
+  }
+  __syncthreads();
+  if (m_incl > target) atomicMax(&s_find, tid);
+  if (top_c && top_k32 >= thr) atomicMin(&s_low, tid);
+  __syncthreads();
+  if (tid == (s_find >= 0 ? s_find : s_low)) {
+    float cum = m_excl;
+    unsigned last = 0u;
+    int last_c = 0;
+    bool hit = false;
+    walk_units(hist, list, n0, n1, key0, [&](unsigned k, float y, int c) {
+      if (k < thr) return false;
+      const float e = expf(__fdiv_rn(y, temperature) - smax);
+      const float m = (float)c * e;
+      if (cum + m > target) {
+        const int jj = (int)((target - cum) / e);
+        s_sel = k;
+        s_j = min(max(jj, 0), c - 1);
+        hit = true;
+        return false;
+      }
+      cum += m;
+      last = k;
+      last_c = c;
+      return true;
+    });
+    if (!hit && last_c) {   // rounding left the target past this thread's last kept group: its last occurrence
+      s_sel = last;
+      s_j = last_c - 1;
+    }
+  }
+  __syncthreads();
+  // ---- the s_j-th id, in index order, whose processed value is the chosen one
+  const unsigned sel = s_sel;
+  const int jsel = s_j;
+  int seen = 0;
+  for (int base = 0; base < V; base += SAMPLE_THREADS) {
+    const int i = base + tid;
+    float y;
+    const bool hit = i < V && value(i, y) && f32_key(y) == sel;
+    const int nh = __syncthreads_count(hit);
+    if (seen + nh > jsel) {
+      const unsigned ball = __ballot_sync(0xffffffffu, hit);
+      if (lane == 0) s_int[warp] = __popc(ball);
+      __syncthreads();
+      if (hit) {
+        int rank = seen + __popc(ball & ((1u << lane) - 1u));
+        for (int w = 0; w < warp; w++) rank += s_int[w];
+        if (rank == jsel) s_tok = i;
+      }
+      break;
+    }
+    seen += nh;
+  }
+}
+
+template <bool PROC>
 __global__ void __launch_bounds__(SAMPLE_THREADS, 1)
 sample_tokens_kernel(const unsigned short* __restrict__ logits, long long ld, int V, float temperature, int top_k,
                      float top_p, int greedy, unsigned long long seed, const long long* __restrict__ rng_step,
-                     int eos_id, int pad_id, int* __restrict__ finished, long long* __restrict__ out_ids) {
+                     int eos_id, int pad_id, int* __restrict__ finished, long long* __restrict__ out_ids,
+                     SampleProc proc) {
   extern __shared__ unsigned hist[];
   __shared__ unsigned long long s_best[32];
   __shared__ int s_int[32];
@@ -108,7 +468,9 @@ sample_tokens_kernel(const unsigned short* __restrict__ logits, long long ld, in
   const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const unsigned short* row = logits + (long long)b * ld;
 
-  if (greedy) {
+  if constexpr (PROC) {
+    select_processed(row, V, temperature, top_k, top_p, greedy, seed, rng_step, proc, hist, s_tok);
+  } else if (greedy) {
     // arg-max, first index among equals (torch.argmax)
     unsigned long long best = 0;
     for (int i = tid; i < V; i += SAMPLE_THREADS) {
@@ -279,6 +641,10 @@ sample_tokens_kernel(const unsigned short* __restrict__ logits, long long ld, in
       else if (tok == eos_id) finished[b] = 1;
     }
     out_ids[b] = tok;
+    if constexpr (PROC) {   // the history the next step reads: h[b, L + step] = the token selected now
+      const long long at = (long long)proc.L + *rng_step;
+      if (proc.append && at < proc.ld_h) proc.hist[(long long)b * proc.ld_h + at] = tok;
+    }
   }
 }
 
@@ -296,12 +662,52 @@ extern "C" int g4r_sample_tokens_bf16(const void* logits, long long ld, int B, i
   cudaStream_t st = (cudaStream_t)stream;
   static bool set = false;
   if (!set) {
-    G4R_CUDA(cudaFuncSetAttribute(sample_tokens_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SAMPLE_SMEM));
+    G4R_CUDA(cudaFuncSetAttribute(sample_tokens_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                  (int)SAMPLE_SMEM));
     set = true;
   }
-  sample_tokens_kernel<<<B, SAMPLE_THREADS, greedy ? 0 : SAMPLE_SMEM, st>>>(
+  sample_tokens_kernel<false><<<B, SAMPLE_THREADS, greedy ? 0 : SAMPLE_SMEM, st>>>(
       (const unsigned short*)logits, ld, V, temperature, top_k, top_p, greedy, seed, rng_step, eos_id, pad_id, finished,
-      out_ids);
+      out_ids, SampleProc{});
   G4R_LAUNCH_CHECK("sample_tokens");
+  return G4R_OK;
+}
+
+extern "C" int g4r_sample_tokens_proc_bf16(const void* logits, long long ld, int B, int V, float temperature, int top_k,
+                                           float top_p, int greedy, unsigned long long seed, const long long* rng_step,
+                                           int eos_id, int pad_id, int* finished, long long* out_ids,
+                                           long long* history, long long ld_h, int L, float repetition_penalty,
+                                           int no_repeat_ngram_size, int min_length, int min_new_tokens,
+                                           const int* eos_ids, int n_eos, int append, void* stream) {
+  G4R_REQUIRE(logits && out_ids && B > 0 && V > 0 && V < 65536 && ld >= V,
+              "sample_tokens_proc: bad arguments (B=%d V=%d ld=%lld; V < 65536)", B, V, ld);
+  G4R_REQUIRE(greedy || (temperature > 0.f && top_p >= 0.f),
+              "sample_tokens_proc: sampling needs temperature > 0 and top_p >= 0 (T=%g top_p=%g)", (double)temperature,
+              (double)top_p);
+  G4R_REQUIRE(history && rng_step && L >= 0 && ld_h >= L && repetition_penalty > 0.f && no_repeat_ngram_size >= 0 &&
+                  n_eos >= 0 && (n_eos == 0 || eos_ids),
+              "sample_tokens_proc: bad processor arguments (L=%d ld_h=%lld penalty=%g n=%d n_eos=%d; the history and "
+              "rng_step are required, penalty > 0)", L, ld_h, (double)repetition_penalty, no_repeat_ngram_size, n_eos);
+  const bool listed = !greedy && repetition_penalty != 1.f;
+  G4R_REQUIRE(!listed || ld_h <= PROC_LIST_MAX,
+              "sample_tokens_proc: sampling with a repetition penalty holds at most %d history ids per row (ld_h=%lld)",
+              PROC_LIST_MAX, ld_h);
+  int list_n = 1;
+  while (listed && list_n < ld_h) list_n <<= 1;
+  const size_t smem = (greedy ? 0 : SAMPLE_SMEM) + 2 * sizeof(unsigned) * ((V + 31) / 32) +
+                      (listed ? list_n * sizeof(unsigned long long) : 0);
+  cudaStream_t st = (cudaStream_t)stream;
+  static bool set = false;
+  if (!set) {
+    const size_t most = SAMPLE_SMEM + 2 * sizeof(unsigned) * 2048 + PROC_LIST_MAX * sizeof(unsigned long long);
+    G4R_CUDA(cudaFuncSetAttribute(sample_tokens_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)most));
+    set = true;
+  }
+  SampleProc pr{history, ld_h, L, repetition_penalty, no_repeat_ngram_size, min_length, min_new_tokens, eos_ids, n_eos,
+                append};
+  sample_tokens_kernel<true><<<B, SAMPLE_THREADS, smem, st>>>(
+      (const unsigned short*)logits, ld, V, temperature, top_k, top_p, greedy, seed, rng_step, eos_id, pad_id, finished,
+      out_ids, pr);
+  G4R_LAUNCH_CHECK("sample_tokens_proc");
   return G4R_OK;
 }

@@ -876,6 +876,54 @@ class StopStrings:
         return state.to(torch.int32)
 
 
+class LogitsProcessors:
+    """transformers' history-dependent logits processors for one decode loop, in HF's order: RepetitionPenalty-
+    (repetition_penalty != 1), NoRepeatNGram- (no_repeat_ngram_size > 0), MinLength- and MinNewTokensLengthLogitsProcessor
+    (min_length / min_new_tokens > 0, suppressing `eos_ids`).  history: int64 [R, ld_h] -- row r's prompt as given (pads
+    included), then the tokens selected so far; the selection of new token s reads history[r, :L + s] and writes the
+    token it selects to history[r, L + s] (kernels.sample_tokens_processed), so the loop's output buffer serves."""
+
+    def __init__(self, history, L, repetition_penalty=1.0, no_repeat_ngram_size=0, min_length=0, min_new_tokens=0,
+                 eos_ids=()):
+        self.history, self.L = history, int(L)
+        self.repetition_penalty = 1.0 if repetition_penalty is None else float(repetition_penalty)
+        self.no_repeat_ngram_size = int(no_repeat_ngram_size or 0)
+        self.min_length, self.min_new_tokens = int(min_length or 0), int(min_new_tokens or 0)
+        self.eos_list = [int(e) for e in eos_ids]
+        self.eos_ids = (torch.tensor(self.eos_list, dtype=torch.int32, device=history.device) if self.eos_list
+                        else None)
+
+    @staticmethod
+    def neutral(repetition_penalty=1.0, no_repeat_ngram_size=0, min_length=0, min_new_tokens=0, eos_ids=()):
+        """True when none of the four would change a score (HF then builds none of them)."""
+        return ((repetition_penalty is None or float(repetition_penalty) == 1.0) and not no_repeat_ngram_size
+                and not ((min_length or min_new_tokens) and len(eos_ids)))
+
+    def apply(self, scores, step):
+        """The four processors restated with torch on fp32 scores [R, V] at new token `step` (the host stand-in path)."""
+        h = self.history[:, :self.L + step].to(scores.device)
+        Lh = h.shape[1]
+        p = self.repetition_penalty
+        if p != 1.0 and Lh:
+            x = scores.gather(1, h)
+            scores = scores.scatter(1, h, torch.where(x < 0, x * p, x / p))
+        n = self.no_repeat_ngram_size
+        if n > 0 and Lh + 1 >= n:
+            scores = scores.clone()
+            for r, row in enumerate(h.tolist()):
+                tail = row[Lh - n + 1:]
+                banned = sorted({row[j + n - 1] for j in range(Lh - n + 1) if row[j:j + n - 1] == tail})
+                scores[r, banned] = float('-inf')
+        if self.eos_list and (Lh < self.min_length or step < self.min_new_tokens):
+            scores = scores.clone()
+            scores[:, self.eos_list] = float('-inf')
+        return scores
+
+    def append(self, tok, step):
+        if self.L + step < self.history.shape[1]:
+            self.history[:, self.L + step] = tok.view(-1).to(self.history.device)
+
+
 class Sampler:
     """Next-token selection of the decode loop (kernels.sample_tokens): arg-max, or a draw from the temperature /
     top-k / top-p processed softmax, with transformers' eos -> pad rule when eos_id and pad_id are both given.
@@ -883,10 +931,12 @@ class Sampler:
     counter, advanced once per selected token) and `finished` (int32 [B], the rows that have emitted eos_id).
     stops (a StopStrings, with stop_state: each row's state after its prompt, int32 [B]): every call then ends with
     kernels.stop_step on the tokens just selected, which keeps the rows' matcher states in `stop_state` and sets
-    `finished` for a row whose token ends a stop string."""
+    `finished` for a row whose token ends a stop string.
+    processors (a LogitsProcessors): the selection runs on the scores its processors leave, reading each row's history
+    at length L + rng_step and appending the selected token to it (kernels.sample_tokens_processed)."""
 
     def __init__(self, B, device, greedy=True, temperature=1.0, top_k=None, top_p=None, seed=0, eos_id=None,
-                 pad_id=None, stops=None, stop_state=None):
+                 pad_id=None, stops=None, stop_state=None, processors=None):
         self.greedy = bool(greedy)
         self.temperature = float(temperature)
         self.top_k = 0 if top_k is None else int(top_k)
@@ -899,26 +949,40 @@ class Sampler:
         self.stop_table = None if stops is None else stops.on(device)
         if stops is not None:
             self.stop_state = torch.zeros_like(self.finished) if stop_state is None else stop_state.to(device, torch.int32)
+        self.processors = processors
 
     def __call__(self, logits, out, update=True):
-        """Select from logits [B, 1, V] into out (int64 [B, 1]).  update=False leaves `finished` and `stop_state` alone
-        (warm-up: the stop-string lookup then runs on copies, so that a graph capture is not its first launch)."""
+        """Select from logits [B, 1, V] into out (int64 [B, 1]).  update=False leaves `finished`, `stop_state` and the
+        processors' history alone (warm-up: the stop-string lookup then runs on copies, so that a graph capture is not
+        its first launch)."""
         if not logits.is_cuda:
             return self._host(logits, out, update)
-        kernels.sample_tokens(logits, out, self.greedy, self.temperature, self.top_k, self.top_p, self.seed,
-                              self.rng_step, self.eos_id, self.pad_id, self.finished if update else None)
+        pr = self.processors
+        if pr is None:
+            kernels.sample_tokens(logits, out, self.greedy, self.temperature, self.top_k, self.top_p, self.seed,
+                                  self.rng_step, self.eos_id, self.pad_id, self.finished if update else None)
+        else:
+            kernels.sample_tokens_processed(
+                logits, out, self.greedy, self.temperature, self.top_k, self.top_p, self.seed, self.rng_step,
+                self.eos_id, self.pad_id, self.finished if update else None, history=pr.history, L=pr.L,
+                repetition_penalty=pr.repetition_penalty, no_repeat_ngram_size=pr.no_repeat_ngram_size,
+                min_length=pr.min_length, min_new_tokens=pr.min_new_tokens, eos_ids=pr.eos_ids, append=update)
         if self.stop_table is not None:
             state, finished = (self.stop_state, self.finished) if update else (self.stop_state.clone(), self.finished.clone())
             kernels.stop_step(out, self.stop_table, state, finished)
         return out
 
     def _host(self, logits, out, update):
-        """Host tensors come only from CPU stand-ins of the engine (the loop's host-side tests): the arg-max and the
-        eos -> pad rule, restated.  Sampling exists on the device only."""
+        """Host tensors come only from CPU stand-ins of the engine (the loop's host-side tests): the arg-max (of the
+        processed fp32 scores with processors), the eos -> pad rule and the history append, restated.  Sampling exists
+        on the device only."""
         if not self.greedy:
             raise RuntimeError('token sampling runs on the CUDA device only (csrc/sample.cu): logits are on %s'
                                % logits.device)
-        tok = logits.reshape(logits.shape[0], -1).argmax(-1)
+        scores = logits.reshape(logits.shape[0], -1)
+        if self.processors is not None:
+            scores = self.processors.apply(scores.float(), int(self.rng_step))
+        tok = scores.argmax(-1)
         if update and self.eos_id >= 0:
             tok = torch.where(self.finished.bool(), torch.full_like(tok, self.pad_id), tok)
             self.finished |= (tok == self.eos_id).to(torch.int32)
@@ -927,6 +991,8 @@ class Sampler:
             state, hit = _stop_lookup(self.stop_table, tok, self.stop_state.to(torch.int64))
             self.stop_state = torch.where(live, state.to(torch.int32), self.stop_state)
             self.finished |= (live & hit).to(torch.int32)
+        if update and self.processors is not None:
+            self.processors.append(tok, int(self.rng_step))
         out.copy_(tok.view(out.shape))
         return out
 
@@ -945,7 +1011,8 @@ def sampling_seed(generator=None):
 def _generate(self, input_ids, images, bboxes, max_new_tokens=32, do_sample=False, temperature=1.0,
               stopping_criteria=None, eos_token_id=None, generator=None, use_graph=True, attention_mask=None,
               pad_token_id=None, cache=None, top_k=None, top_p=None, num_beams=1, length_penalty=1.0,
-              early_stopping=False, num_return_sequences=1, stop_strings=None):
+              early_stopping=False, num_return_sequences=1, stop_strings=None, repetition_penalty=1.0,
+              no_repeat_ngram_size=0, min_length=0, min_new_tokens=0, length_eos_ids=None):
     """Prefill + greedy / sampled decode (gpt4roi/app.py:286-300 calls
     model.generate(input_ids, images=..., do_sample=True, temperature=0.2, max_new_tokens=1024,
     stopping_criteria=[...]) with the boxes bound to forward).  Returns ids [B, L + new]: the prompt as given,
@@ -979,8 +1046,24 @@ def _generate(self, input_ids, images, bboxes, max_new_tokens=32, do_sample=Fals
     the same seed, up to the attention's summation order.  The prompts are prefilled once, at batch B, and the N rows
     of a prompt share its KV cache (SampleCache), whose keys the decode attention reads once per step for all N.
     Greedy selection with N > 1 raises ValueError, as HF does; a conversation cache (cache=) with N > 1 raises
-    NotImplementedError."""
+    NotImplementedError.
+    repetition_penalty, no_repeat_ngram_size, min_length, min_new_tokens: transformers' RepetitionPenalty-,
+    NoRepeatNGram-, MinLength- and MinNewTokensLengthLogitsProcessor, applied on the device before the selection, greedy
+    or sampled (LogitsProcessors; kernels.sample_tokens_processed), to each row's history: its prompt as given (pads
+    of a left-padded batch included; on a conversation cache the whole submitted prompt), then its new tokens (pads of
+    finished rows included).  length_eos_ids: the ids min_length / min_new_tokens suppress (HF's resolved eos list;
+    None: [eos_token_id] when one is given); they do not change when the loop stops or pads.  With all four neutral the
+    loop launches the kernels it launches without them.  Sampling with a repetition penalty holds at most
+    kernels.PROC_LIST_MAX history ids per row; beyond that, and with beam search, they raise NotImplementedError."""
+    if length_eos_ids is None:
+        length_eos_ids = [] if eos_token_id is None else (
+            list(eos_token_id) if isinstance(eos_token_id, (list, tuple)) else [eos_token_id])
+    neutral = LogitsProcessors.neutral(repetition_penalty, no_repeat_ngram_size, min_length, min_new_tokens,
+                                       length_eos_ids)
     if num_beams > 1:
+        if not neutral:
+            raise NotImplementedError('beam search with repetition_penalty / no_repeat_ngram_size / min_length / '
+                                      'min_new_tokens runs on the HF loop only: pass use_hf_loop=True')
         if do_sample:
             raise NotImplementedError('beam search with do_sample runs on the HF loop only: pass use_hf_loop=True')
         if stopping_criteria is not None:
@@ -1004,6 +1087,11 @@ def _generate(self, input_ids, images, bboxes, max_new_tokens=32, do_sample=Fals
         if cache is not None:
             raise NotImplementedError('several sampled answers per prompt (num_return_sequences=%d) on a conversation '
                                       'cache (cache=) run on the HF loop only: pass use_hf_loop=True' % N)
+    if not greedy and repetition_penalty is not None and float(repetition_penalty) != 1.0 \
+            and L + max_new_tokens > kernels.PROC_LIST_MAX:
+        raise NotImplementedError('sampling with repetition_penalty holds at most %d prompt + new tokens per row on the '
+                                  'engine loop (%d asked): pass use_hf_loop=True'
+                                  % (kernels.PROC_LIST_MAX, L + max_new_tokens))
     ids = input_ids.to(self.dev)
     if cache is not None:
         logits = self.prefill_cached(cache, input_ids, images, bboxes, attention_mask, new_tokens=max_new_tokens)
@@ -1030,10 +1118,13 @@ def _generate(self, input_ids, images, bboxes, max_new_tokens=32, do_sample=Fals
         stop_state = stop_strings.initial_states(*_right_padded(input_ids.cpu(), attention_mask)[:2])
         if N > 1:
             stop_state = stop_state.repeat_interleave(N)
-    sampler = Sampler(R, self.dev, greedy, temperature, top_k, top_p, seed=0 if greedy else sampling_seed(generator),
-                      eos_id=eos_token_id, pad_id=pad_token_id, stops=stop_strings, stop_state=stop_state)
     out = torch.empty((R, L + max_new_tokens), dtype=torch.int64, device=self.dev)
     out[:, :L] = ids if N == 1 else ids.repeat_interleave(N, 0)
+    procs = None if neutral else LogitsProcessors(out, L, repetition_penalty, no_repeat_ngram_size, min_length,
+                                                  min_new_tokens, length_eos_ids)   # `out` is the rows' history
+    sampler = Sampler(R, self.dev, greedy, temperature, top_k, top_p, seed=0 if greedy else sampling_seed(generator),
+                      eos_id=eos_token_id, pad_id=pad_token_id, stops=stop_strings, stop_state=stop_state,
+                      processors=procs)
     stepper = None
     if use_graph and max_new_tokens > 4 and self.cfg.head_dim == 128:
         stepper = GraphedDecode(self, cache, sampler=sampler)   # each replay also selects the next token into its ids

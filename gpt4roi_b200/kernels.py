@@ -234,6 +234,51 @@ def sample_tokens(logits, out, greedy, temperature=1.0, top_k=0, top_p=1.0, seed
     return out
 
 
+PROC_LIST_MAX = 8192   # history ids per row that sampling with a repetition penalty holds (csrc/sample.cu)
+
+
+def sample_tokens_processed(logits, out, greedy, temperature=1.0, top_k=0, top_p=1.0, seed=0, rng_step=None, eos_id=-1,
+                            pad_id=-1, finished=None, history=None, L=0, repetition_penalty=1.0, no_repeat_ngram_size=0,
+                            min_length=0, min_new_tokens=0, eos_ids=None, append=True):
+    """sample_tokens on the scores transformers' history-dependent processors leave (include/gpt4roi_b200.h:
+    g4r_sample_tokens_proc_bf16): RepetitionPenaltyLogitsProcessor, NoRepeatNGramLogitsProcessor, MinLengthLogitsProcessor
+    and MinNewTokensLengthLogitsProcessor, applied on the device to row b's history history[b, :L + rng_step].
+    history: contiguous device int64 [B, ld_h] (ld_h >= L); rng_step (device int64 [1]) is required, also for greedy;
+    eos_ids: device int32 [n] (None: none), the ids min_length / min_new_tokens suppress.  append: write the selected
+    id to history[b, L + rng_step] (after the eos -> pad rule)."""
+    rows, act = _logit_rows('sample_tokens_processed', logits)
+    B, V = rows.shape
+    if out.dtype != torch.int64 or out.numel() != B or not out.is_contiguous():
+        raise RuntimeError('sample_tokens_processed: out must be a contiguous int64 tensor of %d elements' % B)
+    if rng_step is None or rng_step.dtype != torch.int64 or rng_step.numel() != 1:
+        raise RuntimeError('sample_tokens_processed: rng_step must be a device int64 [1] counter')
+    if finished is not None and (finished.dtype != torch.int32 or finished.numel() != B or not finished.is_contiguous()):
+        raise RuntimeError('sample_tokens_processed: finished must be a contiguous device int32 [%d] vector' % B)
+    if history is None or history.dtype != torch.int64 or history.dim() != 2 or history.shape[0] != B \
+            or not history.is_contiguous():
+        raise RuntimeError('sample_tokens_processed: history must be a contiguous int64 [%d, ld_h] tensor' % B)
+    ld_h = history.shape[1]
+    if not 0 <= int(L) <= ld_h:
+        raise RuntimeError('sample_tokens_processed: the prompt length L=%d must lie in [0, %d]' % (L, ld_h))
+    if not repetition_penalty > 0 or int(no_repeat_ngram_size) < 0 or int(min_length) < 0 or int(min_new_tokens) < 0:
+        raise RuntimeError('sample_tokens_processed: repetition_penalty must be > 0 and the lengths >= 0 (got %r, %r, %r, '
+                           '%r)' % (repetition_penalty, no_repeat_ngram_size, min_length, min_new_tokens))
+    if not greedy and repetition_penalty != 1.0 and ld_h > PROC_LIST_MAX:
+        raise RuntimeError('sample_tokens_processed: sampling with a repetition penalty holds at most %d history ids per '
+                           'row (ld_h=%d)' % (PROC_LIST_MAX, ld_h))
+    if eos_ids is not None and (eos_ids.dtype != torch.int32 or eos_ids.dim() != 1 or not eos_ids.is_contiguous()):
+        raise RuntimeError('sample_tokens_processed: eos_ids must be a contiguous device int32 vector')
+    n_eos = 0 if eos_ids is None else eos_ids.numel()
+    _L.require_cuda_same_device([('logits', rows), ('out', out), ('rng_step', rng_step), ('finished', finished),
+                                 ('history', history), ('eos_ids', eos_ids)])
+    _call('g4r_sample_tokens_proc_bf16', rows.device, _L.ptr(rows), rows.stride(0), B, V, float(temperature),
+          int(top_k), float(top_p), int(bool(greedy)), int(seed) & 0xFFFFFFFFFFFFFFFF, _L.ptr(rng_step), int(eos_id),
+          int(pad_id), _L.ptr(finished), _L.ptr(out), _L.ptr(history), ld_h, int(L), float(repetition_penalty),
+          int(no_repeat_ngram_size), int(min_length), int(min_new_tokens), _L.ptr(eos_ids) if n_eos else None, n_eos,
+          int(bool(append)), act=act)
+    return out
+
+
 def stop_step(ids, table, state, finished):
     """Stop strings, one step: every row b with finished[b] == 0 advances its matcher state by the token ids[b] through
     table (int16 [V_tok + 1, S], engine.StopStrings) and sets finished[b] when an occurrence of a stop string ended in

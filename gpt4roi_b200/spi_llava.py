@@ -504,31 +504,79 @@ def _generation_config(model, given):
     return gc
 
 
-def resolve_sampling(model, input_len, do_sample=None, temperature=None, **kwargs):
-    """The engine loop's selection rule for a generate call, resolved as transformers resolves it: explicit kwargs, then
-    `generation_config=`, then model.generation_config, then HF's global defaults (GenerationMixin.
-    _prepare_generation_config; `do_sample=True` alone therefore samples with top_k=50).  Returns (do_sample,
-    temperature, top_k, top_p) with top_k 0 / top_p 1 meaning off.  A call whose resolved config would make HF apply
-    any logits processor beyond TemperatureLogitsWarper, TopKLogitsWarper and TopPLogitsWarper (repetition_penalty,
-    min_p, typical_p, no_repeat_ngram_size, a caller's logits_processor, ...), or run beam search, raises
-    NotImplementedError: the engine loop does not implement it, the HF loop (use_hf_loop=True) does."""
-    from transformers.generation.logits_process import TemperatureLogitsWarper, TopKLogitsWarper, TopPLogitsWarper
+def _resolve_selection(model, input_len, do_sample, temperature, kwargs):
+    """-> (do_sample, temperature, top_k, top_p), the history-dependent processors' parameters, the names of every
+    processor beyond the three warpers in HF's order, the names of those that are not history-dependent."""
+    from transformers.generation import logits_process as lp
     given = {k: v for k, v in dict(kwargs, do_sample=do_sample, temperature=temperature).items() if v is not None}
     gc = _generation_config(model, given)
     if (gc.num_beams or 1) > 1:
         raise NotImplementedError('beam search (num_beams=%d) runs on the HF loop only: pass use_hf_loop=True'
                                   % gc.num_beams)
+    if gc.min_new_tokens is not None:   # GenerationMixin._prepare_generated_length: min_new_tokens takes precedence
+        gc.min_length = gc.min_new_tokens + input_len
     procs = model._get_logits_processor(gc, input_ids_seq_length=input_len, device='cpu', model_kwargs={},
                                         logits_processor=kwargs.get('logits_processor'))
-    other = [type(p).__name__ for p in procs
-             if not isinstance(p, (TemperatureLogitsWarper, TopKLogitsWarper, TopPLogitsWarper))]
-    if other:
-        raise NotImplementedError('the engine loop applies temperature, top_k and top_p only; %s run on the HF loop: '
-                                  'pass use_hf_loop=True' % ', '.join(other))
+    found = dict(repetition_penalty=1.0, no_repeat_ngram_size=0, min_length=0, min_new_tokens=0, eos_ids=[])
+    names, other = [], []
+    for p in procs:
+        if isinstance(p, (lp.TemperatureLogitsWarper, lp.TopKLogitsWarper, lp.TopPLogitsWarper)):
+            continue
+        if type(p) is lp.RepetitionPenaltyLogitsProcessor and not p.prompt_ignore_length:
+            found['repetition_penalty'] = float(p.penalty)
+        elif type(p) is lp.NoRepeatNGramLogitsProcessor:
+            found['no_repeat_ngram_size'] = int(p.ngram_size)
+        elif type(p) is lp.MinLengthLogitsProcessor:
+            if p.min_length <= input_len:     # at most the prompt's length: it never suppresses anything
+                continue
+            found['min_length'] = int(p.min_length)
+            found['eos_ids'] = p.eos_token_id.flatten().tolist()
+        elif type(p) is lp.MinNewTokensLengthLogitsProcessor and p.prompt_length_to_skip == input_len:
+            found['min_new_tokens'] = int(p.min_new_tokens)
+            found['eos_ids'] = p.eos_token_id.flatten().tolist()
+        else:
+            other.append(type(p).__name__)
+        names.append(type(p).__name__)
     if not gc.do_sample:
-        return False, 1.0, 0, 1.0
-    return (True, float(gc.temperature if gc.temperature is not None else 1.0), int(gc.top_k or 0),
-            float(gc.top_p if gc.top_p is not None else 1.0))
+        rule = (False, 1.0, 0, 1.0)
+    else:
+        rule = (True, float(gc.temperature if gc.temperature is not None else 1.0), int(gc.top_k or 0),
+                float(gc.top_p if gc.top_p is not None else 1.0))
+    return rule, found, names, other
+
+
+def resolve_processors(model, input_len, do_sample=None, temperature=None, **kwargs):
+    """The engine loop's selection rule for a generate call, resolved as transformers resolves it: explicit kwargs, then
+    `generation_config=`, then model.generation_config, then HF's global defaults (GenerationMixin.
+    _prepare_generation_config; `do_sample=True` alone therefore samples with top_k=50), and read off the processors
+    HF's _get_logits_processor builds from it, after HF's length preparation (GenerationMixin.
+    _prepare_generated_length: a given min_new_tokens sets min_length to min_new_tokens + the input length).  Returns (do_sample, temperature, top_k, top_p, processors) with top_k 0 /
+    top_p 1 meaning off; processors: dict(repetition_penalty, no_repeat_ngram_size, min_length, min_new_tokens,
+    eos_ids) -- the history-dependent processors HF would apply (neutral values for those it does not build or that
+    can never suppress anything: min_length at most the input length, min_new_tokens 0), eos_ids
+    the resolved eos list (generation_config._eos_token_tensor: the eos_token_id kwarg, else the model's config) that
+    the minimum lengths suppress.  A call whose resolved config would make HF apply any other logits processor (min_p,
+    typical_p, epsilon / eta cutoffs, bad_words_ids, suppress_tokens, sequence_bias, a caller's logits_processor, ...),
+    or run beam search, raises NotImplementedError: the engine loop does not implement it, the HF loop
+    (use_hf_loop=True) does."""
+    rule, found, _, other = _resolve_selection(model, input_len, do_sample, temperature, kwargs)
+    if other:
+        raise NotImplementedError('the engine loop applies temperature, top_k, top_p, repetition_penalty, '
+                                  'no_repeat_ngram_size, min_length and min_new_tokens only; %s run on the HF loop: '
+                                  'pass use_hf_loop=True' % ', '.join(other))
+    return rule + (found,)
+
+
+def resolve_sampling(model, input_len, do_sample=None, temperature=None, **kwargs):
+    """resolve_processors for a selection without logits processors: returns (do_sample, temperature, top_k, top_p).
+    A call whose resolved config would make HF apply any logits processor beyond TemperatureLogitsWarper,
+    TopKLogitsWarper and TopPLogitsWarper (repetition_penalty, min_p, typical_p, no_repeat_ngram_size, a caller's
+    logits_processor, ...), or run beam search, raises NotImplementedError naming use_hf_loop=True."""
+    rule, _, names, _ = _resolve_selection(model, input_len, do_sample, temperature, kwargs)
+    if names:
+        raise NotImplementedError('the engine loop applies temperature, top_k and top_p only; %s run on the HF loop: '
+                                  'pass use_hf_loop=True' % ', '.join(names))
+    return rule
 
 
 def resolve_num_return_sequences(model, do_sample=None, temperature=None, **kwargs):
@@ -800,7 +848,9 @@ class SPILlavaMPTForCausalLM(LlamaForCausalLM, _EngineHost):
         Sampling on the engine loop follows HF's resolution of do_sample / temperature / top_k / top_p /
         generation_config (resolve_sampling: the demo's call samples from the top 50 at T = 0.2, as on the HF loop);
         the draws are keyed by torch's default generator (or `generator=`), so torch.manual_seed makes them
-        reproducible.  Other logits processors raise NotImplementedError there.
+        reproducible.  repetition_penalty, no_repeat_ngram_size, min_length and min_new_tokens (resolve_processors, with
+        HF's resolved eos list) run there too, on the device inside the decode step, greedy or sampled; other logits
+        processors raise NotImplementedError there.
         stop_strings (with tokenizer=, as transformers' generate takes them; resolve_stop_strings) are matched on the
         device, per row, inside the decode step (engine.StopStrings): a row that has produced a stop string is finished
         and, when eos_token_id and pad_token_id are given, filled with pad_token_id, as on the HF loop.  Host
@@ -850,7 +900,8 @@ class SPILlavaMPTForCausalLM(LlamaForCausalLM, _EngineHost):
                                 eos_token_id=beam['eos_token_id'], pad_token_id=beam['pad_token_id'],
                                 attention_mask=kwargs.get('attention_mask'))
         nrs = resolve_num_return_sequences(self, do_sample, temperature, **gen)
-        do_sample, temperature, top_k, top_p = resolve_sampling(self, input_ids.shape[1], do_sample, temperature, **gen)
+        do_sample, temperature, top_k, top_p, procs = resolve_processors(self, input_ids.shape[1], do_sample,
+                                                                         temperature, eos_token_id=eos_token_id, **gen)
         pkv = kwargs.get('past_key_values')
         if nrs > 1 and pkv is not None:
             raise NotImplementedError('several sampled answers per prompt (num_return_sequences=%d) on a conversation '
@@ -869,7 +920,9 @@ class SPILlavaMPTForCausalLM(LlamaForCausalLM, _EngineHost):
                             eos_token_id=eos_token_id, attention_mask=kwargs.get('attention_mask'),
                             pad_token_id=kwargs.get('pad_token_id'), cache=kv, generator=kwargs.get('generator'),
                             stop_strings=None if stops is None else stop_strings_from_tokenizer(kwargs['tokenizer'], stops),
-                            num_return_sequences=nrs)
+                            num_return_sequences=nrs, repetition_penalty=procs['repetition_penalty'],
+                            no_repeat_ngram_size=procs['no_repeat_ngram_size'], min_length=procs['min_length'],
+                            min_new_tokens=procs['min_new_tokens'], length_eos_ids=procs['eos_ids'])
 
     def initialize_vision_tokenizer(self, mm_use_im_start_end, tokenizer, device, tune_mm_mlp_adapter=False,
                                     pretrain_mm_mlp_adapter=None):

@@ -341,6 +341,30 @@ int g4r_sample_tokens_bf16(const void* logits, long long ld, int B, int V, float
                            int greedy, unsigned long long seed, const long long* rng_step, int eos_id, int pad_id,
                            int* finished, long long* out_ids, void* stream);
 
+/* ---- next-token selection with transformers' history-dependent logits processors ----------------
+ * g4r_sample_tokens_bf16 (same arguments, same selection and eos -> pad rule) on the processed fp32 scores that
+ * transformers' GenerationMixin._sample builds before TemperatureLogitsWarper (logits_process.py, in its order):
+ *   RepetitionPenaltyLogitsProcessor (repetition_penalty != 1): every id present in the history h gets
+ *     x < 0 ? x * penalty : x / penalty (fp32 multiply / IEEE division of the widened logit), once however often it
+ *     occurs;
+ *   NoRepeatNGramLogitsProcessor (no_repeat_ngram_size n > 0): when len(h) + 1 >= n, t gets -inf if an n-gram lying
+ *     wholly in h has its first n - 1 ids equal to the last n - 1 ids of h and ends in t (n = 1: every id of h);
+ *   MinLengthLogitsProcessor (len(h) < min_length) and MinNewTokensLengthLogitsProcessor (*rng_step < min_new_tokens):
+ *     eos_ids[0 .. n_eos) get -inf.
+ * Greedy: the arg-max of the processed scores, first index among equals.  Sampling: temperature -> top-k -> top-p ->
+ * inverse CDF as g4r_sample_tokens_bf16, over the processed values; -inf ids have probability 0 and equal processed
+ * values form one group whichever ids they come from.
+ * history: int64 [B, ld_h], row pitch ld_h; row b's history is h = history[b, 0 .. L + *rng_step) (the prompt as given,
+ * then the ids selected so far).  append != 0: after the eos -> pad rule, the selected id is written to
+ * history[b, L + *rng_step] (when that is < ld_h), so the next call sees it.  rng_step is required, also for greedy.
+ * Sampling with repetition_penalty != 1 needs ld_h <= 8192 (the penalised ids are listed in shared memory).  V < 65536.
+ * Capturable: every per-step value is read from device memory. */
+int g4r_sample_tokens_proc_bf16(const void* logits, long long ld, int B, int V, float temperature, int top_k,
+                                float top_p, int greedy, unsigned long long seed, const long long* rng_step, int eos_id,
+                                int pad_id, int* finished, long long* out_ids, long long* history, long long ld_h, int L,
+                                float repetition_penalty, int no_repeat_ngram_size, int min_length, int min_new_tokens,
+                                const int* eos_ids, int n_eos, int append, void* stream);
+
 /* ---- stop strings (after the next-token selection, once per decode step) ---------------------
  * Replaces transformers.generation.stopping_criteria.StopStringCriteria.__call__ (and, per row, the reference's
  * KeywordsStoppingCriteria, llava/model/utils.py:26-46) for the decode loop: a row stops at the first generated token
@@ -714,6 +738,11 @@ int g4r_attention_cached_f16(const void* q, long long ldq, const void* kcache, c
 int g4r_sample_tokens_f16(const void* logits, long long ld, int B, int V, float temperature, int top_k, float top_p,
                           int greedy, unsigned long long seed, const long long* rng_step, int eos_id, int pad_id,
                           int* finished, long long* out_ids, void* stream);
+int g4r_sample_tokens_proc_f16(const void* logits, long long ld, int B, int V, float temperature, int top_k,
+                               float top_p, int greedy, unsigned long long seed, const long long* rng_step, int eos_id,
+                               int pad_id, int* finished, long long* out_ids, long long* history, long long ld_h, int L,
+                               float repetition_penalty, int no_repeat_ngram_size, int min_length, int min_new_tokens,
+                               const int* eos_ids, int n_eos, int append, void* stream);
 int g4r_decode_attention_beam_f16(const void* q, long long ldq, const void* kcache, const void* vcache,
                                   void* out, long long ldo, int R, int H, int head_dim, int kv_bound,
                                   const int* pos_rows, const int* anc, int Lmax, float scale, void* stream);
