@@ -13,6 +13,12 @@
 // _beam_search_has_unfinished_sequences.  The last CTA to finish (an integer ticket) folds the samples' flags into the
 // batch's done word.  No float atomics and every float sum has a fixed order, so a replay is bitwise repeatable.
 //
+// Outputs (g4r_beam_step_out_*, transformers' return_dict_in_generate): kernel A writes every id's log-softmax value
+// (x - max) - log sum -- HF's scores entry, before the running score is added -- and the widened logit into slot g (the
+// sample's generated-token count, read from the device state, so graph replays fill successive slots) of fp32 buffers
+// [n_slots, B*N, V]; kernel B keeps a beam-index column beside the sequences (HF's beam_indices: b*N + parent beam at
+// column g, -1 where nothing was generated), double-buffered and gathered exactly as the sequences are.
+//
 // Beam KV layout (engine.BeamCache): cache rows 0..B-1 hold the prompts, rows B..B+B*N-1 the beams.  A cell is written
 // once and never moved; anc[r, p] names the cache row that holds position p of beam row r.  Reordering the beams
 // permutes the generated columns of anc (staged in shared memory) instead of copying K/V.
@@ -51,7 +57,9 @@ __device__ __forceinline__ float key_value(unsigned key) {
 
 __global__ void __launch_bounds__(TOPK_THREADS)
 beam_topk_kernel(const unsigned short* __restrict__ logits, long long ld, int row_div, int V, int K,
-                 const float* __restrict__ run_score, float* __restrict__ cand_score, int* __restrict__ cand_tok) {
+                 const float* __restrict__ run_score, float* __restrict__ cand_score, int* __restrict__ cand_tok,
+                 const int* __restrict__ state, int N, float* __restrict__ out_scores, float* __restrict__ out_logits,
+                 int n_slots) {
   extern __shared__ unsigned short keys[];   // [V] order keys of the row
   constexpr int W = TOPK_THREADS / 32;
   __shared__ unsigned long long s_best[W];
@@ -85,6 +93,17 @@ beam_topk_kernel(const unsigned short* __restrict__ logits, long long ld, int ro
   for (int w = 0; w < W; w++) tot += s_sum[w];
   const float logz = logf(tot);
   const float base = run_score[r];
+  if (out_scores || out_logits) {
+    const int slot = state[4 * (r / N)];
+    if (slot < n_slots) {
+      const long long o = ((long long)slot * gridDim.x + r) * V;
+      for (int i = tid; i < V; i += TOPK_THREADS) {
+        const float x = bits_value(row[i]);
+        if (out_scores) out_scores[o + i] = __fsub_rn(__fsub_rn(x, mx), logz);
+        if (out_logits) out_logits[o + i] = x;
+      }
+    }
+  }
   // top K by (value descending, index ascending): packed = key << 32 | ~index is unique per element, so the k-th pick
   // is the largest packed value below the (k-1)-th
   unsigned long long prev = ~0ULL;
@@ -118,14 +137,15 @@ beam_topk_kernel(const unsigned short* __restrict__ logits, long long ld, int ro
 // is_early_stop_heuristic_unsatisfied, [4b + 2] = flags (1: every finished slot filled, 2: every top-K candidate hit a
 // stopping criterion); state[4B] = ticket, state[4B + 1] = done (the whole batch).  fin_state (int32 [B, N, 2]): the
 // finished slot's is_sent_finished and generated length.  run_seq / fin_seq: int64 [2, B, N, G] generated columns,
-// double-buffered by the parity of g (read g & 1, write the other).
+// double-buffered by the parity of g (read g & 1, write the other); run_bidx / fin_bidx: int32 [2, B, N, G] beam-index
+// columns beside them, the same way (null: not kept).
 __global__ void __launch_bounds__(SEL_THREADS)
 beam_select_kernel(const float* __restrict__ cand_score, const int* __restrict__ cand_tok, int N, int K, int V,
                    const int* __restrict__ eos_ids, int n_eos, int prompt_len, int max_length, double length_penalty,
                    int early, int G, int Lmax, const int* __restrict__ lens, int* state, float* __restrict__ run_score,
                    long long* __restrict__ run_seq, long long* __restrict__ fin_seq, float* __restrict__ fin_score,
                    int* __restrict__ fin_state, long long* __restrict__ ids, int* __restrict__ pos_rows,
-                   int* __restrict__ anc) {
+                   int* __restrict__ anc, int* __restrict__ run_bidx, int* __restrict__ fin_bidx) {
   extern __shared__ int stage[];   // [N][g] generated columns of anc
   __shared__ float s_cs[BEAM_MAX_CAND];
   __shared__ int s_ct[BEAM_MAX_CAND];
@@ -250,6 +270,20 @@ beam_select_kernel(const float* __restrict__ cand_score, const int* __restrict__
       for (int i = tid; i < G; i += SEL_THREADS)
         fdst[(long long)j * G + i] = i == g ? s_tok[fk] : rsrc[(long long)fpar * G + i];
     }
+    if (run_bidx) {   // the beam indices, gathered as the sequences above
+      const int* rbs = run_bidx + ((long long)p * B + b) * N * G;
+      int* rbd = run_bidx + ((long long)(p ^ 1) * B + b) * N * G;
+      const int* fbs = fin_bidx + ((long long)p * B + b) * N * G;
+      int* fbd = fin_bidx + ((long long)(p ^ 1) * B + b) * N * G;
+      for (int i = tid; i < G; i += SEL_THREADS) rbd[(long long)j * G + i] = i == g ? b * N + par : rbs[(long long)par * G + i];
+      if (m < N) {
+        for (int i = tid; i < G; i += SEL_THREADS) fbd[(long long)j * G + i] = fbs[(long long)m * G + i];
+      } else {
+        const int fpar = s_par[m - N];
+        for (int i = tid; i < G; i += SEL_THREADS)
+          fbd[(long long)j * G + i] = i == g ? b * N + fpar : rbs[(long long)fpar * G + i];
+      }
+    }
     if (tid == 0) {
       arow[g] = B + b * N + j;   // cache row of beam row b*N+j (the B prompt rows come first): it writes position lens[b] + g
       ids[b * N + j] = s_tok[k];
@@ -280,18 +314,20 @@ beam_select_kernel(const float* __restrict__ cand_score, const int* __restrict__
 
 using namespace G4R_NS;
 
-extern "C" int g4r_beam_step_bf16(const void* logits, long long ld, int row_div, int B, int N, int V, int K,
-                                  const int* eos_ids, int n_eos, int prompt_len, int max_length, double length_penalty,
-                                  int early_stopping, int G, int Lmax, const int* lens, int* state, float* run_score,
-                                  float* cand_score, int* cand_tok, long long* run_seq, long long* fin_seq,
-                                  float* fin_score, int* fin_state, long long* ids, int* pos_rows, int* anc,
-                                  void* stream) {
+static int beam_step(const void* logits, long long ld, int row_div, int B, int N, int V, int K, const int* eos_ids,
+                     int n_eos, int prompt_len, int max_length, double length_penalty, int early_stopping, int G,
+                     int Lmax, const int* lens, int* state, float* run_score, float* cand_score, int* cand_tok,
+                     long long* run_seq, long long* fin_seq, float* fin_score, int* fin_state, long long* ids,
+                     int* pos_rows, int* anc, float* scores, float* raw_logits, int n_slots, int* run_bidx,
+                     int* fin_bidx, void* stream) {
   G4R_REQUIRE(logits && lens && state && run_score && cand_score && cand_tok && run_seq && fin_seq && fin_score &&
               fin_state && ids && pos_rows && anc && (n_eos == 0 || eos_ids),
               "beam_step: NULL argument");
   G4R_REQUIRE(B > 0 && N > 1 && N <= BEAM_MAX_N && K >= N && K <= BEAM_MAX_KEEP && N * K <= BEAM_MAX_CAND && V >= K &&
               ld >= V && (row_div == 1 || row_div == N) && G > 0 && early_stopping >= 0 && early_stopping <= 2,
               "beam_step: bad arguments (B=%d N=%d K=%d V=%d row_div=%d G=%d)", B, N, K, V, row_div, G);
+  G4R_REQUIRE((!scores && !raw_logits) || n_slots > 0, "beam_step: outputs need n_slots > 0 (n_slots=%d)", n_slots);
+  G4R_REQUIRE(!run_bidx == !fin_bidx, "beam_step: run_bidx and fin_bidx go together");
   const size_t smem_a = (size_t)V * sizeof(unsigned short);
   const size_t smem_b = (size_t)N * G * sizeof(int);
   G4R_REQUIRE(smem_a <= 200 * 1024 && smem_b <= 200 * 1024,
@@ -304,12 +340,35 @@ extern "C" int g4r_beam_step_bf16(const void* logits, long long ld, int row_div,
     set = true;
   }
   beam_topk_kernel<<<B * N, TOPK_THREADS, smem_a, st>>>((const unsigned short*)logits, ld, row_div, V, K, run_score,
-                                                         cand_score, cand_tok);
+                                                         cand_score, cand_tok, state, N, scores, raw_logits, n_slots);
   G4R_LAUNCH_CHECK("beam_topk");
   beam_select_kernel<<<B, SEL_THREADS, smem_b, st>>>(cand_score, cand_tok, N, K, V, eos_ids, n_eos, prompt_len,
                                                      max_length, length_penalty, early_stopping, G, Lmax, lens, state,
                                                      run_score, run_seq, fin_seq, fin_score, fin_state, ids, pos_rows,
-                                                     anc);
+                                                     anc, run_bidx, fin_bidx);
   G4R_LAUNCH_CHECK("beam_select");
   return G4R_OK;
+}
+
+extern "C" int g4r_beam_step_bf16(const void* logits, long long ld, int row_div, int B, int N, int V, int K,
+                                  const int* eos_ids, int n_eos, int prompt_len, int max_length, double length_penalty,
+                                  int early_stopping, int G, int Lmax, const int* lens, int* state, float* run_score,
+                                  float* cand_score, int* cand_tok, long long* run_seq, long long* fin_seq,
+                                  float* fin_score, int* fin_state, long long* ids, int* pos_rows, int* anc,
+                                  void* stream) {
+  return beam_step(logits, ld, row_div, B, N, V, K, eos_ids, n_eos, prompt_len, max_length, length_penalty,
+                   early_stopping, G, Lmax, lens, state, run_score, cand_score, cand_tok, run_seq, fin_seq, fin_score,
+                   fin_state, ids, pos_rows, anc, nullptr, nullptr, 0, nullptr, nullptr, stream);
+}
+
+extern "C" int g4r_beam_step_out_bf16(const void* logits, long long ld, int row_div, int B, int N, int V, int K,
+                                      const int* eos_ids, int n_eos, int prompt_len, int max_length,
+                                      double length_penalty, int early_stopping, int G, int Lmax, const int* lens,
+                                      int* state, float* run_score, float* cand_score, int* cand_tok,
+                                      long long* run_seq, long long* fin_seq, float* fin_score, int* fin_state,
+                                      long long* ids, int* pos_rows, int* anc, float* scores, float* raw_logits,
+                                      int n_slots, int* run_bidx, int* fin_bidx, void* stream) {
+  return beam_step(logits, ld, row_div, B, N, V, K, eos_ids, n_eos, prompt_len, max_length, length_penalty,
+                   early_stopping, G, Lmax, lens, state, run_score, cand_score, cand_tok, run_seq, fin_seq, fin_score,
+                   fin_state, ids, pos_rows, anc, scores, raw_logits, n_slots, run_bidx, fin_bidx, stream);
 }

@@ -119,6 +119,27 @@ struct SampleProc {
   int append;             // write the selected token to h[b, L + *rng_step]
 };
 
+// The output pass (g4r_sample_tokens_out_*): transformers' return_dict_in_generate scores.  Slot *rng_step of two fp32
+// buffers [n_slots, B, V] gets, for every id, the processed score the selection used (the history-dependent processors,
+// then, when sampling, / temperature and -inf below the top-k / top-p thresholds: HF's next_token_scores) and the
+// widened logit (HF's next_token_logits).  Either pointer may be null; a slot past n_slots is not written.
+struct SampleOut {
+  float* scores;
+  float* logits;
+  long long n_slots;
+};
+
+template <typename F>
+__device__ __forceinline__ void write_outputs(const SampleOut& o, const unsigned short* __restrict__ row, int V,
+                                              long long slot, F&& score) {
+  if (slot < 0 || slot >= o.n_slots) return;
+  const long long base = (slot * gridDim.x + blockIdx.x) * V;
+  for (int i = threadIdx.x; i < V; i += SAMPLE_THREADS) {
+    if (o.scores) o.scores[base + i] = score(i);
+    if (o.logits) o.logits[base + i] = bits_value(row[i]);
+  }
+}
+
 // Order key of an fp32 value: ascends with the value; -0 folded onto +0, every NaN onto the top key (torch.argmax).
 __device__ __forceinline__ unsigned f32_key(float y) {
   if (y != y) return 0xFFFFFFFFu;
@@ -170,9 +191,10 @@ __device__ __forceinline__ int list_owner(unsigned long long e) {
   return (int)(order_key(bits_rd(f32_of_key((unsigned)(e >> 32)))) >> 6);
 }
 
+template <bool OUT>
 __device__ void select_processed(const unsigned short* __restrict__ row, int V, float temperature, int top_k,
                                  float top_p, int greedy, unsigned long long seed, const long long* __restrict__ rng_step,
-                                 const SampleProc& pr, unsigned* smem, int& s_tok) {
+                                 const SampleProc& pr, const SampleOut& out, unsigned* smem, int& s_tok) {
   __shared__ unsigned long long s_best[32];
   __shared__ int s_int[32];
   __shared__ float s_flt[32];
@@ -244,6 +266,11 @@ __device__ void select_processed(const unsigned short* __restrict__ row, int V, 
       for (int w = 1; w < 32; w++) best = s_best[w] > best ? s_best[w] : best;
       s_tok = (int)(0xFFFFFFFFu - (unsigned)best);
     }
+    if constexpr (OUT)
+      write_outputs(out, row, V, step, [&](int i) {
+        float y;
+        return value(i, y) ? y : -INFINITY;
+      });
     return;
   }
 
@@ -451,14 +478,19 @@ __device__ void select_processed(const unsigned short* __restrict__ row, int V, 
     }
     seen += nh;
   }
+  if constexpr (OUT)
+    write_outputs(out, row, V, step, [&](int i) {
+      float y;
+      return value(i, y) && f32_key(y) >= thr ? __fdiv_rn(y, temperature) : -INFINITY;
+    });
 }
 
-template <bool PROC>
-__global__ void __launch_bounds__(SAMPLE_THREADS, 1)
-sample_tokens_kernel(const unsigned short* __restrict__ logits, long long ld, int V, float temperature, int top_k,
-                     float top_p, int greedy, unsigned long long seed, const long long* __restrict__ rng_step,
-                     int eos_id, int pad_id, int* __restrict__ finished, long long* __restrict__ out_ids,
-                     SampleProc proc) {
+template <bool PROC, bool OUT>
+__device__ __forceinline__ void sample_row(const unsigned short* __restrict__ logits, long long ld, int V,
+                                           float temperature, int top_k, float top_p, int greedy,
+                                           unsigned long long seed, const long long* __restrict__ rng_step, int eos_id,
+                                           int pad_id, int* __restrict__ finished, long long* __restrict__ out_ids,
+                                           const SampleProc& proc, const SampleOut& out) {
   extern __shared__ unsigned hist[];
   __shared__ unsigned long long s_best[32];
   __shared__ int s_int[32];
@@ -469,7 +501,7 @@ sample_tokens_kernel(const unsigned short* __restrict__ logits, long long ld, in
   const unsigned short* row = logits + (long long)b * ld;
 
   if constexpr (PROC) {
-    select_processed(row, V, temperature, top_k, top_p, greedy, seed, rng_step, proc, hist, s_tok);
+    select_processed<OUT>(row, V, temperature, top_k, top_p, greedy, seed, rng_step, proc, out, hist, s_tok);
   } else if (greedy) {
     // arg-max, first index among equals (torch.argmax)
     unsigned long long best = 0;
@@ -488,6 +520,7 @@ sample_tokens_kernel(const unsigned short* __restrict__ logits, long long ld, in
       for (int w = 1; w < 32; w++) best = s_best[w] > best ? s_best[w] : best;
       s_tok = (int)(0xFFFFFFFFu - (unsigned)best);
     }
+    if constexpr (OUT) write_outputs(out, row, V, *rng_step, [&](int i) { return bits_value(row[i]); });
   } else {
     // ---- histogram of the row's bit patterns
     for (int i = tid; i < SAMPLE_SMEM_WORDS; i += SAMPLE_THREADS) hist[i] = 0u;
@@ -632,6 +665,10 @@ sample_tokens_kernel(const unsigned short* __restrict__ logits, long long ld, in
       }
       seen += n;
     }
+    if constexpr (OUT)
+      write_outputs(out, row, V, step, [&](int i) {
+        return order_key(row[i]) >= thr ? __fdiv_rn(bits_value(row[i]), temperature) : -INFINITY;
+      });
   }
   __syncthreads();
   if (tid == 0) {
@@ -648,13 +685,36 @@ sample_tokens_kernel(const unsigned short* __restrict__ logits, long long ld, in
   }
 }
 
+template <bool PROC>
+__global__ void __launch_bounds__(SAMPLE_THREADS, 1)
+sample_tokens_kernel(const unsigned short* __restrict__ logits, long long ld, int V, float temperature, int top_k,
+                     float top_p, int greedy, unsigned long long seed, const long long* __restrict__ rng_step,
+                     int eos_id, int pad_id, int* __restrict__ finished, long long* __restrict__ out_ids,
+                     SampleProc proc) {
+  sample_row<PROC, false>(logits, ld, V, temperature, top_k, top_p, greedy, seed, rng_step, eos_id, pad_id, finished,
+                          out_ids, proc, SampleOut{});
+}
+
+// The same selection followed by the output pass; a separate kernel, so the selection-only kernels stay as they are.
+template <bool PROC>
+__global__ void __launch_bounds__(SAMPLE_THREADS, 1)
+sample_tokens_out_kernel(const unsigned short* __restrict__ logits, long long ld, int V, float temperature, int top_k,
+                         float top_p, int greedy, unsigned long long seed, const long long* __restrict__ rng_step,
+                         int eos_id, int pad_id, int* __restrict__ finished, long long* __restrict__ out_ids,
+                         SampleProc proc, SampleOut out) {
+  sample_row<PROC, true>(logits, ld, V, temperature, top_k, top_p, greedy, seed, rng_step, eos_id, pad_id, finished,
+                         out_ids, proc, out);
+}
+
 }  // namespace G4R_NS
 
 using namespace G4R_NS;
 
-extern "C" int g4r_sample_tokens_bf16(const void* logits, long long ld, int B, int V, float temperature, int top_k,
-                                      float top_p, int greedy, unsigned long long seed, const long long* rng_step,
-                                      int eos_id, int pad_id, int* finished, long long* out_ids, void* stream) {
+// The selection-only kernels (OUT false) or their output-pass instances (OUT true).
+template <bool OUT>
+static int launch_plain(const void* logits, long long ld, int B, int V, float temperature, int top_k, float top_p,
+                        int greedy, unsigned long long seed, const long long* rng_step, int eos_id, int pad_id,
+                        int* finished, long long* out_ids, SampleOut out, void* stream) {
   G4R_REQUIRE(logits && out_ids && B > 0 && V > 0 && ld >= V, "sample_tokens: bad arguments (B=%d V=%d ld=%lld)", B, V, ld);
   G4R_REQUIRE(greedy || (V < 65536 && rng_step && temperature > 0.f && top_p >= 0.f),
               "sample_tokens: sampling needs V < 65536 (16-bit bin counts), rng_step, temperature > 0 and top_p >= 0 "
@@ -662,23 +722,32 @@ extern "C" int g4r_sample_tokens_bf16(const void* logits, long long ld, int B, i
   cudaStream_t st = (cudaStream_t)stream;
   static bool set = false;
   if (!set) {
-    G4R_CUDA(cudaFuncSetAttribute(sample_tokens_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                  (int)SAMPLE_SMEM));
+    if constexpr (OUT)
+      G4R_CUDA(cudaFuncSetAttribute(sample_tokens_out_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                    (int)SAMPLE_SMEM));
+    else
+      G4R_CUDA(cudaFuncSetAttribute(sample_tokens_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                    (int)SAMPLE_SMEM));
     set = true;
   }
-  sample_tokens_kernel<false><<<B, SAMPLE_THREADS, greedy ? 0 : SAMPLE_SMEM, st>>>(
-      (const unsigned short*)logits, ld, V, temperature, top_k, top_p, greedy, seed, rng_step, eos_id, pad_id, finished,
-      out_ids, SampleProc{});
+  if constexpr (OUT)
+    sample_tokens_out_kernel<false><<<B, SAMPLE_THREADS, greedy ? 0 : SAMPLE_SMEM, st>>>(
+        (const unsigned short*)logits, ld, V, temperature, top_k, top_p, greedy, seed, rng_step, eos_id, pad_id,
+        finished, out_ids, SampleProc{}, out);
+  else
+    sample_tokens_kernel<false><<<B, SAMPLE_THREADS, greedy ? 0 : SAMPLE_SMEM, st>>>(
+        (const unsigned short*)logits, ld, V, temperature, top_k, top_p, greedy, seed, rng_step, eos_id, pad_id,
+        finished, out_ids, SampleProc{});
   G4R_LAUNCH_CHECK("sample_tokens");
   return G4R_OK;
 }
 
-extern "C" int g4r_sample_tokens_proc_bf16(const void* logits, long long ld, int B, int V, float temperature, int top_k,
-                                           float top_p, int greedy, unsigned long long seed, const long long* rng_step,
-                                           int eos_id, int pad_id, int* finished, long long* out_ids,
-                                           long long* history, long long ld_h, int L, float repetition_penalty,
-                                           int no_repeat_ngram_size, int min_length, int min_new_tokens,
-                                           const int* eos_ids, int n_eos, int append, void* stream) {
+template <bool OUT>
+static int launch_proc(const void* logits, long long ld, int B, int V, float temperature, int top_k, float top_p,
+                       int greedy, unsigned long long seed, const long long* rng_step, int eos_id, int pad_id,
+                       int* finished, long long* out_ids, long long* history, long long ld_h, int L,
+                       float repetition_penalty, int no_repeat_ngram_size, int min_length, int min_new_tokens,
+                       const int* eos_ids, int n_eos, int append, SampleOut out, void* stream) {
   G4R_REQUIRE(logits && out_ids && B > 0 && V > 0 && V < 65536 && ld >= V,
               "sample_tokens_proc: bad arguments (B=%d V=%d ld=%lld; V < 65536)", B, V, ld);
   G4R_REQUIRE(greedy || (temperature > 0.f && top_p >= 0.f),
@@ -700,14 +769,68 @@ extern "C" int g4r_sample_tokens_proc_bf16(const void* logits, long long ld, int
   static bool set = false;
   if (!set) {
     const size_t most = SAMPLE_SMEM + 2 * sizeof(unsigned) * 2048 + PROC_LIST_MAX * sizeof(unsigned long long);
-    G4R_CUDA(cudaFuncSetAttribute(sample_tokens_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)most));
+    if constexpr (OUT)
+      G4R_CUDA(cudaFuncSetAttribute(sample_tokens_out_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                    (int)most));
+    else
+      G4R_CUDA(cudaFuncSetAttribute(sample_tokens_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)most));
     set = true;
   }
   SampleProc pr{history, ld_h, L, repetition_penalty, no_repeat_ngram_size, min_length, min_new_tokens, eos_ids, n_eos,
                 append};
-  sample_tokens_kernel<true><<<B, SAMPLE_THREADS, smem, st>>>(
-      (const unsigned short*)logits, ld, V, temperature, top_k, top_p, greedy, seed, rng_step, eos_id, pad_id, finished,
-      out_ids, pr);
+  if constexpr (OUT)
+    sample_tokens_out_kernel<true><<<B, SAMPLE_THREADS, smem, st>>>(
+        (const unsigned short*)logits, ld, V, temperature, top_k, top_p, greedy, seed, rng_step, eos_id, pad_id,
+        finished, out_ids, pr, out);
+  else
+    sample_tokens_kernel<true><<<B, SAMPLE_THREADS, smem, st>>>(
+        (const unsigned short*)logits, ld, V, temperature, top_k, top_p, greedy, seed, rng_step, eos_id, pad_id,
+        finished, out_ids, pr);
   G4R_LAUNCH_CHECK("sample_tokens_proc");
   return G4R_OK;
+}
+
+extern "C" int g4r_sample_tokens_bf16(const void* logits, long long ld, int B, int V, float temperature, int top_k,
+                                      float top_p, int greedy, unsigned long long seed, const long long* rng_step,
+                                      int eos_id, int pad_id, int* finished, long long* out_ids, void* stream) {
+  return launch_plain<false>(logits, ld, B, V, temperature, top_k, top_p, greedy, seed, rng_step, eos_id, pad_id,
+                             finished, out_ids, SampleOut{}, stream);
+}
+
+extern "C" int g4r_sample_tokens_proc_bf16(const void* logits, long long ld, int B, int V, float temperature, int top_k,
+                                           float top_p, int greedy, unsigned long long seed, const long long* rng_step,
+                                           int eos_id, int pad_id, int* finished, long long* out_ids,
+                                           long long* history, long long ld_h, int L, float repetition_penalty,
+                                           int no_repeat_ngram_size, int min_length, int min_new_tokens,
+                                           const int* eos_ids, int n_eos, int append, void* stream) {
+  return launch_proc<false>(logits, ld, B, V, temperature, top_k, top_p, greedy, seed, rng_step, eos_id, pad_id,
+                            finished, out_ids, history, ld_h, L, repetition_penalty, no_repeat_ngram_size, min_length,
+                            min_new_tokens, eos_ids, n_eos, append, SampleOut{}, stream);
+}
+
+extern "C" int g4r_sample_tokens_out_bf16(const void* logits, long long ld, int B, int V, float temperature, int top_k,
+                                          float top_p, int greedy, unsigned long long seed, const long long* rng_step,
+                                          int eos_id, int pad_id, int* finished, long long* out_ids,
+                                          long long* history, long long ld_h, int L, float repetition_penalty,
+                                          int no_repeat_ngram_size, int min_length, int min_new_tokens,
+                                          const int* eos_ids, int n_eos, int append, float* scores, float* raw_logits,
+                                          long long n_slots, void* stream) {
+  G4R_REQUIRE(history || (repetition_penalty == 1.f && no_repeat_ngram_size == 0 && n_eos == 0),
+              "sample_tokens_out: the logits processors need the history (penalty=%g n=%d n_eos=%d)",
+              (double)repetition_penalty, no_repeat_ngram_size, n_eos);
+  const SampleOut out{scores, raw_logits, n_slots};
+  if (!scores && !raw_logits)   // nothing to write: exactly the selection-only launch
+    return history ? launch_proc<false>(logits, ld, B, V, temperature, top_k, top_p, greedy, seed, rng_step, eos_id,
+                                        pad_id, finished, out_ids, history, ld_h, L, repetition_penalty,
+                                        no_repeat_ngram_size, min_length, min_new_tokens, eos_ids, n_eos, append, out,
+                                        stream)
+                   : launch_plain<false>(logits, ld, B, V, temperature, top_k, top_p, greedy, seed, rng_step, eos_id,
+                                         pad_id, finished, out_ids, out, stream);
+  G4R_REQUIRE(rng_step && n_slots > 0, "sample_tokens_out: the output slot is *rng_step: rng_step and n_slots > 0 are "
+              "required (n_slots=%lld)", n_slots);
+  return history ? launch_proc<true>(logits, ld, B, V, temperature, top_k, top_p, greedy, seed, rng_step, eos_id, pad_id,
+                                     finished, out_ids, history, ld_h, L, repetition_penalty, no_repeat_ngram_size,
+                                     min_length, min_new_tokens, eos_ids, n_eos, append, out, stream)
+                 : launch_plain<true>(logits, ld, B, V, temperature, top_k, top_p, greedy, seed, rng_step, eos_id,
+                                      pad_id, finished, out_ids, out, stream);
 }

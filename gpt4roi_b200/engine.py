@@ -933,10 +933,13 @@ class Sampler:
     kernels.stop_step on the tokens just selected, which keeps the rows' matcher states in `stop_state` and sets
     `finished` for a row whose token ends a stop string.
     processors (a LogitsProcessors): the selection runs on the scores its processors leave, reading each row's history
-    at length L + rng_step and appending the selected token to it (kernels.sample_tokens_processed)."""
+    at length L + rng_step and appending the selected token to it (kernels.sample_tokens_processed).
+    scores / logits (fp32 [n_slots, B, V], either may be None): every call also writes transformers'
+    next_token_scores / next_token_logits of its rows into slot rng_step (kernels.sample_tokens_out); without them it
+    launches exactly what it launches otherwise."""
 
     def __init__(self, B, device, greedy=True, temperature=1.0, top_k=None, top_p=None, seed=0, eos_id=None,
-                 pad_id=None, stops=None, stop_state=None, processors=None):
+                 pad_id=None, stops=None, stop_state=None, processors=None, scores=None, logits=None):
         self.greedy = bool(greedy)
         self.temperature = float(temperature)
         self.top_k = 0 if top_k is None else int(top_k)
@@ -950,6 +953,7 @@ class Sampler:
         if stops is not None:
             self.stop_state = torch.zeros_like(self.finished) if stop_state is None else stop_state.to(device, torch.int32)
         self.processors = processors
+        self.out_scores, self.out_logits = scores, logits
 
     def __call__(self, logits, out, update=True):
         """Select from logits [B, 1, V] into out (int64 [B, 1]).  update=False leaves `finished`, `stop_state` and the
@@ -958,7 +962,15 @@ class Sampler:
         if not logits.is_cuda:
             return self._host(logits, out, update)
         pr = self.processors
-        if pr is None:
+        if self.out_scores is not None or self.out_logits is not None:
+            proc = {} if pr is None else dict(
+                history=pr.history, L=pr.L, repetition_penalty=pr.repetition_penalty,
+                no_repeat_ngram_size=pr.no_repeat_ngram_size, min_length=pr.min_length,
+                min_new_tokens=pr.min_new_tokens, eos_ids=pr.eos_ids, append=update)
+            kernels.sample_tokens_out(logits, out, self.greedy, self.temperature, self.top_k, self.top_p, self.seed,
+                                      self.rng_step, self.eos_id, self.pad_id, self.finished if update else None,
+                                      scores=self.out_scores, raw_logits=self.out_logits, **proc)
+        elif pr is None:
             kernels.sample_tokens(logits, out, self.greedy, self.temperature, self.top_k, self.top_p, self.seed,
                                   self.rng_step, self.eos_id, self.pad_id, self.finished if update else None)
         else:
@@ -974,14 +986,18 @@ class Sampler:
 
     def _host(self, logits, out, update):
         """Host tensors come only from CPU stand-ins of the engine (the loop's host-side tests): the arg-max (of the
-        processed fp32 scores with processors), the eos -> pad rule and the history append, restated.  Sampling exists
-        on the device only."""
+        processed fp32 scores with processors), the output slots, the eos -> pad rule and the history append, restated.
+        Sampling exists on the device only."""
         if not self.greedy:
             raise RuntimeError('token sampling runs on the CUDA device only (csrc/sample.cu): logits are on %s'
                                % logits.device)
         scores = logits.reshape(logits.shape[0], -1)
         if self.processors is not None:
             scores = self.processors.apply(scores.float(), int(self.rng_step))
+        slot = int(self.rng_step)
+        for buf, val in ((self.out_scores, scores), (self.out_logits, logits)):
+            if buf is not None and slot < buf.shape[0]:
+                buf[slot].copy_(val.reshape(buf.shape[1:]))
         tok = scores.argmax(-1)
         if update and self.eos_id >= 0:
             tok = torch.where(self.finished.bool(), torch.full_like(tok, self.pad_id), tok)
@@ -1012,7 +1028,8 @@ def _generate(self, input_ids, images, bboxes, max_new_tokens=32, do_sample=Fals
               stopping_criteria=None, eos_token_id=None, generator=None, use_graph=True, attention_mask=None,
               pad_token_id=None, cache=None, top_k=None, top_p=None, num_beams=1, length_penalty=1.0,
               early_stopping=False, num_return_sequences=1, stop_strings=None, repetition_penalty=1.0,
-              no_repeat_ngram_size=0, min_length=0, min_new_tokens=0, length_eos_ids=None):
+              no_repeat_ngram_size=0, min_length=0, min_new_tokens=0, length_eos_ids=None, output_scores=False,
+              output_logits=False, return_dict_in_generate=False):
     """Prefill + greedy / sampled decode (gpt4roi/app.py:286-300 calls
     model.generate(input_ids, images=..., do_sample=True, temperature=0.2, max_new_tokens=1024,
     stopping_criteria=[...]) with the boxes bound to forward).  Returns ids [B, L + new]: the prompt as given,
@@ -1054,7 +1071,16 @@ def _generate(self, input_ids, images, bboxes, max_new_tokens=32, do_sample=Fals
     finished rows included).  length_eos_ids: the ids min_length / min_new_tokens suppress (HF's resolved eos list;
     None: [eos_token_id] when one is given); they do not change when the loop stops or pads.  With all four neutral the
     loop launches the kernels it launches without them.  Sampling with a repetition penalty holds at most
-    kernels.PROC_LIST_MAX history ids per row; beyond that, and with beam search, they raise NotImplementedError."""
+    kernels.PROC_LIST_MAX history ids per row; beyond that, and with beam search, they raise NotImplementedError.
+    output_scores / output_logits / return_dict_in_generate (transformers' generate outputs): with any of them the call
+    returns a dict -- sequences (the ids above), scores and logits (None unless asked for: one fp32 [R, V] tensor per
+    new token, R = B * num_return_sequences; scores are HF's next_token_scores, the fp32 logits through the processors
+    and, when sampling, the temperature / top-k / top-p warpers, -inf where HF masks; logits the widened logits; entry 0
+    comes from the prefill).  The selection kernel writes them inside the (graphed) step into slot s of fp32 buffers
+    [max_new_tokens, R, V], allocated up front: 4 * V bytes (128 KB at V = 32 000) per row, token and output, where HF
+    grows its tuples as it goes -- the same peak at full length.  Beam search adds sequences_scores (the returned
+    beams' final scores) and beam_indices (int32 [B * num_return_sequences, n], b * num_beams + beam, -1 past a beam's
+    end); its scores are each beam row's log_softmax before the running score is added, as HF stores them."""
     if length_eos_ids is None:
         length_eos_ids = [] if eos_token_id is None else (
             list(eos_token_id) if isinstance(eos_token_id, (list, tuple)) else [eos_token_id])
@@ -1074,7 +1100,8 @@ def _generate(self, input_ids, images, bboxes, max_new_tokens=32, do_sample=Fals
             raise NotImplementedError('beam search on a conversation cache (cache=) runs on the HF loop only: pass '
                                       'use_hf_loop=True')
         return _generate_beams(self, input_ids, images, bboxes, max_new_tokens, num_beams, eos_token_id, pad_token_id,
-                               attention_mask, length_penalty, early_stopping, num_return_sequences, use_graph)
+                               attention_mask, length_penalty, early_stopping, num_return_sequences, use_graph,
+                               output_scores, output_logits, return_dict_in_generate)
     B, L = input_ids.shape
     N = int(num_return_sequences)
     greedy = not (do_sample and temperature > 0)
@@ -1122,9 +1149,11 @@ def _generate(self, input_ids, images, bboxes, max_new_tokens=32, do_sample=Fals
     out[:, :L] = ids if N == 1 else ids.repeat_interleave(N, 0)
     procs = None if neutral else LogitsProcessors(out, L, repetition_penalty, no_repeat_ngram_size, min_length,
                                                   min_new_tokens, length_eos_ids)   # `out` is the rows' history
+    slots = [torch.empty((max(max_new_tokens, 1), R, logits.shape[-1]), dtype=torch.float32, device=self.dev)
+             if want else None for want in (output_scores, output_logits)]
     sampler = Sampler(R, self.dev, greedy, temperature, top_k, top_p, seed=0 if greedy else sampling_seed(generator),
                       eos_id=eos_token_id, pad_id=pad_token_id, stops=stop_strings, stop_state=stop_state,
-                      processors=procs)
+                      processors=procs, scores=slots[0], logits=slots[1])
     stepper = None
     if use_graph and max_new_tokens > 4 and self.cfg.head_dim == 128:
         stepper = GraphedDecode(self, cache, sampler=sampler)   # each replay also selects the next token into its ids
@@ -1152,7 +1181,10 @@ def _generate(self, input_ids, images, bboxes, max_new_tokens=32, do_sample=Fals
     out = out[:, :L + n]
     if pos0 is not None and n > 1:   # outside the decode step, so its (graphed) launch sequence is unchanged
         cache.record_ids(out[:, L:L + n - 1], pos0)
-    return out
+    if not (output_scores or output_logits or return_dict_in_generate):
+        return out
+    scores, raw = (None if t is None else tuple(t[:n].unbind(0)) for t in slots)
+    return dict(sequences=out, scores=scores, logits=raw)
 
 
 def _capture(dev, warm, body):
@@ -1300,6 +1332,18 @@ class BeamCache(_SharedPromptCache):
         self.fin_seq = torch.full((2, B, N, self.G), self.fill, dtype=torch.int64, device=dev)
         self.fin_score = torch.full((B, N), -1e9, dtype=torch.float32, device=dev)
         self.fin_state = torch.zeros((B, N, 2), dtype=torch.int32, device=dev)
+        self.out_scores = self.out_logits = self.bidx = None
+
+    def keep_outputs(self, V, scores=False, logits=False, indices=False):
+        """Have every beam step also write transformers' generate outputs (kernels.beam_step): scores / logits into
+        slot g (the step's count of generated tokens) of fp32 [max_new_tokens, B*N, V] buffers, and the beam indices
+        (int32 [running / finished, 2, B, N, G], -1 where nothing was generated) beside the sequences."""
+        dev = self.anc.device
+        shape = (self.G, self.B, V)
+        self.out_scores = torch.empty(shape, dtype=torch.float32, device=dev) if scores else None
+        self.out_logits = torch.empty(shape, dtype=torch.float32, device=dev) if logits else None
+        self.bidx = torch.full((2, 2, self.n_samples, self.N, self.G), -1, dtype=torch.int32, device=dev) \
+            if indices else None
 
     def start(self, lens):
         """After the prefill: lens (device int32 [B]) each sample's prompt length; every beam row's prompt positions
@@ -1327,6 +1371,20 @@ class BeamCache(_SharedPromptCache):
         n = int(self.fin_state[:, :num_return_sequences, 1].max())
         prompt = prompt_ids.to(seqs.device).repeat_interleave(num_return_sequences, 0)
         return torch.cat([prompt, seqs[:, :n]], 1)
+
+    def outputs(self, num_return_sequences, prompt_ids):
+        """result() with the outputs keep_outputs asked for, as a dict: sequences, scores / logits (a tuple of one
+        [B*N, V] tensor per step, or None), sequences_scores (fp32 [B * num_return_sequences]: the returned beams' final
+        scores) and beam_indices (int32 [B * num_return_sequences, n], or None), HF's _beam_search outputs."""
+        seqs = self.result(num_return_sequences, prompt_ids)
+        g = int(self.state[0])
+        n = seqs.shape[1] - prompt_ids.shape[1]
+        nrs = num_return_sequences
+        scores, raw = (None if t is None else tuple(t[:g].unbind(0)) for t in (self.out_scores, self.out_logits))
+        bidx = None if self.bidx is None else \
+            self.bidx[1, g & 1, :, :nrs].reshape(self.n_samples * nrs, self.G)[:, :n]
+        return dict(sequences=seqs, scores=scores, logits=raw, beam_indices=bidx,
+                    sequences_scores=self.fin_score[:, :nrs].reshape(-1).clone())
 
 
 class GraphedBeamDecode:
@@ -1363,7 +1421,8 @@ class GraphedBeamDecode:
 
 @torch.no_grad()
 def _generate_beams(self, input_ids, images, bboxes, max_new_tokens, num_beams, eos_token_id, pad_token_id,
-                    attention_mask, length_penalty, early_stopping, num_return_sequences, use_graph):
+                    attention_mask, length_penalty, early_stopping, num_return_sequences, use_graph,
+                    output_scores=False, output_logits=False, return_dict_in_generate=False):
     B, L = input_ids.shape
     N = int(num_beams)
     if not 1 <= num_return_sequences <= N:
@@ -1380,6 +1439,9 @@ def _generate_beams(self, input_ids, images, bboxes, max_new_tokens, num_beams, 
                                  self.plan_boxes(bboxes), validate=True, last_only=True, seqlens=_seqlens(lens, L),
                                  cache=cache.prompt)
     cache.start(lens)
+    want = output_scores or output_logits or return_dict_in_generate
+    if want:
+        cache.keep_outputs(logits.shape[-1], output_scores, output_logits, indices=True)
     cache.step(logits, first=True)
     stepper = None
     if use_graph and max_new_tokens > 4 and self.cfg.head_dim == 128:
@@ -1391,6 +1453,8 @@ def _generate_beams(self, input_ids, images, bboxes, max_new_tokens, num_beams, 
             stepper.step()
         else:
             cache.step(self.decode_step(cache.ids, cache))
+    if want:
+        return cache.outputs(num_return_sequences, ids)
     return cache.result(num_return_sequences, ids)
 
 

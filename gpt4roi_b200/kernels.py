@@ -279,6 +279,70 @@ def sample_tokens_processed(logits, out, greedy, temperature=1.0, top_k=0, top_p
     return out
 
 
+def _slot_buffer(name, t, rows, V):
+    """An output slot buffer: None, or a contiguous device fp32 [n_slots, rows, V] tensor; returns n_slots (0: None)."""
+    if t is None:
+        return 0
+    if t.dtype != torch.float32 or t.dim() != 3 or tuple(t.shape[1:]) != (rows, V) or not t.is_contiguous() \
+            or t.shape[0] < 1:
+        raise RuntimeError('%s must be a contiguous fp32 [n_slots, %d, %d] tensor, got %s %s'
+                           % (name, rows, V, t.dtype, tuple(t.shape)))
+    return t.shape[0]
+
+
+def sample_tokens_out(logits, out, greedy, temperature=1.0, top_k=0, top_p=1.0, seed=0, rng_step=None, eos_id=-1,
+                      pad_id=-1, finished=None, history=None, L=0, repetition_penalty=1.0, no_repeat_ngram_size=0,
+                      min_length=0, min_new_tokens=0, eos_ids=None, append=True, scores=None, raw_logits=None):
+    """sample_tokens (history None) or sample_tokens_processed, writing transformers' generate() outputs into slot
+    *rng_step of scores / raw_logits (contiguous device fp32 [n_slots, B, V], either may be None; include/gpt4roi_b200.h:
+    g4r_sample_tokens_out_bf16): scores gets HF's next_token_scores (the processors, then when sampling / temperature
+    and -inf below the top-k / top-p thresholds), raw_logits the widened logits.  With both None it launches what
+    sample_tokens / sample_tokens_processed launch."""
+    rows, act = _logit_rows('sample_tokens_out', logits)
+    B, V = rows.shape
+    if scores is None and raw_logits is None:
+        if history is None:
+            return sample_tokens(logits, out, greedy, temperature, top_k, top_p, seed, rng_step, eos_id, pad_id, finished)
+        return sample_tokens_processed(logits, out, greedy, temperature, top_k, top_p, seed, rng_step, eos_id, pad_id,
+                                       finished, history, L, repetition_penalty, no_repeat_ngram_size, min_length,
+                                       min_new_tokens, eos_ids, append)
+    n_slots = max(_slot_buffer('sample_tokens_out: scores', scores, B, V),
+                  _slot_buffer('sample_tokens_out: raw_logits', raw_logits, B, V))
+    if scores is not None and raw_logits is not None and scores.shape[0] != raw_logits.shape[0]:
+        raise RuntimeError('sample_tokens_out: scores and raw_logits must hold the same number of slots')
+    if out.dtype != torch.int64 or out.numel() != B or not out.is_contiguous():
+        raise RuntimeError('sample_tokens_out: out must be a contiguous int64 tensor of %d elements' % B)
+    if rng_step is None or rng_step.dtype != torch.int64 or rng_step.numel() != 1:
+        raise RuntimeError('sample_tokens_out: rng_step (the output slot) must be a device int64 [1] counter')
+    if finished is not None and (finished.dtype != torch.int32 or finished.numel() != B or not finished.is_contiguous()):
+        raise RuntimeError('sample_tokens_out: finished must be a contiguous device int32 [%d] vector' % B)
+    ld_h = 0
+    if history is not None:
+        if history.dtype != torch.int64 or history.dim() != 2 or history.shape[0] != B or not history.is_contiguous():
+            raise RuntimeError('sample_tokens_out: history must be a contiguous int64 [%d, ld_h] tensor' % B)
+        ld_h = history.shape[1]
+        if not 0 <= int(L) <= ld_h:
+            raise RuntimeError('sample_tokens_out: the prompt length L=%d must lie in [0, %d]' % (L, ld_h))
+        if not greedy and repetition_penalty != 1.0 and ld_h > PROC_LIST_MAX:
+            raise RuntimeError('sample_tokens_out: sampling with a repetition penalty holds at most %d history ids per '
+                               'row (ld_h=%d)' % (PROC_LIST_MAX, ld_h))
+    if not repetition_penalty > 0 or int(no_repeat_ngram_size) < 0 or int(min_length) < 0 or int(min_new_tokens) < 0:
+        raise RuntimeError('sample_tokens_out: repetition_penalty must be > 0 and the lengths >= 0 (got %r, %r, %r, %r)'
+                           % (repetition_penalty, no_repeat_ngram_size, min_length, min_new_tokens))
+    if eos_ids is not None and (eos_ids.dtype != torch.int32 or eos_ids.dim() != 1 or not eos_ids.is_contiguous()):
+        raise RuntimeError('sample_tokens_out: eos_ids must be a contiguous device int32 vector')
+    n_eos = 0 if eos_ids is None else eos_ids.numel()
+    _L.require_cuda_same_device([('logits', rows), ('out', out), ('rng_step', rng_step), ('finished', finished),
+                                 ('history', history), ('eos_ids', eos_ids), ('scores', scores),
+                                 ('raw_logits', raw_logits)])
+    _call('g4r_sample_tokens_out_bf16', rows.device, _L.ptr(rows), rows.stride(0), B, V, float(temperature),
+          int(top_k), float(top_p), int(bool(greedy)), int(seed) & 0xFFFFFFFFFFFFFFFF, _L.ptr(rng_step), int(eos_id),
+          int(pad_id), _L.ptr(finished), _L.ptr(out), _L.ptr(history), ld_h, int(L), float(repetition_penalty),
+          int(no_repeat_ngram_size), int(min_length), int(min_new_tokens), _L.ptr(eos_ids) if n_eos else None, n_eos,
+          int(bool(append)), _L.ptr(scores), _L.ptr(raw_logits), n_slots, act=act)
+    return out
+
+
 def stop_step(ids, table, state, finished):
     """Stop strings, one step: every row b with finished[b] == 0 advances its matcher state by the token ids[b] through
     table (int16 [V_tok + 1, S], engine.StopStrings) and sets finished[b] when an occurrence of a stop string ended in
@@ -368,13 +432,32 @@ def decode_attention_group(qkv, kcache, vcache, B, N, n_heads, head_dim, prompt_
 
 def beam_step(logits, row_div, st):
     """One beam-search step (csrc/beam.cu) on 16-bit logits [rows, V] (or [rows, 1, V]; unit column stride) with the
-    device state of st (engine.BeamCache): B*N rows, or B with row_div = N (the first step, from the prefill)."""
+    device state of st (engine.BeamCache): B*N rows, or B with row_div = N (the first step, from the prefill).  When st
+    holds output buffers (out_scores / out_logits: fp32 [n_slots, B*N, V]; bidx: int32 [2 (running, finished), 2, B, N,
+    G] beam-index columns), the step also writes them (g4r_beam_step_out_bf16)."""
     rows, act = _logit_rows('beam_step', logits)
     V = rows.shape[1]
     B, N = st.n_samples, st.N
     if rows.shape[0] * row_div != B * N:
         raise RuntimeError('beam_step: logits must be [%d, V] rows' % (B * N // row_div))
     _L.require_cuda_same_device([('logits', rows), ('state', st.state), ('anc', st.anc)])
+    scores, raw, bidx = st.out_scores, st.out_logits, st.bidx
+    if scores is not None or raw is not None or bidx is not None:
+        n_slots = max(_slot_buffer('beam_step: scores', scores, B * N, V),
+                      _slot_buffer('beam_step: raw_logits', raw, B * N, V))
+        if scores is not None and raw is not None and scores.shape[0] != raw.shape[0]:
+            raise RuntimeError('beam_step: scores and raw_logits must hold the same number of slots')
+        shape = (2, 2, B, N, st.G)
+        if bidx is not None and (bidx.dtype != torch.int32 or tuple(bidx.shape) != shape or not bidx.is_contiguous()):
+            raise RuntimeError('beam_step: the beam indices must be a contiguous int32 %s tensor' % (shape,))
+        _L.require_cuda_same_device([('logits', rows), ('scores', scores), ('raw_logits', raw), ('beam_indices', bidx)])
+        _call('g4r_beam_step_out_bf16', rows.device, _L.ptr(rows), rows.stride(0), int(row_div), B, N, V, st.K,
+              _L.ptr(st.eos), st.n_eos, st.prompt_len, st.max_length, float(st.length_penalty), st.early, st.G, st.Lmax,
+              _L.ptr(st.prompt_lens), _L.ptr(st.state), _L.ptr(st.run_score), _L.ptr(st.cand_score),
+              _L.ptr(st.cand_tok), _L.ptr(st.run_seq), _L.ptr(st.fin_seq), _L.ptr(st.fin_score), _L.ptr(st.fin_state),
+              _L.ptr(st.ids), _L.ptr(st.pos_rows), _L.ptr(st.anc), _L.ptr(scores), _L.ptr(raw), n_slots,
+              None if bidx is None else _L.ptr(bidx[0]), None if bidx is None else _L.ptr(bidx[1]), act=act)
+        return
     _call('g4r_beam_step_bf16', rows.device, _L.ptr(rows), rows.stride(0), int(row_div), B, N, V, st.K,
           _L.ptr(st.eos), st.n_eos, st.prompt_len, st.max_length, float(st.length_penalty), st.early, st.G, st.Lmax,
           _L.ptr(st.prompt_lens), _L.ptr(st.state), _L.ptr(st.run_score), _L.ptr(st.cand_score), _L.ptr(st.cand_tok),

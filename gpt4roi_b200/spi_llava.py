@@ -592,9 +592,10 @@ def resolve_beam_search(model, input_len, max_new_tokens, do_sample=None, **kwar
     """The engine loop's beam search for a generate call, resolved as transformers resolves it (explicit kwargs, then
     `generation_config=`, then model.generation_config, then HF's defaults: GenerationMixin._prepare_generation_config).
     Returns None when the resolved num_beams is 1, else a dict of num_beams, length_penalty, early_stopping,
-    num_return_sequences, eos_token_id (a list), pad_token_id and max_length.  Beam search with do_sample, with any
-    logits processor, or with output_scores / return_dict_in_generate raises NotImplementedError: the HF loop
-    (use_hf_loop=True) runs those."""
+    num_return_sequences, eos_token_id (a list), pad_token_id and max_length.  Beam search with do_sample or with any
+    logits processor raises NotImplementedError: the HF loop (use_hf_loop=True) runs those.  This resolves the search
+    alone: a call whose resolved config asks for outputs (output_scores / output_logits / return_dict_in_generate)
+    raises NotImplementedError too; generate() resolves those with resolve_outputs and calls this with them off."""
     given = {k: v for k, v in dict(kwargs, do_sample=do_sample, max_new_tokens=max_new_tokens).items() if v is not None}
     gc = _generation_config(model, given)
     N = gc.num_beams or 1
@@ -604,7 +605,9 @@ def resolve_beam_search(model, input_len, max_new_tokens, do_sample=None, **kwar
     if gc.do_sample:
         raise NotImplementedError('beam search with do_sample (beam sampling) ' + hf)
     if gc.output_scores or gc.output_logits or gc.return_dict_in_generate:
-        raise NotImplementedError('beam search with output_scores / return_dict_in_generate ' + hf)
+        raise NotImplementedError('resolve_beam_search resolves the search alone: resolve output_scores / output_logits '
+                                  '/ return_dict_in_generate with resolve_outputs and pass them off here, as generate() '
+                                  'does (or generate with use_hf_loop=True)')
     procs = model._get_logits_processor(gc, input_ids_seq_length=input_len, device='cpu', model_kwargs={},
                                         logits_processor=kwargs.get('logits_processor'))
     if len(procs):
@@ -620,6 +623,34 @@ def resolve_beam_search(model, input_len, max_new_tokens, do_sample=None, **kwar
                 num_return_sequences=int(nrs), eos_token_id=None if eos is None else eos.flatten().tolist(),
                 pad_token_id=None if pad is None else int(pad),
                 max_length=int(input_len + gc.max_new_tokens if gc.max_new_tokens is not None else gc.max_length))
+
+
+def resolve_outputs(model, do_sample=None, temperature=None, **kwargs):
+    """What a generate call returns besides the ids, resolved as transformers resolves it (the explicit kwargs, then
+    `generation_config=`, then model.generation_config): a dict of return_dict_in_generate, output_scores and
+    output_logits (the last two only count with the first, as in HF).  output_attentions / output_hidden_states raise
+    NotImplementedError: the fused engine materialises neither, on either loop."""
+    given = {k: v for k, v in dict(kwargs, do_sample=do_sample, temperature=temperature).items() if v is not None}
+    gc = _generation_config(model, given)
+    if gc.output_attentions or gc.output_hidden_states:
+        raise NotImplementedError('output_attentions / output_hidden_states: attention maps and per-layer hidden states '
+                                  'are not materialised by the fused engine')
+    rd = bool(gc.return_dict_in_generate)
+    return dict(return_dict_in_generate=rd, output_scores=rd and bool(gc.output_scores),
+                output_logits=rd and bool(gc.output_logits))
+
+
+def _generate_output(res, outs, past_key_values):
+    """The engine loop's result as transformers' own generate output class (GenerateDecoderOnlyOutput, or
+    GenerateBeamDecoderOnlyOutput for beam search).  past_key_values: the caller's cache, else None (the engine's own
+    cache is not a transformers Cache)."""
+    from transformers.generation.utils import GenerateBeamDecoderOnlyOutput, GenerateDecoderOnlyOutput
+    if 'beam_indices' in res:
+        return GenerateBeamDecoderOnlyOutput(
+            sequences=res['sequences'], sequences_scores=res['sequences_scores'] if outs['output_scores'] else None,
+            scores=res['scores'], logits=res['logits'], beam_indices=res['beam_indices'], past_key_values=past_key_values)
+    return GenerateDecoderOnlyOutput(sequences=res['sequences'], scores=res['scores'], logits=res['logits'],
+                                     past_key_values=past_key_values)
 
 
 _STOP_STRINGS = collections.OrderedDict()   # (vocabulary, stop strings) -> StopStrings; the last 8 used
@@ -857,12 +888,17 @@ class SPILlavaMPTForCausalLM(LlamaForCausalLM, _EngineHost):
         stopping_criteria (KeywordsStoppingCriteria) keep running as callbacks after every token.
         num_beams > 1 (do_sample false) runs beam search on the engine loop (resolve_beam_search: length_penalty,
         early_stopping, num_return_sequences, eos / max length as HF resolves them): the prompt is prefilled once per
-        sample and the beams share its KV cache; beam sampling, logits processors, stopping_criteria, stop_strings, output_scores /
-        return_dict_in_generate and past_key_values raise NotImplementedError there, and run with use_hf_loop=True.
+        sample and the beams share its KV cache; beam sampling, logits processors, stopping_criteria, stop_strings and
+        past_key_values raise NotImplementedError there, and run with use_hf_loop=True.
         do_sample with num_return_sequences = N > 1 (resolve_num_return_sequences) returns N independent samples per
         prompt, [B * N, L + new] with row b*N + i sample i of prompt b, as HF does; the engine loop prefills each prompt
         once and its N rows share the prompt's KV cache.  With past_key_values it raises NotImplementedError (run it
-        with use_hf_loop=True)."""
+        with use_hf_loop=True).
+        return_dict_in_generate with output_scores / output_logits (resolve_outputs) returns, on the engine loop too,
+        transformers' GenerateDecoderOnlyOutput (GenerateBeamDecoderOnlyOutput with beam search: sequences_scores,
+        beam_indices) with HF's scores / logits, written by the selection and beam kernels inside the graphed step;
+        model.compute_transition_scores takes them.  Its past_key_values is the caller's cache when one was passed,
+        else None.  output_attentions / output_hidden_states raise NotImplementedError on both loops."""
         if bboxes is None:
             bboxes = getattr(getattr(self, 'forward', None), 'keywords', {}).get('bboxes')
         if use_hf_loop:
@@ -879,10 +915,12 @@ class SPILlavaMPTForCausalLM(LlamaForCausalLM, _EngineHost):
                                     do_sample=bool(do_sample), use_cache=True, **kw)
         gen = {k: v for k, v in kwargs.items() if k not in ('attention_mask', 'pad_token_id', 'past_key_values',
                                                              'generator', 'tokenizer')}
+        outs = resolve_outputs(self, do_sample, temperature, **gen)
         stops = resolve_stop_strings(self, kwargs.get('tokenizer'), kwargs.get('stop_strings'),
                                      kwargs.get('generation_config'))
+        no_outs = dict(return_dict_in_generate=False, output_scores=False, output_logits=False)   # resolved above
         beam = resolve_beam_search(self, input_ids.shape[1], max_new_tokens, do_sample, eos_token_id=eos_token_id,
-                                   pad_token_id=kwargs.get('pad_token_id'), **gen)
+                                   pad_token_id=kwargs.get('pad_token_id'), **dict(gen, **no_outs))
         if beam is not None:
             if stopping_criteria is not None:
                 raise NotImplementedError('beam search with stopping_criteria runs on the HF loop only: pass '
@@ -894,11 +932,12 @@ class SPILlavaMPTForCausalLM(LlamaForCausalLM, _EngineHost):
                 raise NotImplementedError('beam search on a conversation cache (past_key_values) runs on the HF loop '
                                           'only: pass use_hf_loop=True')
             eng = self._get_engine(input_ids.device)
-            return eng.generate(input_ids, images, bboxes, max_new_tokens=beam['max_length'] - input_ids.shape[1],
-                                num_beams=beam['num_beams'], length_penalty=beam['length_penalty'],
-                                early_stopping=beam['early_stopping'], num_return_sequences=beam['num_return_sequences'],
-                                eos_token_id=beam['eos_token_id'], pad_token_id=beam['pad_token_id'],
-                                attention_mask=kwargs.get('attention_mask'))
+            res = eng.generate(input_ids, images, bboxes, max_new_tokens=beam['max_length'] - input_ids.shape[1],
+                               num_beams=beam['num_beams'], length_penalty=beam['length_penalty'],
+                               early_stopping=beam['early_stopping'], num_return_sequences=beam['num_return_sequences'],
+                               eos_token_id=beam['eos_token_id'], pad_token_id=beam['pad_token_id'],
+                               attention_mask=kwargs.get('attention_mask'), **outs)
+            return _generate_output(res, outs, None) if outs['return_dict_in_generate'] else res
         nrs = resolve_num_return_sequences(self, do_sample, temperature, **gen)
         do_sample, temperature, top_k, top_p, procs = resolve_processors(self, input_ids.shape[1], do_sample,
                                                                          temperature, eos_token_id=eos_token_id, **gen)
@@ -915,14 +954,15 @@ class SPILlavaMPTForCausalLM(LlamaForCausalLM, _EngineHost):
                 pkv._g4r_cache = cache      # ride on HF's Cache object, as the HF loop's prefill does
             cache.stepper = None
             kv = cache.kv
-        return eng.generate(input_ids, images, bboxes, max_new_tokens=max_new_tokens, do_sample=do_sample,
-                            temperature=temperature, top_k=top_k, top_p=top_p, stopping_criteria=stopping_criteria,
-                            eos_token_id=eos_token_id, attention_mask=kwargs.get('attention_mask'),
-                            pad_token_id=kwargs.get('pad_token_id'), cache=kv, generator=kwargs.get('generator'),
-                            stop_strings=None if stops is None else stop_strings_from_tokenizer(kwargs['tokenizer'], stops),
-                            num_return_sequences=nrs, repetition_penalty=procs['repetition_penalty'],
-                            no_repeat_ngram_size=procs['no_repeat_ngram_size'], min_length=procs['min_length'],
-                            min_new_tokens=procs['min_new_tokens'], length_eos_ids=procs['eos_ids'])
+        res = eng.generate(input_ids, images, bboxes, max_new_tokens=max_new_tokens, do_sample=do_sample,
+                           temperature=temperature, top_k=top_k, top_p=top_p, stopping_criteria=stopping_criteria,
+                           eos_token_id=eos_token_id, attention_mask=kwargs.get('attention_mask'),
+                           pad_token_id=kwargs.get('pad_token_id'), cache=kv, generator=kwargs.get('generator'),
+                           stop_strings=None if stops is None else stop_strings_from_tokenizer(kwargs['tokenizer'], stops),
+                           num_return_sequences=nrs, repetition_penalty=procs['repetition_penalty'],
+                           no_repeat_ngram_size=procs['no_repeat_ngram_size'], min_length=procs['min_length'],
+                           min_new_tokens=procs['min_new_tokens'], length_eos_ids=procs['eos_ids'], **outs)
+        return _generate_output(res, outs, pkv) if outs['return_dict_in_generate'] else res
 
     def initialize_vision_tokenizer(self, mm_use_im_start_end, tokenizer, device, tune_mm_mlp_adapter=False,
                                     pretrain_mm_mlp_adapter=None):

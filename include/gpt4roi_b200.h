@@ -321,6 +321,20 @@ int g4r_beam_step_bf16(const void* logits, long long ld, int row_div, int B, int
                        long long* run_seq, long long* fin_seq, float* fin_score, int* fin_state, long long* ids,
                        int* pos_rows, int* anc, void* stream);
 
+/* g4r_beam_step_bf16 (same arguments, same step) with transformers' generate() outputs for return_dict_in_generate:
+ *   scores / raw_logits (fp32 [n_slots, B*N, V], contiguous, either may be NULL): slot g = state[4b] (the step's
+ *     generated-token count) of beam row r gets the row's log_softmax, (x - max) - log sum exp(x - max), before the
+ *     running score is added (HF's scores entry), and the widened logits; at the first step (row_div = N) each
+ *     sample's single row is written for all its N beams;
+ *   run_bidx / fin_bidx (int32 [2, B, N, G], both or neither; initialised to -1): HF's beam_indices beside run_seq /
+ *     fin_seq, double-buffered and gathered as they are; column g of a new beam holds b * N + its parent beam. */
+int g4r_beam_step_out_bf16(const void* logits, long long ld, int row_div, int B, int N, int V, int K,
+                           const int* eos_ids, int n_eos, int prompt_len, int max_length, double length_penalty,
+                           int early_stopping, int G, int Lmax, const int* lens, int* state, float* run_score,
+                           float* cand_score, int* cand_tok, long long* run_seq, long long* fin_seq, float* fin_score,
+                           int* fin_state, long long* ids, int* pos_rows, int* anc, float* scores, float* raw_logits,
+                           int n_slots, int* run_bidx, int* fin_bidx, void* stream);
+
 /* ---- next-token selection (the decode loop's last kernel) ------------------------------------
  * logits: 16-bit [B, V] rows, row pitch ld elements.  Writes out_ids[b] (int64, like the decode step's ids buffer).
  * greedy != 0: the arg-max of each row, first index among equal values -- replaces the `argmax` of transformers'
@@ -364,6 +378,25 @@ int g4r_sample_tokens_proc_bf16(const void* logits, long long ld, int B, int V, 
                                 int pad_id, int* finished, long long* out_ids, long long* history, long long ld_h, int L,
                                 float repetition_penalty, int no_repeat_ngram_size, int min_length, int min_new_tokens,
                                 const int* eos_ids, int n_eos, int append, void* stream);
+
+/* ---- next-token selection with transformers' generate() outputs (return_dict_in_generate) ------
+ * g4r_sample_tokens_proc_bf16 (same arguments, same selection, eos -> pad rule and history append) followed by an
+ * output pass into slot s = *rng_step of two fp32 buffers [n_slots, B, V] (contiguous; a slot >= n_slots is not
+ * written):
+ *   scores[s, b, :]: HF's next_token_scores -- the widened logits through the history-dependent processors, then,
+ *     when sampling, / temperature (IEEE division) and -inf below the top-k and top-p thresholds the selection uses
+ *     (the top-p group of equal values at the boundary kept whole, as the selection keeps it); greedy: no warpers;
+ *   raw_logits[s, b, :]: HF's next_token_logits, the logits widened to fp32.
+ * Either pointer may be NULL; with both NULL the call launches exactly what g4r_sample_tokens_bf16 (history NULL) or
+ * g4r_sample_tokens_proc_bf16 launches.  history may be NULL: the plain selection, with every processor neutral
+ * (repetition_penalty 1, no_repeat_ngram_size 0, n_eos 0), else refused.  With an output rng_step is required.
+ * Capturable: every per-step value is read from device memory. */
+int g4r_sample_tokens_out_bf16(const void* logits, long long ld, int B, int V, float temperature, int top_k,
+                               float top_p, int greedy, unsigned long long seed, const long long* rng_step, int eos_id,
+                               int pad_id, int* finished, long long* out_ids, long long* history, long long ld_h, int L,
+                               float repetition_penalty, int no_repeat_ngram_size, int min_length, int min_new_tokens,
+                               const int* eos_ids, int n_eos, int append, float* scores, float* raw_logits,
+                               long long n_slots, void* stream);
 
 /* ---- stop strings (after the next-token selection, once per decode step) ---------------------
  * Replaces transformers.generation.stopping_criteria.StopStringCriteria.__call__ (and, per row, the reference's
@@ -755,6 +788,18 @@ int g4r_beam_step_f16(const void* logits, long long ld, int row_div, int B, int 
                       int Lmax, const int* lens, int* state, float* run_score, float* cand_score, int* cand_tok,
                       long long* run_seq, long long* fin_seq, float* fin_score, int* fin_state, long long* ids,
                       int* pos_rows, int* anc, void* stream);
+int g4r_sample_tokens_out_f16(const void* logits, long long ld, int B, int V, float temperature, int top_k,
+                              float top_p, int greedy, unsigned long long seed, const long long* rng_step, int eos_id,
+                              int pad_id, int* finished, long long* out_ids, long long* history, long long ld_h, int L,
+                              float repetition_penalty, int no_repeat_ngram_size, int min_length, int min_new_tokens,
+                              const int* eos_ids, int n_eos, int append, float* scores, float* raw_logits,
+                              long long n_slots, void* stream);
+int g4r_beam_step_out_f16(const void* logits, long long ld, int row_div, int B, int N, int V, int K,
+                          const int* eos_ids, int n_eos, int prompt_len, int max_length, double length_penalty,
+                          int early_stopping, int G, int Lmax, const int* lens, int* state, float* run_score,
+                          float* cand_score, int* cand_tok, long long* run_seq, long long* fin_seq, float* fin_score,
+                          int* fin_state, long long* ids, int* pos_rows, int* anc, float* scores, float* raw_logits,
+                          int n_slots, int* run_bidx, int* fin_bidx, void* stream);
 
 #ifdef __cplusplus
 }
