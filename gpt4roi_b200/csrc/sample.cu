@@ -485,12 +485,14 @@ __device__ void select_processed(const unsigned short* __restrict__ row, int V, 
     });
 }
 
+// rng_row: the row word of the plain selection's Philox counter -- blockIdx.x for a batch, 0 for the per-row kernel,
+// whose rows each draw as a batch of one would.
 template <bool PROC, bool OUT>
 __device__ __forceinline__ void sample_row(const unsigned short* __restrict__ logits, long long ld, int V,
                                            float temperature, int top_k, float top_p, int greedy,
                                            unsigned long long seed, const long long* __restrict__ rng_step, int eos_id,
                                            int pad_id, int* __restrict__ finished, long long* __restrict__ out_ids,
-                                           const SampleProc& proc, const SampleOut& out) {
+                                           const SampleProc& proc, const SampleOut& out, unsigned rng_row) {
   extern __shared__ unsigned hist[];
   __shared__ unsigned long long s_best[32];
   __shared__ int s_int[32];
@@ -608,7 +610,7 @@ __device__ __forceinline__ void sample_row(const unsigned short* __restrict__ lo
     __syncthreads();
     // ---- inverse CDF over the kept values, from the top
     const long long step = *rng_step;
-    const uint4 r = philox4x32_10(make_uint4((unsigned)step, (unsigned)((unsigned long long)step >> 32), (unsigned)b, 0u),
+    const uint4 r = philox4x32_10(make_uint4((unsigned)step, (unsigned)((unsigned long long)step >> 32), rng_row, 0u),
                                   make_uint2((unsigned)seed, (unsigned)(seed >> 32)));
     const float target = (float)(r.x >> 8) * 0x1p-24f * s_zk;
     if (tid == 0) {
@@ -692,7 +694,7 @@ sample_tokens_kernel(const unsigned short* __restrict__ logits, long long ld, in
                      int eos_id, int pad_id, int* __restrict__ finished, long long* __restrict__ out_ids,
                      SampleProc proc) {
   sample_row<PROC, false>(logits, ld, V, temperature, top_k, top_p, greedy, seed, rng_step, eos_id, pad_id, finished,
-                          out_ids, proc, SampleOut{});
+                          out_ids, proc, SampleOut{}, blockIdx.x);
 }
 
 // The same selection followed by the output pass; a separate kernel, so the selection-only kernels stay as they are.
@@ -703,7 +705,28 @@ sample_tokens_out_kernel(const unsigned short* __restrict__ logits, long long ld
                          int eos_id, int pad_id, int* __restrict__ finished, long long* __restrict__ out_ids,
                          SampleProc proc, SampleOut out) {
   sample_row<PROC, true>(logits, ld, V, temperature, top_k, top_p, greedy, seed, rng_step, eos_id, pad_id, finished,
-                         out_ids, proc, out);
+                         out_ids, proc, out, blockIdx.x);
+}
+
+// The per-row kernel (g4r_sample_tokens_rows_*): the decode step of a continuous batch, whose rows are independent
+// requests.  Row r runs the plain selection on its own rule, seed and counter step[r]; an inactive row returns before
+// any work.  `lens` is the step's last write: the decode kernels of the same step have read it already.
+__global__ void __launch_bounds__(SAMPLE_THREADS, 1)
+sample_tokens_rows_kernel(const unsigned short* __restrict__ logits, long long ld, int V, const int* __restrict__ greedy,
+                          const float* __restrict__ temperature, const int* __restrict__ top_k,
+                          const float* __restrict__ top_p, const unsigned long long* __restrict__ seed,
+                          long long* __restrict__ step, const int* __restrict__ eos_id, const int* __restrict__ active,
+                          int* __restrict__ finished, long long* __restrict__ out_ids, int* __restrict__ lens) {
+  const int r = blockIdx.x;
+  if (!active[r]) return;   // uniform over the CTA
+  sample_row<false, false>(logits, ld, V, temperature[r], top_k[r], top_p[r], greedy[r], seed[r], step + r, -1, -1,
+                           nullptr, out_ids, SampleProc{}, SampleOut{}, 0u);
+  if (threadIdx.x == 0) {   // the thread that wrote out_ids[r]
+    const long long tok = out_ids[r];
+    if (eos_id[r] >= 0 && tok == eos_id[r]) finished[r] = 1;
+    step[r] += 1;
+    if (lens) lens[r] += 1;
+  }
 }
 
 }  // namespace G4R_NS
@@ -795,6 +818,30 @@ extern "C" int g4r_sample_tokens_bf16(const void* logits, long long ld, int B, i
                                       int eos_id, int pad_id, int* finished, long long* out_ids, void* stream) {
   return launch_plain<false>(logits, ld, B, V, temperature, top_k, top_p, greedy, seed, rng_step, eos_id, pad_id,
                              finished, out_ids, SampleOut{}, stream);
+}
+
+extern "C" int g4r_sample_tokens_rows_bf16(const void* logits, long long ld, int S, int V, const int* greedy,
+                                           const float* temperature, const int* top_k, const float* top_p,
+                                           const unsigned long long* seed, long long* step, const int* eos_id,
+                                           const int* active, int* finished, long long* out_ids, int* lens,
+                                           void* stream) {
+  G4R_REQUIRE(logits && out_ids && S > 0 && V > 0 && V < 65536 && ld >= V,
+              "sample_tokens_rows: bad arguments (S=%d V=%d ld=%lld; V < 65536)", S, V, ld);
+  G4R_REQUIRE(greedy && temperature && top_k && top_p && seed && step && eos_id && active && finished,
+              "sample_tokens_rows: every per-row array but lens is required");
+  cudaStream_t st = (cudaStream_t)stream;
+  static bool set = false;
+  if (!set) {
+    G4R_CUDA(cudaFuncSetAttribute(sample_tokens_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                  (int)SAMPLE_SMEM));
+    set = true;
+  }
+  // the sampling amount always: which rows sample is device data, and a captured launch serves every later admission
+  sample_tokens_rows_kernel<<<S, SAMPLE_THREADS, SAMPLE_SMEM, st>>>(
+      (const unsigned short*)logits, ld, V, greedy, temperature, top_k, top_p, seed, step, eos_id, active, finished,
+      out_ids, lens);
+  G4R_LAUNCH_CHECK("sample_tokens_rows");
+  return G4R_OK;
 }
 
 extern "C" int g4r_sample_tokens_proc_bf16(const void* logits, long long ld, int B, int V, float temperature, int top_k,

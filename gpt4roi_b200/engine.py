@@ -1248,6 +1248,225 @@ class GraphedDecode:
         return self.logits
 
 
+class Request:
+    """A request of a ContinuousBatcher: `sequences` (host int64 [1, L + n]: the prompt as given, then the n new tokens,
+    HF's layout) grows by one token per step while it runs; `done` turns True when it retires -- it emitted its eos id,
+    ended a stop string, or has max_new_tokens new tokens -- or when its admission failed: `error` is then the exception,
+    which ContinuousBatcher.step() raised, and the request has no new tokens."""
+
+    def __init__(self, input_ids, images, bboxes, max_new_tokens, greedy, temperature, top_k, top_p, seed, eos_id,
+                 streamer):
+        self.input_ids, self.images, self.bboxes = input_ids, images, bboxes
+        self.max_new_tokens = max_new_tokens
+        self.greedy, self.temperature, self.top_k, self.top_p, self.seed = greedy, temperature, top_k, top_p, seed
+        self.eos_id, self.streamer = eos_id, streamer
+        self.tokens = []
+        self.done = False
+        self.error = None
+
+    @property
+    def sequences(self):
+        return torch.cat([self.input_ids.cpu(), torch.tensor(self.tokens, dtype=torch.int64)[None]], 1)
+
+
+class ContinuousBatcher:
+    """Continuous (in-flight) batching of generate requests on one engine: `slots` decode rows, each holding one request
+    with its own prompt length, sampling rule, seed, eos id and answer length.  A queued request joins a free row
+    between two decode steps -- prefilled at batch 1 straight into its row of the batcher's KV cache -- while the others
+    keep decoding, and leaves it as soon as it finishes, so the weights streamed by each step serve every running request.
+
+    Row r's token is the one generate() selects for the request alone: the first from its prefill logits, then one per
+    decode step, drawn by kernels.sample_tokens_rows with Philox key = its seed and counter (its token count, 0), as a
+    batch-1 generate() draws.  The decode step runs on a KVCache(cfg, slots, max_len) with per-row lengths, allocated
+    up front and never grown; on CUDA it is one graph (decode step, selection, stop strings), captured once, whose
+    device-side state -- the per-row rule arrays, `active`, `finished`, the lengths -- admissions rewrite in place.
+    stop_strings: a StopStrings for every request (transformers' stop_strings).  On CPU tensors (the engine's host
+    stand-ins) the steps run eagerly with a greedy host selection."""
+
+    def __init__(self, engine, slots, max_len, stop_strings=None):
+        if slots < 1 or max_len < 2:
+            raise ValueError('ContinuousBatcher needs slots >= 1 and max_len >= 2 (got %d, %d)' % (slots, max_len))
+        self.eng, self.slots, self.max_len = engine, int(slots), int(max_len)
+        dev = engine.dev
+        S = self.slots
+        self.cache = KVCache(engine.cfg, S, self.max_len, dev)
+        self.cache.lens = torch.zeros(S, dtype=torch.int32, device=dev)
+
+        def vec(fill, dt):
+            return torch.full((S,), fill, dtype=dt, device=dev)
+        # the per-row rule and state that kernels.sample_tokens_rows reads, in its argument order
+        self.greedy, self.temperature = vec(1, torch.int32), vec(1.0, torch.float32)
+        self.top_k, self.top_p = vec(0, torch.int32), vec(1.0, torch.float32)
+        self.seed, self.step_count = vec(0, torch.int64), vec(0, torch.int64)
+        self.eos_id, self.active, self.finished = vec(-1, torch.int32), vec(0, torch.int32), vec(0, torch.int32)
+        self.stops = stop_strings
+        self.stop_table = None if stop_strings is None else stop_strings.on(dev)
+        self.stop_state = vec(0, torch.int32)
+        self.ids = torch.zeros((S, 1), dtype=torch.int64, device=dev)     # the decode step's input: each row's last token
+        self.pos = torch.zeros(1, dtype=torch.int32, device=dev)          # pos_dev: positions come from cache.lens
+        self.readback = torch.zeros((S, 2), dtype=torch.int64, device=dev)   # (token, finished) per row: one copy out
+        self.queue = collections.deque()
+        self.running = [None] * S
+        self.graph = None
+        if engine.dev.type == 'cuda':
+            self.graph, _ = _capture(dev, self._decode, self._decode)   # every row is idle: the warm-up selects nothing
+
+    def _select(self, logits, rows, lens):
+        """The selection of rows `rows` (a slice) from logits [n, 1, V] into self.ids[rows], then the stop strings."""
+        ids, fin = self.ids[rows], self.finished[rows]
+        if logits.is_cuda:
+            kernels.sample_tokens_rows(logits, ids, self.greedy[rows], self.temperature[rows], self.top_k[rows],
+                                       self.top_p[rows], self.seed[rows], self.step_count[rows], self.eos_id[rows],
+                                       self.active[rows], fin, lens)
+            if self.stop_table is not None:
+                kernels.stop_step(ids, self.stop_table, self.stop_state[rows], fin)
+            return
+        # host stand-in (Sampler._host's counterpart): greedy rows only, same state updates as the kernels
+        live = self.active[rows].bool()
+        if bool((live & (self.greedy[rows] == 0)).any()):
+            raise RuntimeError('token sampling runs on the CUDA device only (csrc/sample.cu): logits are on %s'
+                               % logits.device)
+        tok = torch.where(live, logits.reshape(live.shape[0], -1).argmax(-1), ids[:, 0])
+        ids[:, 0] = tok
+        eos = self.eos_id[rows]
+        fin |= (live & (eos >= 0) & (tok == eos)).to(torch.int32)
+        self.step_count[rows] += live.to(torch.int64)
+        if lens is not None:
+            lens += live.to(torch.int32)
+        if self.stop_table is not None:
+            state = self.stop_state[rows]
+            new, hit = _stop_lookup(self.stop_table, tok, state.to(torch.int64))
+            open_ = fin == 0
+            state.copy_(torch.where(open_, new.to(torch.int32), state))
+            fin |= (open_ & hit).to(torch.int32)
+
+    def _decode(self):
+        """One decode step over every row (the captured graph's body): forward, selection, stop strings, readback."""
+        self.cache.length = 0     # positions come from cache.lens; pos_dev sizes the attention by max_len
+        logits = self.eng.decode_step(self.ids, self.cache, self.pos)
+        self.cache.length = 0
+        self._select(logits, slice(None), self.cache.lens)
+        self.readback[:, 0:1].copy_(self.ids)
+        self.readback[:, 1].copy_(self.finished)
+        return logits
+
+    def submit(self, input_ids, images=None, bboxes=None, max_new_tokens=32, do_sample=False, temperature=1.0,
+               top_k=None, top_p=None, generator=None, eos_token_id=None, streamer=None):
+        """Queue one request and return its Request.  input_ids: int64 [1, L] or [L]; images [1, 3, S, S] or None;
+        bboxes: a list of one [K, 4] box tensor, or None.  Sampling as generate(): do_sample with temperature > 0 draws
+        from the temperature / top_k / top_p processed softmax with a seed taken from `generator` (default: torch's
+        default generator) now, at submission; otherwise the arg-max.  eos_token_id: an id, or a list of one.
+        streamer: transformers' BaseStreamer contract -- put(prompt ids) at admission, put(token) per new token, end()."""
+        ids = torch.as_tensor(input_ids)
+        if ids.dim() == 1:
+            ids = ids[None]
+        if ids.dim() != 2 or ids.shape[0] != 1 or ids.shape[1] < 1:
+            raise ValueError('submit takes one prompt: input_ids [1, L] or [L], got %s' % (tuple(ids.shape),))
+        L, n = ids.shape[1], int(max_new_tokens)
+        if n < 1:
+            raise ValueError('max_new_tokens must be >= 1, got %d' % n)
+        if L + n > self.max_len:
+            raise ValueError('prompt (%d) + max_new_tokens (%d) exceed the batcher\'s max_len %d'
+                             % (L, n, self.max_len))
+        if isinstance(eos_token_id, (list, tuple)):
+            if len(eos_token_id) > 1:
+                raise NotImplementedError('the continuous batcher stops a request on one eos id, got %r: run it with '
+                                          'model.generate' % (list(eos_token_id),))
+            eos_token_id = eos_token_id[0] if eos_token_id else None
+        greedy = not (do_sample and temperature > 0)
+        if not greedy and top_p is not None and top_p < 0:
+            raise ValueError('top_p must be >= 0, got %r' % (top_p,))
+        req = Request(ids.to(torch.int64), images, bboxes, n, greedy, float(temperature), int(top_k or 0),
+                      1.0 if top_p is None else float(top_p), 0 if greedy else sampling_seed(generator),
+                      -1 if eos_token_id is None else int(eos_token_id), streamer)
+        self.queue.append(req)
+        return req
+
+    def _emit(self, s, tok, finished):
+        """Give slot s's request its new token; retire it when it is done.  Returns it when it retired."""
+        req = self.running[s]
+        req.tokens.append(int(tok))
+        if req.streamer is not None:
+            req.streamer.put(torch.tensor([int(tok)]))
+        if not (finished or len(req.tokens) >= req.max_new_tokens):
+            return None
+        req.done = True
+        self.running[s] = None
+        self.active[s] = 0
+        if req.streamer is not None:
+            req.streamer.end()
+        return req
+
+    def _admit(self, req, s):
+        """Prefill `req` into slot s (batch 1, straight into the slot's rows of the cache) and select its first token.
+        The slot's device state is written only once the prefill has succeeded, and a failure after that makes the slot
+        idle again: a request that cannot run (say, a <bbox> count its boxes do not match) leaves no active row behind."""
+        eng, cfg = self.eng, self.eng.cfg
+        dev = eng.dev
+        ids = req.input_ids.to(dev)
+        L = ids.shape[1]
+        row = slice(s, s + 1)
+        one = KVCache(cfg, 1, self.max_len, dev, kv=([k[row] for k in self.cache.k], [v[row] for v in self.cache.v]))
+        images = None if req.images is None else req.images.to(dev, eng.dt)
+        logits = eng.forward_device(ids, images, eng.plan_boxes(req.bboxes), validate=True, last_only=True, cache=one)
+        try:
+            for t, v in ((self.greedy, int(req.greedy)), (self.temperature, req.temperature), (self.top_k, req.top_k),
+                         (self.top_p, req.top_p), (self.seed, req.seed), (self.step_count, 0),
+                         (self.eos_id, req.eos_id), (self.finished, 0), (self.active, 1)):
+                t[row] = v
+            if self.stops is not None:
+                self.stop_state[row] = self.stops.initial_states(req.input_ids, torch.tensor([L])).to(dev)
+            self._select(logits, row, None)
+            self.cache.lens[row] = L
+            tok, fin = torch.stack([self.ids[s, 0], self.finished[s].to(torch.int64)]).tolist()
+        except BaseException:
+            self.active[row] = 0
+            raise
+        if req.streamer is not None:
+            req.streamer.put(req.input_ids.cpu())
+        self.running[s] = req
+        return self._emit(s, tok, fin)
+
+    def step(self):
+        """Admit queued requests into free slots (first in, first out), run one decode step over every slot, hand each
+        running request its token and retire the finished ones.  Returns the requests that finished.  When a request's
+        admission fails, it is retired with `error` set and the exception propagates; its slot stays idle and the next
+        step() carries on with the other requests."""
+        done = []
+        for s in range(self.slots):
+            while self.running[s] is None and self.queue:
+                req = self.queue.popleft()
+                try:
+                    r = self._admit(req, s)
+                except Exception as e:   # the request retires unanswered; the others keep their rows
+                    req.error, req.done = e, True
+                    if req.streamer is not None:
+                        req.streamer.end()
+                    raise
+                if r is not None:
+                    done.append(r)
+        if not any(r is not None for r in self.running):
+            return done
+        if self.graph is not None:
+            self.graph.replay()
+        else:
+            self._decode()
+        rb = self.readback.cpu()
+        for s in range(self.slots):
+            if self.running[s] is not None:
+                r = self._emit(s, rb[s, 0], bool(rb[s, 1]))
+                if r is not None:
+                    done.append(r)
+        return done
+
+    def run(self):
+        """Step until nothing is queued or running; returns every request that finished, in the order they did."""
+        done = []
+        while self.queue or any(r is not None for r in self.running):
+            done += self.step()
+        return done
+
+
 class _SharedPromptCache:
     """KV layout of N decode rows per prompt that share the prompt's K/V (beam search, several sampled answers).  Per
     layer one [B + B*N, Lmax, HD] tensor (full_k / full_v): rows 0..B-1 hold the B prompts (n_samples; the B-row

@@ -234,6 +234,33 @@ def sample_tokens(logits, out, greedy, temperature=1.0, top_k=0, top_p=1.0, seed
     return out
 
 
+def sample_tokens_rows(logits, out, greedy, temperature, top_k, top_p, seed, step, eos_id, active, finished, lens=None):
+    """Next token of every active row of 16-bit logits [S, V] (or [S, 1, V]; unit column stride) into out (int64, S
+    contiguous elements), each row with its own rule (include/gpt4roi_b200.h: g4r_sample_tokens_rows_bf16): row r selects
+    as sample_tokens on that row alone with rng_step = step[r].  Per-row contiguous device vectors of S entries: greedy,
+    top_k, eos_id (-1: none), active (int32); temperature, top_p (fp32); seed (int64, read as uint64); step (int64).
+    An active row sets finished[r] when its token is eos_id[r], advances step[r] and, when given, lens[r] (int32 [S]);
+    an inactive row is left alone.  A sampled row needs temperature > 0 and top_p >= 0: the caller checks, the rule is
+    device data."""
+    rows, act = _logit_rows('sample_tokens_rows', logits)
+    S, V = rows.shape
+    if out.dtype != torch.int64 or out.numel() != S or not out.is_contiguous():
+        raise RuntimeError('sample_tokens_rows: out must be a contiguous int64 tensor of %d elements' % S)
+    named = [('greedy', greedy, torch.int32), ('temperature', temperature, torch.float32),
+             ('top_k', top_k, torch.int32), ('top_p', top_p, torch.float32), ('seed', seed, torch.int64),
+             ('step', step, torch.int64), ('eos_id', eos_id, torch.int32), ('active', active, torch.int32),
+             ('finished', finished, torch.int32), ('lens', lens, torch.int32)]
+    for name, t, dt in named:
+        if t is None and name == 'lens':
+            continue
+        if t is None or t.dtype != dt or t.numel() != S or not t.is_contiguous():
+            raise RuntimeError('sample_tokens_rows: %s must be a contiguous device %s [%d] vector' % (name, dt, S))
+    _L.require_cuda_same_device([('logits', rows), ('out', out)] + [(n, t) for n, t, _ in named])
+    _call('g4r_sample_tokens_rows_bf16', rows.device, _L.ptr(rows), rows.stride(0), S, V,
+          *[_L.ptr(t) for _, t, _ in named[:8]], _L.ptr(finished), _L.ptr(out), _L.ptr(lens), act=act)
+    return out
+
+
 PROC_LIST_MAX = 8192   # history ids per row that sampling with a repetition penalty holds (csrc/sample.cu)
 
 

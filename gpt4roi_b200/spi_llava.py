@@ -36,8 +36,8 @@ import torch.nn as nn
 from transformers import LlamaConfig, LlamaForCausalLM, LlamaModel
 from transformers.modeling_outputs import BaseModelOutputWithPast, CausalLMOutputWithPast
 
-from .engine import (BF16, EngineConfig, KVCache, PrefillEngine, StopStrings, _right_padded, from_right_padded,
-                     right_pad_layout)
+from .engine import (BF16, ContinuousBatcher, EngineConfig, KVCache, PrefillEngine, StopStrings, _right_padded,
+                     from_right_padded, right_pad_layout)
 from .roi_align import RoIAlign
 
 DEFAULT_IMAGE_PATCH_TOKEN = '<im_patch>'
@@ -964,6 +964,17 @@ class SPILlavaMPTForCausalLM(LlamaForCausalLM, _EngineHost):
                            min_new_tokens=procs['min_new_tokens'], length_eos_ids=procs['eos_ids'], **outs)
         return _generate_output(res, outs, pkv) if outs['return_dict_in_generate'] else res
 
+    def continuous_batcher(self, slots=8, max_len=2048, tokenizer=None, stop_strings=None):
+        """A ContinuousBatcher (engine.ContinuousBatcher: requests join and leave the graphed decode step one row at a
+        time) on this model's engine, with `slots` rows of up to max_len tokens each.  stop_strings (with tokenizer=;
+        resolve_stop_strings, so the model's generation config counts) apply to every request.  Its submit(input_ids,
+        images=, bboxes=, max_new_tokens=, **generate_kwargs) resolves each request's sampling rule as the engine loop
+        of generate() does."""
+        stops = resolve_stop_strings(self, tokenizer, stop_strings)
+        eng = self._get_engine(self.device)
+        return SeamBatcher(self, ContinuousBatcher(eng, slots, max_len, None if stops is None else
+                                                   stop_strings_from_tokenizer(tokenizer, stops)))
+
     def initialize_vision_tokenizer(self, mm_use_im_start_end, tokenizer, device, tune_mm_mlp_adapter=False,
                                     pretrain_mm_mlp_adapter=None):
         """spi_llava.py:242-306: token bookkeeping, embedding resize and the optional copy of the pretrained
@@ -1007,6 +1018,54 @@ class SPILlavaMPTForCausalLM(LlamaForCausalLM, _EngineHost):
         for m in self.modules():
             m.tokenizer = tokenizer
         self.invalidate_engine()
+
+
+class SeamBatcher:
+    """model.continuous_batcher(): the engine's ContinuousBatcher (`batcher`) with generate()'s keyword resolution."""
+
+    def __init__(self, model, batcher):
+        self.model, self.batcher = model, batcher
+
+    def submit(self, input_ids, images=None, bboxes=None, max_new_tokens=32, do_sample=None, temperature=None,
+               eos_token_id=None, generator=None, streamer=None, **generate_kwargs):
+        """Queue one request ([1, L] or [L] ids) and return its engine.Request.  do_sample / temperature / top_k /
+        top_p / generation_config resolve as on generate()'s engine loop (resolve_sampling: `do_sample=True` alone
+        samples from the top 50); eos_token_id stops the request as it stops that loop.  As on that loop, only the
+        sampling rule (and what is refused below) is read from generation_config: max_new_tokens and eos_token_id are
+        this call's arguments.  What the batcher does not run -- logits processors, beam search, several answers per
+        prompt, generate outputs, stop strings per request (stop_strings=, or in generation_config) -- raises
+        NotImplementedError naming model.generate.  tokenizer= is accepted and unused: the batcher's stop strings, if
+        any, were resolved with its own tokenizer."""
+        gen = {k: v for k, v in generate_kwargs.items() if k not in ('pad_token_id', 'attention_mask', 'tokenizer')}
+        gc = gen.get('generation_config')
+        for k, v in (('stop_strings', gen.pop('stop_strings', None)), ('past_key_values', gen.pop('past_key_values', None)),
+                     ('generation_config.stop_strings', getattr(gc, 'stop_strings', None))):
+            if v is not None:
+                raise NotImplementedError('%s per request: the batcher takes stop strings once '
+                                          '(continuous_batcher(tokenizer=, stop_strings=)) and has no conversation '
+                                          'cache; run the request with model.generate' % k)
+        mask = generate_kwargs.get('attention_mask')
+        if mask is not None and not bool(torch.as_tensor(mask).bool().all()):
+            raise NotImplementedError('a padded prompt: submit its tokens alone, or run it with model.generate')
+        L = torch.as_tensor(input_ids).shape[-1]
+        try:
+            if resolve_num_return_sequences(self.model, do_sample, temperature, **gen) > 1:
+                raise NotImplementedError('num_return_sequences > 1')
+            if resolve_outputs(self.model, do_sample, temperature, **gen)['return_dict_in_generate']:
+                raise NotImplementedError('return_dict_in_generate / output_scores / output_logits')
+            do_sample, temperature, top_k, top_p = resolve_sampling(self.model, L, do_sample, temperature,
+                                                                    eos_token_id=eos_token_id, **gen)
+        except NotImplementedError as e:
+            raise NotImplementedError('the continuous batcher selects with temperature, top_k and top_p only (%s): run '
+                                      'this request with model.generate' % e) from None
+        return self.batcher.submit(input_ids, images, bboxes, max_new_tokens, do_sample, temperature, top_k, top_p,
+                                   generator, eos_token_id, streamer)
+
+    def step(self):
+        return self.batcher.step()
+
+    def run(self):
+        return self.batcher.run()
 
 
 class KeywordsStoppingCriteria:

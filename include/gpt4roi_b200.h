@@ -398,6 +398,22 @@ int g4r_sample_tokens_out_bf16(const void* logits, long long ld, int B, int V, f
                                const int* eos_ids, int n_eos, int append, float* scores, float* raw_logits,
                                long long n_slots, void* stream);
 
+/* ---- next-token selection with a rule per row (a continuous batch of independent requests) -------
+ * logits: 16-bit [S, V] rows, row pitch ld elements.  Per-row device arrays of S entries: greedy (int32), temperature
+ * (fp32), top_k (int32, 0: off), top_p (fp32, 1: off), seed (uint64), step (int64: the row's Philox counter and
+ * token count), eos_id (int32, -1: none), active (int32).  For every row r with active[r] != 0, the selection of
+ * g4r_sample_tokens_bf16 on row r's parameters, with Philox counter (step[r], 0, 0) -- the token a B = 1 call with
+ * the same logits, seed and *rng_step = step[r] selects; greedy and sampled rows may share one launch.  Then
+ * out_ids[r] = the token, finished[r] = 1 when it equals eos_id[r] (no pad rule), step[r] += 1, and, when lens
+ * (int32 [S], the KV cache's per-row lengths) is non-NULL, lens[r] += 1 as the launch's last write.  A row with
+ * active[r] == 0 is left alone: finished, step, lens and out_ids[r] keep their values.  Needs V < 65536; a sampled
+ * row needs temperature > 0 and top_p >= 0 (the caller's check: the rule is device data).
+ * Capturable: every per-step value is read from device memory. */
+int g4r_sample_tokens_rows_bf16(const void* logits, long long ld, int S, int V, const int* greedy,
+                                const float* temperature, const int* top_k, const float* top_p,
+                                const unsigned long long* seed, long long* step, const int* eos_id, const int* active,
+                                int* finished, long long* out_ids, int* lens, void* stream);
+
 /* ---- stop strings (after the next-token selection, once per decode step) ---------------------
  * Replaces transformers.generation.stopping_criteria.StopStringCriteria.__call__ (and, per row, the reference's
  * KeywordsStoppingCriteria, llava/model/utils.py:26-46) for the decode loop: a row stops at the first generated token
@@ -800,6 +816,10 @@ int g4r_beam_step_out_f16(const void* logits, long long ld, int row_div, int B, 
                           float* cand_score, int* cand_tok, long long* run_seq, long long* fin_seq, float* fin_score,
                           int* fin_state, long long* ids, int* pos_rows, int* anc, float* scores, float* raw_logits,
                           int n_slots, int* run_bidx, int* fin_bidx, void* stream);
+int g4r_sample_tokens_rows_f16(const void* logits, long long ld, int S, int V, const int* greedy,
+                               const float* temperature, const int* top_k, const float* top_p,
+                               const unsigned long long* seed, long long* step, const int* eos_id, const int* active,
+                               int* finished, long long* out_ids, int* lens, void* stream);
 
 #ifdef __cplusplus
 }
