@@ -16,11 +16,15 @@
 //                coordinates are zero-filled by TMA = the padding.
 //   warpgroups 1, 2 : consumers -- each issues wgmma m64nBNk16 for its 64 rows of the tile (fp32
 //                accumulators in registers) and releases the smem slot (`empty`) once its MMAs have read it.
-//                After the last k-block both stage their accumulators in shared memory, 128 columns at a
-//                time, and run the epilogue on each 128-column half: thread = (row, half of the columns),
-//                32 columns at a time -- fused bias / activation / residual / SwiGLU / RoPE / GroupNorm
-//                statistics, bf16 or fp32 store.  Meanwhile the producer is already loading the next tile's
-//                operands.
+//                After the last k-block a 16-bit output (forward GEMMs, no split-K, 16-bit or no residual,
+//                TMA-aligned rows) takes the register epilogue (epilogue_regs): each warpgroup finishes its
+//                accumulators in place -- bias / activation / residual / SwiGLU / RoPE -- into 64 x 64 swizzled
+//                boxes in shared memory, one thread stores them with TMA, and the warpgroup goes on to its next
+//                tile; the residual was loaded by TMA into those boxes while the MMAs ran.  Everything else (fp32
+//                outputs and residuals, split-K, convs with GroupNorm statistics, the training GEMMs) stages the
+//                accumulators in shared memory, 128 columns at a time, and runs epilogue_tile on each half:
+//                thread = (row, half of the columns), 32 columns at a time.  Meanwhile the producer is already
+//                loading the next tile's operands.
 // The operand majorness (TA, TB) is a template parameter, so each mainloop is straight-line code: every
 // k-block's four MMAs and their commit_group sit in one basic block, and wait_group 1 keeps one k-block of
 // MMAs in flight.  At BN = 256 the 128 accumulators per consumer thread need setmaxnreg: the producer
@@ -64,6 +68,7 @@ struct GemmParams {
   int act;
   int out_f32;   // 1: fp32 output
   int d_vec, r_vec;  // D / residual rows take 16-byte vector accesses: 16-byte aligned base and row pitch (launch_gemm)
+  int tma_epi;       // register epilogue with TMA stores (epilogue_regs): tmap_d / tmap_r describe D and the residual
   // conv mode
   int conv;
   int cH, cW, cBH, cBW, tiles_x, tiles_y, cin_blocks, taps;  // taps = 9 (3x3) or 1
@@ -88,6 +93,7 @@ struct GemmParams {
 
 // Shared memory: BN = 128: 4 stages x 32 KB + 66 KB staging = 194 KB;
 //                BN = 256: 3 stages x 48 KB + 66 KB staging = 210 KB (a 4th stage does not fit beside the staging tile).
+// The register epilogue's boxes (2 warpgroups x BN / 64 boxes of 8 KB: 32 or 64 KB) reuse the staging tile.
 template <int BN>
 struct GemmCfg {
   static constexpr int kStages = BN == 256 ? 3 : 4;
@@ -96,8 +102,13 @@ struct GemmCfg {
   static constexpr int kStageBytes = kABytes + kBBytes;
   static constexpr int kAccLd = kEpiN + 4;                // fp32 staging row stride (conflict-free row reads)
   static constexpr int kAccBytes = kBlockM * kAccLd * 4;  // 66 KB
-  static constexpr int kBarBytes = 2 * kStages * 8;
+  static constexpr int kBarBytes = (2 * kStages + 2) * 8;
   static constexpr int kSmemBytes = kStages * kStageBytes + kAccBytes + kBarBytes + 1024;  // +1024 alignment slack
+  // register epilogue: each consumer warpgroup's 64 x BN output block as BN / 64 TMA boxes of 64 rows x 128 B,
+  // in the region of the fp32 staging tile
+  static constexpr int kBoxBytes = 64 * 128;
+  static constexpr int kWgStageBytes = (BN / 64) * kBoxBytes;
+  static_assert(2 * kWgStageBytes <= kAccBytes, "register-epilogue staging exceeds the staging tile");
 };
 static_assert(GemmCfg<128>::kSmemBytes <= 227 * 1024, "GEMM shared memory exceeds the sm_90 per-block limit");
 static_assert(GemmCfg<256>::kSmemBytes <= 227 * 1024, "GEMM shared memory exceeds the sm_90 per-block limit");
@@ -341,6 +352,136 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float* 
   }
 }
 
+// Epilogue of one consumer warpgroup's 64 x BN block straight from the accumulators (16-bit output, no split-K,
+// no GroupNorm statistics, 16-bit or no residual; gemm_impl decides).  The same fp32 operations in the same order as
+// epilogue_tile, so the output is bitwise the same.  The thread holds rows rl and rl + 8 of the block, columns
+// 8j + 2(lane & 3) + {0, 1} (acc[4j + 2h + e]: row rl + 8h); each pair is finished, packed to 16 bits and written at
+// once into `stg`, BN / 64 boxes of 64 rows x 128 B in the 128-byte swizzle of the D / residual tensor maps.  The
+// residual, when there is one, has already been loaded by TMA into exactly those places, so each pair reads its
+// residual where it then writes its output.  SwiGLU halves the columns: pair j of row r becomes output column
+// 4j + (lane & 3).  Rows at or past M are computed but never stored (TMA clips the box).
+template <int BN>
+__device__ __forceinline__ void epilogue_regs(const GemmParams& p, float (&acc)[BN / 2], uint32_t stg, int row0,
+                                              int col0, int wt) {
+  constexpr int kBox = GemmCfg<BN>::kBoxBytes;
+  const int lane = wt & 31, c = lane & 3;
+  const int rl = (wt >> 5) * 16 + (lane >> 2);
+  const int sw = lane >> 2;  // row & 7 of both rows: a row's 16-byte chunk index is xor-ed with it
+  const uint32_t srow = stg + rl * 128;
+  // pair (j, h): 16-byte chunk j & 7 of box j / 8, row rl + 8h
+  auto pair_addr = [&](int j, int h) { return srow + h * 1024 + (j >> 3) * kBox + (((j & 7) ^ sw) << 4) + 4 * c; };
+  if (p.rope_cos != nullptr && col0 < p.rope_cols) {
+    // RoPE as in epilogue_tile: dims d and d + 64 of a head are accumulator blocks j and j + 8; the cos / sin values
+    // of the thread's dims are the same for every head of the tile, so they are loaded once per row, up front
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+      const long long out_row = row0 + rl + 8 * h;
+      int pos = 0;
+      if (out_row < p.M) {
+        const int base = p.rope_pos_rows ? p.rope_pos_rows[out_row / p.rope_L] : (p.rope_pos_dev ? *p.rope_pos_dev : p.rope_pos0);
+        pos = base + (int)(out_row % p.rope_L);
+      }
+      const uint32_t* ct = reinterpret_cast<const uint32_t*>(p.rope_cos + (long long)pos * 128) + c;
+      const uint32_t* st = reinterpret_cast<const uint32_t*>(p.rope_sin + (long long)pos * 128) + c;
+      uint32_t c1[8], s1[8], c2[8], s2[8];
+#pragma unroll
+      for (int j = 0; j < 8; j++) {
+        c1[j] = ct[4 * j]; s1[j] = st[4 * j]; c2[j] = ct[32 + 4 * j]; s2[j] = st[32 + 4 * j];
+      }
+#pragma unroll
+      for (int hd = 0; hd < BN / 128; hd++) {
+#pragma unroll
+        for (int j = 0; j < 8; j++) {
+          const int ja = hd * 16 + j, jb = ja + 8;
+          const float2 fc1 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&c1[j]));
+          const float2 fs1 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&s1[j]));
+          const float2 fc2 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&c2[j]));
+          const float2 fs2 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&s2[j]));
+          float r1[2], r2[2];
+#pragma unroll
+          for (int e = 0; e < 2; e++) {
+            const float x1 = __bfloat162float(__float2bfloat16_rn(acc[4 * ja + 2 * h + e]));
+            const float x2 = __bfloat162float(__float2bfloat16_rn(acc[4 * jb + 2 * h + e]));
+            const float cc1 = e ? fc1.y : fc1.x, ss1 = e ? fs1.y : fs1.x;
+            const float cc2 = e ? fc2.y : fc2.x, ss2 = e ? fs2.y : fs2.x;
+            const float a1 = __bfloat162float(__float2bfloat16_rn(x1 * cc1));
+            const float b1 = __bfloat162float(__float2bfloat16_rn(-x2 * ss1));
+            const float a2 = __bfloat162float(__float2bfloat16_rn(x2 * cc2));
+            const float b2 = __bfloat162float(__float2bfloat16_rn(x1 * ss2));
+            r1[e] = a1 + b1;
+            r2[e] = a2 + b2;
+          }
+          __nv_bfloat162 o1 = __floats2bfloat162_rn(r1[0], r1[1]);
+          __nv_bfloat162 o2 = __floats2bfloat162_rn(r2[0], r2[1]);
+          ptx::st_shared_u32(pair_addr(ja, h), *reinterpret_cast<uint32_t*>(&o1));
+          ptx::st_shared_u32(pair_addr(jb, h), *reinterpret_cast<uint32_t*>(&o2));
+        }
+      }
+    }
+    return;
+  }
+  // One branch-free pass over the accumulators per step that applies, so that the code a launch runs stays small
+  // (one loop holding every case unrolled over 64 pairs overflows the instruction cache at BN = 256).
+  // Columns at or past N get no bias and are never stored.
+  if (p.bias != nullptr) {
+#pragma unroll
+    for (int j = 0; j < BN / 8; j++) {
+#pragma unroll
+      for (int e = 0; e < 2; e++) {
+        const int col = col0 + 8 * j + 2 * c + e;
+        if (col < p.N) {
+          const float b = p.bias_f32 ? reinterpret_cast<const float*>(p.bias)[col]
+                                     : __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(p.bias)[col]);
+          acc[4 * j + e] += b;
+          acc[4 * j + 2 + e] += b;
+        }
+      }
+    }
+  }
+  if (p.act == ACT_RELU) {
+#pragma unroll
+    for (int i = 0; i < BN / 2; i++) acc[i] = fmaxf(acc[i], 0.f);
+  } else if (p.act == ACT_QUICK_GELU) {
+#pragma unroll
+    for (int i = 0; i < BN / 2; i++) acc[i] = act_apply(acc[i], ACT_QUICK_GELU);
+  } else if (p.act == ACT_SWIGLU) {
+    // interleaved gate / up: pair j of a row is output column 4j + c of the half-width output
+#pragma unroll
+    for (int j = 0; j < BN / 8; j++) {
+#pragma unroll
+      for (int h = 0; h < 2; h++) {
+        const float g = acc[4 * j + 2 * h], u = acc[4 * j + 2 * h + 1];
+        const __nv_bfloat16 o = __float2bfloat16_rn(g / (1.f + __expf(-g)) * u);
+        ptx::st_shared_u16(srow + h * 1024 + (j >> 4) * kBox + ((((j & 15) >> 1) ^ sw) << 4) + 8 * (j & 1) + 2 * c,
+                           *reinterpret_cast<const uint16_t*>(&o));
+      }
+    }
+    return;
+  }
+  if (p.residual != nullptr) {
+#pragma unroll
+    for (int j = 0; j < BN / 8; j++) {
+#pragma unroll
+      for (int h = 0; h < 2; h++) {
+        const uint32_t a = pair_addr(j, h);
+        const uint32_t r = ptx::ld_shared_u32(a);
+        const float2 rf = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&r));
+        __nv_bfloat162 o = __floats2bfloat162_rn(acc[4 * j + 2 * h] + rf.x, acc[4 * j + 2 * h + 1] + rf.y);
+        ptx::st_shared_u32(a, *reinterpret_cast<uint32_t*>(&o));
+      }
+    }
+    return;
+  }
+#pragma unroll
+  for (int j = 0; j < BN / 8; j++) {
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+      __nv_bfloat162 o = __floats2bfloat162_rn(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+      ptx::st_shared_u32(pair_addr(j, h), *reinterpret_cast<uint32_t*>(&o));
+    }
+  }
+}
+
 // One k = 16 MMA of the warpgroup's 64 x BN block; ZERO: the tile's first (scale-d = 0, write-only accumulators).
 template <int TA, int TB, int BN, bool ZERO>
 __device__ __forceinline__ void mma_k16(float (&acc)[BN / 2], uint64_t da, uint64_t db) {
@@ -368,11 +509,14 @@ __device__ __forceinline__ void mma_kblock(float (&acc)[BN / 2], uint64_t da, ui
 template <bool CONV, int TA, int TB, int BN>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                const __grid_constant__ CUtensorMap tmap_d, const __grid_constant__ CUtensorMap tmap_r,
                 const __grid_constant__ GemmParams p) {
   static_assert(BN == 128 || BN == 256, "tile width");
   static_assert(!CONV || (TA == 0 && TB == 0), "conv operands are K-major");
   using Cfg = GemmCfg<BN>;
   constexpr int kStages = Cfg::kStages;
+  // the register epilogue serves the forward GEMMs (K-major operands); convs and the training GEMMs stage
+  constexpr bool kRegEpi = !CONV && TA == 0 && TB == 0;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smem_a = smem;
@@ -381,6 +525,7 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmap_a, const __grid_constan
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kStages * Cfg::kStageBytes + Cfg::kAccBytes);
   uint64_t* full = bars;
   uint64_t* empty = bars + kStages;
+  uint64_t* stg_ready = bars + 2 * kStages;  // register epilogue: warpgroup wg's staging boxes may be written
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -391,6 +536,12 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmap_a, const __grid_constan
     for (int i = 0; i < kStages; i++) {
       ptx::mbar_init(&full[i], 1);
       ptx::mbar_init(&empty[i], 2);  // one arrival per consumer warpgroup
+    }
+    if (kRegEpi && p.tma_epi) {
+      ptx::prefetch_tensormap(&tmap_d);
+      if (p.residual) ptx::prefetch_tensormap(&tmap_r);
+      ptx::mbar_init(&stg_ready[0], 1);
+      ptx::mbar_init(&stg_ready[1], 1);
     }
     ptx::fence_barrier_init();
   }
@@ -468,12 +619,16 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmap_a, const __grid_constan
   const int row = ct & 127, half = ct >> 7;
   int stage = 0;
   uint32_t phase = 0;
+  uint32_t stg_phase = 0;
+  // register epilogue: this warpgroup's staging boxes (64 rows each) and the tile's first output row
+  uint8_t* stg = smem + kStages * Cfg::kStageBytes + wg * Cfg::kWgStageBytes;
   float acc[BN / 2];
   for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
     const int split = t / tiles_mn;
     const int mn = t % tiles_mn;
     const int n_blk = p.n_fast ? mn % p.num_n_tiles : mn / p.num_m_tiles;
     const int m_blk = p.n_fast ? mn / p.num_n_tiles : mn % p.num_m_tiles;
+    const int row0 = m_blk * kBlockM + wg * 64, col0 = n_blk * BN;
     // this warpgroup's 64 rows of A start 8 KB into the stage in both layouts (64 rows x 128 B, or mn atom wg)
     auto desc_a = [&](int s) { return ptx::gmma_desc_sw128(ptx::smem_u32(smem_a + s * Cfg::kABytes + wg * 8192), 0); };
     auto desc_b = [&](int s) { return ptx::gmma_desc_sw128(ptx::smem_u32(smem_b + s * Cfg::kBBytes), lbo_b); };
@@ -484,6 +639,19 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmap_a, const __grid_constan
     ptx::wgmma_commit();
     int prev = stage;
     if (++stage == kStages) { stage = 0; phase ^= 1; }
+    if (kRegEpi && p.tma_epi && wt == 0) {
+      // While the MMAs run: once the previous tile's stores have read the staging boxes, load this tile's residual
+      // into them (the layout the output takes there), or just hand them back to the warpgroup.
+      ptx::bulk_wait_read<0>();
+      if (p.residual != nullptr && row0 < p.M) {
+        const int nbox = min(BN / 64, (p.N - col0 + 63) / 64);
+        ptx::mbar_arrive_expect_tx(&stg_ready[wg], (uint32_t)(nbox * Cfg::kBoxBytes));
+        for (int b = 0; b < nbox; b++)
+          ptx::tma_load_2d(stg + b * Cfg::kBoxBytes, &tmap_r, &stg_ready[wg], col0 + 64 * b, row0);
+      } else {
+        ptx::mbar_arrive(&stg_ready[wg]);
+      }
+    }
     for (int kb = 1; kb < p.num_k_blocks; kb++) {
       ptx::mbar_wait(&full[stage], phase);
       ptx::wgmma_fence();
@@ -497,6 +665,23 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmap_a, const __grid_constan
     ptx::wgmma_wait<0>();
     ptx::fence_regs(acc);
     if (wt == 0) ptx::mbar_arrive(&empty[prev]);
+    if (kRegEpi && p.tma_epi) {
+      // ---- register epilogue: finish the accumulators in place into the staging boxes, then one thread stores
+      // them with TMA and the warpgroup goes on to its next tile while the stores drain
+      ptx::mbar_wait(&stg_ready[wg], stg_phase);
+      stg_phase ^= 1;
+      epilogue_regs<BN>(p, acc, ptx::smem_u32(stg), row0, col0, wt);
+      ptx::fence_proxy_async_smem();
+      ptx::named_bar_sync(2 + wg, 128);
+      if (wt == 0 && row0 < p.M) {
+        const bool glu = p.act == ACT_SWIGLU;
+        const int ocol0 = glu ? col0 / 2 : col0, on = glu ? p.N / 2 : p.N;
+        const int nbox = min(glu ? BN / 128 : BN / 64, (on - ocol0 + 63) / 64);
+        for (int b = 0; b < nbox; b++) ptx::tma_store_2d(&tmap_d, stg + b * Cfg::kBoxBytes, ocol0 + 64 * b, row0);
+        ptx::bulk_commit();
+      }
+      continue;
+    }
     // ---- stage the accumulators (fragment layout -> row-major fp32), 128 columns at a time, and run the epilogue
 #pragma unroll
     for (int h = 0; h < BN / kEpiN; h++) {
@@ -515,6 +700,7 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmap_a, const __grid_constan
       epilogue_tile<CONV>(p, acc_s + row * Cfg::kAccLd, m_blk, n_blk * BN + h * kEpiN, split, row, half, lane);
     }
   }
+  if (kRegEpi && p.tma_epi && wt == 0) ptx::bulk_wait<0>();  // the last stores have read shared memory and landed
 }
 
 // ------------------------------------------------------------------------------------------
@@ -563,8 +749,10 @@ static int vec16(const void* base, long long ld, int elem_bytes) {
   return ((uintptr_t)base % 16 == 0) && (ld * elem_bytes % 16 == 0);
 }
 
+// td / tr: the D and residual maps of the register epilogue (p.tma_epi), unused otherwise
 template <bool CONV, int TA, int TB, int BN>
-static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, GemmParams p, cudaStream_t st) {
+static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, GemmParams p, cudaStream_t st,
+                       const CUtensorMap& td = CUtensorMap{}, const CUtensorMap& tr = CUtensorMap{}) {
   p.d_vec = vec16(p.D, p.ldd, p.out_f32 ? 4 : 2);
   p.r_vec = vec16(p.residual, p.ldr, p.residual_f32 ? 4 : 2);
   static bool attr_set = false;
@@ -575,7 +763,7 @@ static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, GemmParams 
   }
   const int total = p.num_m_tiles * p.num_n_tiles * p.k_splits;
   const int grid = total < sm_budget() ? total : sm_budget();
-  kern<<<grid, kGemmThreads, GemmCfg<BN>::kSmemBytes, st>>>(ta, tb, p);
+  kern<<<grid, kGemmThreads, GemmCfg<BN>::kSmemBytes, st>>>(ta, tb, td, tr, p);
   G4R_LAUNCH_CHECK("gemm_bf16_wgmma");
   return G4R_OK;
 }
@@ -812,8 +1000,30 @@ static int gemm_impl(const void* A, long long lda, const void* B, long long ldb,
     int rc = make_tmap(&tb, B, 2, dims, str, box);
     if (rc) return rc;
   }
-  return bn == 256 ? launch_gemm<false, 0, 0, 256>(ta, tb, p, (cudaStream_t)stream)
-                   : launch_gemm<false, 0, 0, 128>(ta, tb, p, (cudaStream_t)stream);
+  // Register epilogue with TMA stores for a 16-bit output with a 16-bit or no residual, when D and the residual
+  // meet TMA's 16-byte base and row-pitch alignment and the row ends on a 16-byte boundary (a TMA store writes
+  // whole 16-byte pieces of a row, so a row of 32006 columns would overwrite its two pad columns); fp32 outputs and
+  // residuals, split-K and the rounded branch keep the staged epilogue too.  Both store / load 64 x 64 boxes (one
+  // consumer warpgroup's rows, 128 B of columns).
+  CUtensorMap td{}, tr{};
+  const int n_out = act == ACT_SWIGLU ? N / 2 : N;
+  p.tma_epi = !out_f32 && k_splits == 1 && !bias_round_bf16 && !residual_f32 && n_out % 8 == 0 &&
+              vec16(D, ldd, 2) && (!residual || vec16(residual, ldr, 2));
+  if (p.tma_epi) {
+    cuuint64_t dims[2] = {(cuuint64_t)n_out, (cuuint64_t)M};
+    cuuint64_t str[1] = {(cuuint64_t)ldd * 2};
+    cuuint32_t box[2] = {64, 64};
+    int rc = make_tmap(&td, D, 2, dims, str, box);
+    if (rc) return rc;
+    if (residual) {
+      cuuint64_t rdims[2] = {(cuuint64_t)N, (cuuint64_t)M};
+      cuuint64_t rstr[1] = {(cuuint64_t)ldr * 2};
+      rc = make_tmap(&tr, residual, 2, rdims, rstr, box);
+      if (rc) return rc;
+    }
+  }
+  return bn == 256 ? launch_gemm<false, 0, 0, 256>(ta, tb, p, (cudaStream_t)stream, td, tr)
+                   : launch_gemm<false, 0, 0, 128>(ta, tb, p, (cudaStream_t)stream, td, tr);
 }
 
 // spatial tiling used by the conv kernel for an H x W map (also tells callers how many GN partial slots exist)
