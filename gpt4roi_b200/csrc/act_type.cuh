@@ -57,6 +57,8 @@
 #define g4r_kv_append_rows_bf16 g4r_kv_append_rows_f16
 #define g4r_decode_attention_rows_bf16 g4r_decode_attention_rows_f16
 #define g4r_attention_cached_bf16 g4r_attention_cached_f16
+#define g4r_kv_append_rows_at_bf16 g4r_kv_append_rows_at_f16
+#define g4r_attention_cached_rows_bf16 g4r_attention_cached_rows_f16
 #define g4r_sample_tokens_bf16 g4r_sample_tokens_f16
 #define g4r_sample_tokens_proc_bf16 g4r_sample_tokens_proc_f16
 #define g4r_sample_tokens_out_bf16 g4r_sample_tokens_out_f16

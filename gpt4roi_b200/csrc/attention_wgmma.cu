@@ -21,6 +21,9 @@
 // The last key block reads cache rows past start[b] + qlen[b], up to the next multiple of 64: those rows must hold
 // finite values (masked scores give p = 0, but 0 * NaN in P.V would still poison the row), so the cache is allocated
 // zero-filled.
+// Through a cache-row table (fa_cached_rows_wgmma, g4r_attention_cached_rows_bf16) chunk row b reads cache row
+// cache_rows[b] of a cache with any number of rows: the K/V tensor maps span all of them, and reads past the last row
+// come back as zeros from the TMA unit.
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -58,10 +61,11 @@ __device__ __forceinline__ void wgmma_pv(float (&o)[D / 2], const uint32_t (&a)[
   else ptx::wgmma_m64n64_rs<1>(o, a, db, 1);
 }
 
-template <int D, bool CAUSAL, bool CACHED = false>
-__global__ void __launch_bounds__(kFaThreads, 1)
-fa_fwd_wgmma(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ CUtensorMap tm_k,
-             const __grid_constant__ CUtensorMap tm_v, const __grid_constant__ FaParams p) {
+// The kernel body, shared by fa_fwd_wgmma and fa_cached_rows_wgmma.  ROWS (CACHED only): chunk row b reads cache row
+// cache_rows[b] of K/V tensor maps that span every row of the cache, instead of row b.
+template <int D, bool CAUSAL, bool CACHED, bool ROWS>
+__device__ __forceinline__ void fa_fwd_body(const CUtensorMap& tm_q, const CUtensorMap& tm_k, const CUtensorMap& tm_v,
+                                            const FaParams& p, const int* cache_rows) {
   constexpr int ATOMS = D / 64;
   constexpr int Q_BYTES = ATOMS * kAtomBytes;     // Q tile: 128 rows x D
   constexpr int KV_ATOM = kFaBN * 128;            // [BN keys][64 bf16]
@@ -97,7 +101,7 @@ fa_fwd_wgmma(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ C
                                   (long long)h * D + (i % (D / 8)) * 8) = make_uint4(0, 0, 0, 0);
       return;
     }
-    kv_base = b * p.kv_L;
+    kv_base = (ROWS ? cache_rows[b] : b) * p.kv_L;
     koff = p.start[b];
     Lk = koff + min(q0 + kFaBM, ql);
     nblk = (Lk + kFaBN - 1) / kFaBN;
@@ -249,6 +253,23 @@ fa_fwd_wgmma(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ C
   }
 }
 
+template <int D, bool CAUSAL, bool CACHED = false>
+__global__ void __launch_bounds__(kFaThreads, 1)
+fa_fwd_wgmma(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ CUtensorMap tm_k,
+             const __grid_constant__ CUtensorMap tm_v, const __grid_constant__ FaParams p) {
+  fa_fwd_body<D, CAUSAL, CACHED, false>(tm_q, tm_k, tm_v, p, nullptr);
+}
+
+// CACHED mode through a cache-row table (g4r_attention_cached_rows_bf16): chunk row b continues the sequence held in
+// cache row cache_rows[b] (device int32 [B]) of a [rows, kv_L, H*D] cache.
+template <int D>
+__global__ void __launch_bounds__(kFaThreads, 1)
+fa_cached_rows_wgmma(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ CUtensorMap tm_k,
+                     const __grid_constant__ CUtensorMap tm_v, const __grid_constant__ FaParams p,
+                     const int* __restrict__ cache_rows) {
+  fa_fwd_body<D, true, true, true>(tm_q, tm_k, tm_v, p, cache_rows);
+}
+
 typedef CUresult (*EncodeTiledFn2)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                    const cuuint64_t*, const cuuint32_t*, const cuuint32_t*,
                                    CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion,
@@ -281,10 +302,13 @@ static int make_tmap_rows(CUtensorMap* m, const void* base, long long cols, long
   return G4R_OK;
 }
 
+template <int D>
+constexpr int fa_smem_bytes() { return (D / 64) * kAtomBytes + 4 * (D / 64) * kFaBN * 128 + 128 + 1024; }  // +1024 alignment slack
+
 template <int D, bool CAUSAL, bool CACHED = false>
 static int launch_fa(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const FaParams& p, int B,
                      cudaStream_t st) {
-  constexpr int smem = (D / 64) * kAtomBytes + 4 * (D / 64) * kFaBN * 128 + 128 + 1024;  // +1024 alignment slack
+  constexpr int smem = fa_smem_bytes<D>();
   static bool set = false;
   auto kern = fa_fwd_wgmma<D, CAUSAL, CACHED>;
   if (!set) {
@@ -294,6 +318,22 @@ static int launch_fa(const CUtensorMap& tq, const CUtensorMap& tk, const CUtenso
   dim3 grid((p.L + kFaBM - 1) / kFaBM, p.H, B);
   kern<<<grid, kFaThreads, smem, st>>>(tq, tk, tv, p);
   G4R_LAUNCH_CHECK("fa_fwd_wgmma");
+  return G4R_OK;
+}
+
+template <int D>
+static int launch_fa_rows(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const FaParams& p,
+                          const int* cache_rows, int B, cudaStream_t st) {
+  constexpr int smem = fa_smem_bytes<D>();
+  static bool set = false;
+  auto kern = fa_cached_rows_wgmma<D>;
+  if (!set) {
+    G4R_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    set = true;
+  }
+  dim3 grid((p.L + kFaBM - 1) / kFaBM, p.H, B);
+  kern<<<grid, kFaThreads, smem, st>>>(tq, tk, tv, p, cache_rows);
+  G4R_LAUNCH_CHECK("fa_cached_rows_wgmma");
   return G4R_OK;
 }
 
@@ -363,4 +403,29 @@ extern "C" int g4r_attention_cached_bf16(const void* q, long long ldq, const voi
   cudaStream_t st = (cudaStream_t)stream;
   if (head_dim == 64) return launch_fa<64, true, true>(tq, tk, tv, p, B, st);
   return launch_fa<128, true, true>(tq, tk, tv, p, B, st);
+}
+
+// g4r_attention_cached_bf16 through a cache-row table (continuous batching: several chunks continue sequences held in
+// rows of the batcher's cache that need not be adjacent): kcache / vcache are [rows, lmax, H*D]; chunk row b's keys and
+// values come from cache row cache_rows[b] (device int32 [B], each < rows).  Same CACHED rules otherwise.
+extern "C" int g4r_attention_cached_rows_bf16(const void* q, long long ldq, const void* kcache, const void* vcache,
+                                              int rows, int lmax, void* out, long long ldo, int B, int H, int Lc,
+                                              int head_dim, float scale, const int* start, const int* qlen,
+                                              const int* cache_rows, void* stream) {
+  G4R_REQUIRE(q && kcache && vcache && out && start && cache_rows && B > 0 && H > 0 && Lc > 0 && lmax > 0 && rows > 0,
+              "attention_cached_rows: bad arguments");
+  G4R_REQUIRE(head_dim == 64 || head_dim == 128, "attention_cached_rows: head_dim %d (64 or 128)", head_dim);
+  G4R_REQUIRE(ldq % 8 == 0 && ldo % 8 == 0, "attention_cached_rows: strides must keep 16-byte alignment");
+  G4R_REQUIRE((((uintptr_t)q | (uintptr_t)kcache | (uintptr_t)vcache | (uintptr_t)out) & 15) == 0,
+              "attention_cached_rows: misaligned pointers");
+  CUtensorMap tq, tk, tv;
+  const long long cols = (long long)H * head_dim;
+  int rc;
+  if ((rc = make_tmap_rows(&tq, q, cols, (long long)B * Lc, ldq, kFaBM))) return rc;
+  if ((rc = make_tmap_rows(&tk, kcache, cols, (long long)rows * lmax, cols, kFaBN))) return rc;
+  if ((rc = make_tmap_rows(&tv, vcache, cols, (long long)rows * lmax, cols, kFaBN))) return rc;
+  FaParams p{(__nv_bfloat16*)out, ldo, (long long)Lc * ldo, Lc, H, scale, nullptr, nullptr, lmax, start, qlen};
+  cudaStream_t st = (cudaStream_t)stream;
+  if (head_dim == 64) return launch_fa_rows<64>(tq, tk, tv, p, cache_rows, B, st);
+  return launch_fa_rows<128>(tq, tk, tv, p, cache_rows, B, st);
 }

@@ -33,6 +33,29 @@ kv_append_bf16(const __nv_bfloat16* __restrict__ qkv, long long ld, __nv_bfloat1
   }
 }
 
+// rows [B*Ln, 3*HD] packed (q|k|v) -> caches [rows, Lmax, HD] through a cache-row table: chunk row b's first qlen[b]
+// rows go to cache row cache_rows[b] at positions pos_rows[b] .. pos_rows[b]+qlen[b]-1; its padding rows are not
+// written, and no write leaves the row (positions >= Lmax are dropped; the caller checks pos_rows[b] + qlen[b] <= Lmax)
+__global__ void __launch_bounds__(256)
+kv_append_rows_at_bf16(const __nv_bfloat16* __restrict__ qkv, long long ld, __nv_bfloat16* __restrict__ kc,
+                       __nv_bfloat16* __restrict__ vc, int B, int Ln, const int* __restrict__ pos_rows,
+                       const int* __restrict__ cache_rows, const int* __restrict__ qlen, int Lmax, int HD) {
+  const int nvec = HD >> 3;
+  const long long total = (long long)B * Ln * nvec * 2;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
+       i += (long long)gridDim.x * blockDim.x) {
+    const int v = (int)(i % nvec);
+    const int which = (int)((i / nvec) & 1);  // 0 = k, 1 = v
+    const long long r = i / (2LL * nvec);     // row in [0, B*Ln)
+    const int t = (int)(r % Ln), b = (int)(r / Ln);
+    const int pos = pos_rows[b] + t;
+    if (t >= qlen[b] || pos >= Lmax) continue;
+    const uint4 val = *reinterpret_cast<const uint4*>(qkv + r * ld + (long long)(1 + which) * HD + v * 8);
+    __nv_bfloat16* dst = (which ? vc : kc) + ((long long)cache_rows[b] * Lmax + pos) * HD + v * 8;
+    *reinterpret_cast<uint4*>(dst) = val;
+  }
+}
+
 // Single-query attention over the KV cache: out = softmax(q . K^T * scale) V for the first kv_len
 // cached positions.  Grid (H, B, S) with a thread-block cluster of S CTAs along z: each CTA of the
 // cluster owns a contiguous slice of the keys (split-KV), and the softmax statistics and the partial
@@ -401,6 +424,22 @@ extern "C" int g4r_kv_append_rows_bf16(const void* qkv, long long ld, void* kcac
   G4R_REQUIRE(qkv && kcache && vcache && pos_rows && B > 0 && Ln > 0 && Ln <= Lmax && HD % 8 == 0 && ld % 8 == 0,
               "kv_append_rows: bad arguments (Ln=%d Lmax=%d)", Ln, Lmax);
   return launch_kv_append(qkv, ld, kcache, vcache, B, Ln, 0, nullptr, pos_rows, Lmax, HD, (cudaStream_t)stream);
+}
+
+extern "C" int g4r_kv_append_rows_at_bf16(const void* qkv, long long ld, void* kcache, void* vcache, int B, int Ln,
+                                          const int* pos_rows, const int* cache_rows, const int* qlen, int Lmax, int HD,
+                                          void* stream) {
+  G4R_REQUIRE(qkv && kcache && vcache && pos_rows && cache_rows && qlen && B > 0 && Ln > 0 && Ln <= Lmax &&
+              HD % 8 == 0 && ld % 8 == 0, "kv_append_rows_at: bad arguments (Ln=%d Lmax=%d)", Ln, Lmax);
+  const long long total = (long long)B * Ln * (HD / 8) * 2;
+  long long grid = (total + 255) / 256;
+  const long long cap = (long long)num_sms() * 16;
+  if (grid > cap) grid = cap;
+  kv_append_rows_at_bf16<<<(unsigned)grid, 256, 0, (cudaStream_t)stream>>>(
+      (const __nv_bfloat16*)qkv, ld, (__nv_bfloat16*)kcache, (__nv_bfloat16*)vcache, B, Ln, pos_rows, cache_rows, qlen,
+      Lmax, HD);
+  G4R_LAUNCH_CHECK("kv_append_rows_at");
+  return G4R_OK;
 }
 
 template <int D, bool BEAM>

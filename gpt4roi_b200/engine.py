@@ -277,17 +277,32 @@ class PrefillEngine:
         hidden states [B, L, hidden] instead of logits (LlamaModel.forward's last_hidden_state).
         start: device int32 [B] -- the L rows of each sample continue the sequence held in `cache`: they sit at
         positions start[b].. (seqlens: each sample's valid rows), are appended there and attend over the cached prefix
-        too (kernels.attention_cached; head_dim 128)."""
+        too (kernels.attention_cached; head_dim 128).  On a row view (cache.rows) the rows are those of the larger cache
+        the table names, and only each sample's valid rows are appended."""
         c = self.cfg
         x = embeds.view(B * L, c.hidden)
-        cos, sin = self._rope(L) if start is None else self._rope_span(cache.max_len)
+        if start is None:
+            cos, sin = self._rope(L)
+        else:
+            # the fused QKV-RoPE epilogue rotates every chunk row, padding included, at start[b] + t (t < L): a cache that
+            # grows covers those positions; a row view never grows, so its table is sized by the last position touched
+            n = cache.max_len if cache.rows is None else max(cache.max_len, int(start.max()) + L)
+            cos, sin = self._rope_span(n)
         scale = c.head_dim ** -0.5
         # fp32 residual stream: the first o_proj epilogue widens it (bf16 residual in, fp32 out); every branch output
         # is rounded to bf16 before the fp32 add, as a bf16 nn.Linear output added to an fp32 stream under autocast
         f32 = dict(out_dtype=torch.float32, round_branch=True) if c.llama_stream == 'fp32' else {}
+        rows = cache.rows if start is not None else None
+        if rows is not None:   # a row view of a larger cache: only each row's valid chunk rows are appended
+            qlen = seqlens if seqlens is not None else torch.full((B,), L, dtype=torch.int32, device=self.dev)
         for li, w in enumerate(self.layers):
             h = kernels.rmsnorm(x, w['ln_in'], c.rms_eps)
-            if start is not None:
+            if rows is not None:
+                qkv = dense.qkv_rope(h, w['wqkv'], cos, sin, L, 2 * c.hidden, pos_rows=start)
+                kernels.kv_append(qkv, cache.k[li], cache.v[li], B, L, 0, pos_rows=start, cache_rows=rows, qlen=qlen)
+                a = kernels.attention_cached(qkv, cache.k[li], cache.v[li], B, c.n_heads, c.head_dim, L, scale, start,
+                                             qlen, cache_rows=rows)
+            elif start is not None:
                 qkv = dense.qkv_rope(h, w['wqkv'], cos, sin, L, 2 * c.hidden, pos_rows=start)
                 kernels.kv_append(qkv, cache.k[li], cache.v[li], B, L, 0, pos_rows=start)
                 a = kernels.attention_cached(qkv, cache.k[li], cache.v[li], B, c.n_heads, c.head_dim, L, scale, start,
@@ -411,7 +426,8 @@ class PrefillEngine:
         cached), whose region tokens come from a ViT + fuse rerun on `images` (only when the chunk holds any).
         Returns logits [B, 1, V] at each row's last chunk token (last_only=False: [B, Lc, V] at every chunk position);
         the cache then holds prefix + chunk and records them.  It grows (zero-filled) when a row's start plus Lc exceeds
-        its length, so a CUDA graph captured on it must be rebuilt afterwards."""
+        its length, so a CUDA graph captured on it must be rebuilt afterwards.  A row view (cache.rows: rows of a larger
+        cache, the continuous batcher's) never grows: each row appends only its valid tokens, which must fit in max_len."""
         c = self.cfg
         if c.head_dim != 128:
             raise NotImplementedError('continuing a cached sequence needs the fused-RoPE QKV GEMM (head_dim 128)')
@@ -423,7 +439,11 @@ class PrefillEngine:
         qlen = _seqlens(lens, Lc)
         start = cache.row_lens().clone()
         start_h = start.cpu()
-        cache.grow(int(start_h.max()) + Lc)   # every row appends all Lc chunk rows, its padding included
+        if cache.rows is None:
+            cache.grow(int(start_h.max()) + Lc)   # every row appends all Lc chunk rows, its padding included
+        elif bool((start_h + lens.cpu() > cache.max_len).any()):
+            raise ValueError('extend: a row view of a larger cache cannot grow: start + chunk length %s exceed max_len %d'
+                             % ((start_h + lens.cpu()).tolist(), cache.max_len))
         plan = self.plan_boxes(bboxes)
         taps = None
         if plan is not None and plan['K'] > 0 and bool((ids == c.bbox_token).any()):
@@ -442,7 +462,11 @@ class PrefillEngine:
             new = _row_boxes(bboxes, b, host=True)
             new = torch.zeros(0, 4) if new is None else new
             boxes.append(torch.cat([old[:n_old], new], 0))
-        cache.record_ids(ids, start)
+        if cache.rows is None:
+            cache.record_ids(ids, start)
+        else:   # the padding was not appended, and may reach past max_len
+            for b, n in enumerate(lens.tolist()):
+                cache.ids[b, int(start_h[b]):int(start_h[b]) + n] = ids[b, :n]
         cache.lens = (start + valid).to(torch.int32)
         cache.length = int(cache.lens.max())
         if images is not None:
@@ -465,11 +489,9 @@ class PrefillEngine:
         cache.grow(L + new_tokens)
         reuse = cache.reusable(input_ids, images, bboxes, attention_mask)
         ids_h, lens_h = ids.cpu(), lens.cpu()
-        image_tok = (ids_h == c.im_patch_token) | (ids_h == c.im_start_token) | (ids_h == c.im_end_token)
         covered = c.head_dim == 128
         for b in range(B):
-            span = image_tok[b, :int(lens_h[b])].nonzero()
-            covered = covered and (len(span) == 0 or int(span.max()) < int(reuse[b]))
+            covered = covered and covers_image_span(c, ids_h[b, :int(lens_h[b])], int(reuse[b]))
         if not covered:
             images = None if images is None else images.to(self.dev, self.dt).contiguous()
             logits = self.forward_device(ids, images, self.plan_boxes(bboxes), validate=True, last_only=True,
@@ -490,6 +512,39 @@ class PrefillEngine:
         cache.lens = reuse.to(self.dev, torch.int32)
         cache.length = int(reuse.max())
         return self.extend(cache, tail, images, tail_boxes, attention_mask=mask)
+
+
+def covers_image_span(cfg, ids, p):
+    """Whether a kept prefix of p tokens of the prompt `ids` (host int64 [L]) holds all its image tokens: a later chunk
+    (extend) takes no image tokens, so a prefix is reusable only when this holds."""
+    span = ((ids == cfg.im_patch_token) | (ids == cfg.im_start_token) | (ids == cfg.im_end_token)).nonzero()
+    return len(span) == 0 or int(span.max()) < p
+
+
+def same_image(held, image):
+    """Whether K/V computed from the image `held` ([3, S, S], None: text-only) can serve a prompt on `image` (the same
+    image, compared in held's device and dtype; or both None)."""
+    if held is None or image is None:
+        return held is None and image is None
+    return torch.equal(held, image.to(held.device, held.dtype))
+
+
+def reusable_prefix(cfg, row, rec, held, old_boxes, new_boxes):
+    """KVCache.reusable's rule for one row: how many leading tokens of `row` (host int64 [n], the new prompt) a cache row
+    holding the ids `rec` (host int64, at least `held` entries) at its first `held` positions, computed with the boxes
+    old_boxes (host fp32 [K, 4] or None) for its <bbox> tokens, can keep for a prompt whose boxes are new_boxes: the
+    longest common prefix, cut at the first <bbox> whose box differs, and at most n - 1 (the image is checked by the
+    caller)."""
+    n = row.shape[0]
+    m = min(n - 1, int(held))
+    diff = (row[:m] != rec[:m]).nonzero()
+    p = int(diff[0]) if len(diff) else m
+    for k, t in enumerate((row[:p] == cfg.bbox_token).nonzero().flatten().tolist()):
+        if old_boxes is None or new_boxes is None or k >= old_boxes.shape[0] or k >= new_boxes.shape[0] \
+                or not torch.equal(old_boxes[k], new_boxes[k]):
+            p = t
+            break
+    return max(p, 0)
 
 
 def _row_boxes(bboxes, b, host=False):
@@ -565,11 +620,14 @@ class KVCache:
     each row's boxes (host fp32 [K, 4] or None) for its <bbox> tokens.  Until a writer records the images and boxes
     (`source_known`), nothing is reusable.
     The K/V tensors are zero-filled, and grow() zero-fills the new space: the chunk attention (kernels.attention_cached)
-    reads cache rows past each row's valid length, up to the next multiple of 64, and needs them finite."""
+    reads cache rows past each row's valid length, up to the next multiple of 64, and needs them finite.
+    A row view (`rows`) is a cache whose B rows are rows rows[b] of larger K/V tensors (the continuous batcher's): the
+    chunk prefill (PrefillEngine.extend) reads and appends through that table, and the view cannot grow."""
 
-    def __init__(self, cfg, B, max_len, device, kv=None):
+    def __init__(self, cfg, B, max_len, device, kv=None, rows=None):
         """kv: optional (k, v) lists of per-layer [B, max_len, HD] tensors to use instead of allocating (BeamCache's
-        prompt rows)."""
+        prompt rows).  rows: with kv, a device int32 [B] table -- the kv tensors are [R, max_len, HD] with any R, and
+        row b of this cache is row rows[b] of theirs."""
         hd = cfg.n_heads * cfg.head_dim
         dt = cfg.torch_dtype
         self.cfg = cfg
@@ -578,6 +636,9 @@ class KVCache:
         else:
             self.k = [torch.zeros((B, max_len, hd), dtype=dt, device=device) for _ in range(cfg.n_layers)]
             self.v = [torch.zeros((B, max_len, hd), dtype=dt, device=device) for _ in range(cfg.n_layers)]
+        if rows is not None and (kv is None or rows.dtype != torch.int32 or tuple(rows.shape) != (B,)):
+            raise ValueError('KVCache: rows must be a device int32 [%d] table over given kv tensors' % B)
+        self.rows = rows
         self.ids = torch.full((B, max_len), -1, dtype=torch.int64, device=device)
         self.B, self.max_len, self.length = B, max_len, 0
         self.lens = None
@@ -616,6 +677,8 @@ class KVCache:
         are replaced, so a CUDA graph captured on the old ones must be rebuilt."""
         if max_len <= self.max_len:
             return
+        if self.rows is not None:
+            raise ValueError('a row view of a larger cache cannot grow (max_len %d, %d asked)' % (self.max_len, max_len))
 
         def big(t, fill):
             n = torch.full((t.shape[0], max_len) + tuple(t.shape[2:]), fill, dtype=t.dtype, device=t.device)
@@ -628,9 +691,7 @@ class KVCache:
         self.max_len = max_len
 
     def _same_image(self, b, images):
-        if self.images is None or images is None:
-            return self.images is None and images is None
-        return torch.equal(self.images[b], images[b].to(self.images.device, self.images.dtype))
+        return same_image(None if self.images is None else self.images[b], None if images is None else images[b])
 
     def reusable(self, input_ids, images, bboxes, attention_mask=None):
         """How many leading tokens of each row of a new prompt the cache already holds, as a host int64 [B]: the longest
@@ -647,18 +708,8 @@ class KVCache:
         for b in range(B):
             if not self._same_image(b, images):
                 continue
-            n = int(lens[b])
-            row = ids[b, :n]
-            m = min(n - 1, int(held[b]))
-            diff = (row[:m] != rec[b, :m]).nonzero()
-            p = int(diff[0]) if len(diff) else m
-            old = self.boxes[b]
-            new = _row_boxes(bboxes, b, host=True)
-            for k, t in enumerate((row[:p] == self.cfg.bbox_token).nonzero().flatten().tolist()):
-                if old is None or new is None or k >= old.shape[0] or k >= new.shape[0] or not torch.equal(old[k], new[k]):
-                    p = t
-                    break
-            out[b] = max(p, 0)
+            out[b] = reusable_prefix(self.cfg, ids[b, :int(lens[b])], rec[b], held[b], self.boxes[b],
+                                     _row_boxes(bboxes, b, host=True))
         return out
 
 
@@ -1252,7 +1303,8 @@ class Request:
     """A request of a ContinuousBatcher: `sequences` (host int64 [1, L + n]: the prompt as given, then the n new tokens,
     HF's layout) grows by one token per step while it runs; `done` turns True when it retires -- it emitted its eos id,
     ended a stop string, or has max_new_tokens new tokens -- or when its admission failed: `error` is then the exception,
-    which ContinuousBatcher.step() raised, and the request has no new tokens."""
+    which ContinuousBatcher.step() raised, and the request has no new tokens.  `reused`: how many prompt tokens its
+    admission took from K/V a batcher row already held (ContinuousBatcher(prefix_reuse=True)); 0 for a full prefill."""
 
     def __init__(self, input_ids, images, bboxes, max_new_tokens, greedy, temperature, top_k, top_p, seed, eos_id,
                  streamer):
@@ -1263,10 +1315,26 @@ class Request:
         self.tokens = []
         self.done = False
         self.error = None
+        self.reused = 0
 
     @property
     def sequences(self):
         return torch.cat([self.input_ids.cpu(), torch.tensor(self.tokens, dtype=torch.int64)[None]], 1)
+
+
+def _image_sig(image):
+    """A few hundred strided samples of an image, on the host (None without an image): images whose samples differ differ,
+    so a batcher admission compares each row's image on the device only when the samples agree."""
+    return None if image is None else image.reshape(-1)[::2039].float().cpu()
+
+
+def _held_ids(rec):
+    """The token ids a ContinuousBatcher row record stands for: its ids, then its request's new tokens but the last."""
+    if rec is None:
+        return torch.zeros(0, dtype=torch.int64)
+    if rec['req'] is None:
+        return rec['ids']
+    return torch.cat([rec['ids'], torch.tensor(rec['req'].tokens[:-1], dtype=torch.int64)])
 
 
 class ContinuousBatcher:
@@ -1281,11 +1349,31 @@ class ContinuousBatcher:
     up front and never grown; on CUDA it is one graph (decode step, selection, stop strings), captured once, whose
     device-side state -- the per-row rule arrays, `active`, `finished`, the lengths -- admissions rewrite in place.
     stop_strings: a StopStrings for every request (transformers' stop_strings).  On CPU tensors (the engine's host
-    stand-ins) the steps run eagerly with a greedy host selection."""
+    stand-ins) the steps run eagerly with a greedy host selection.
 
-    def __init__(self, engine, slots, max_len, stop_strings=None):
+    prefix_reuse=True: a request prefills only what no row already holds -- a follow-up turn of a conversation that is
+    sent again whole, or another question on the same image.  The batcher keeps a host record of each row (row_record:
+    the token ids whose K/V it holds, its image and boxes; a row keeps it after its request retires) and admits a
+    request, FIFO as always, where KVCache.reusable's rules find the longest prefix that covers the prompt's image span:
+    in place when a free row holds it; else, when a running row (or one prefilled earlier in the same step) holds a
+    strictly longer one, in a free row into which that prefix's K/V are copied; else by a full prefill.  Free rows are
+    taken never-used first, then least recently retired, so held conversations live as long as they can.  The requests
+    of a step that reuse a prefix are prefilled together by one chunk prefill (PrefillEngine.extend on a row view of
+    the cache).  A reused request's tokens are those of that chunk prefill -- generate(cache=) on the conversation --
+    not those of a full prefill, and may depend on what the row held: the caller opts into that."""
+
+    def __init__(self, engine, slots, max_len, stop_strings=None, prefix_reuse=False):
         if slots < 1 or max_len < 2:
             raise ValueError('ContinuousBatcher needs slots >= 1 and max_len >= 2 (got %d, %d)' % (slots, max_len))
+        if prefix_reuse and engine.cfg.head_dim != 128:
+            raise NotImplementedError('prefix_reuse needs the chunk prefill, which needs head_dim 128 (got %d)'
+                                      % engine.cfg.head_dim)
+        self.prefix_reuse = bool(prefix_reuse)
+        # per row (prefix_reuse): what its K/V were computed from -- dict(ids: the held prefix, host int64, req: the
+        # request whose prompt and tokens follow it or None, images, boxes) or None (never held anything)
+        self.records = [None] * int(slots)
+        self.retired = [0] * int(slots)   # when each row's request retired (a counter): the least recent is taken first
+        self.clock = 0
         self.eng, self.slots, self.max_len = engine, int(slots), int(max_len)
         dev = engine.dev
         S = self.slots
@@ -1393,6 +1481,8 @@ class ContinuousBatcher:
         req.done = True
         self.running[s] = None
         self.active[s] = 0
+        self.clock += 1
+        self.retired[s] = self.clock
         if req.streamer is not None:
             req.streamer.end()
         return req
@@ -1433,6 +1523,9 @@ class ContinuousBatcher:
         admission fails, it is retired with `error` set and the exception propagates; its slot stays idle and the next
         step() carries on with the other requests."""
         done = []
+        if self.prefix_reuse:
+            while self.queue and None in self.running:
+                done += self._admit_round()
         for s in range(self.slots):
             while self.running[s] is None and self.queue:
                 req = self.queue.popleft()
@@ -1457,6 +1550,188 @@ class ContinuousBatcher:
                 r = self._emit(s, rb[s, 0], bool(rb[s, 1]))
                 if r is not None:
                     done.append(r)
+        return done
+
+    # ---------------------------------------------------------------- prefix reuse
+    def row_record(self, s):
+        """The token ids (host int64) whose K/V row s holds: after an admission the prompt, then, while the request runs
+        and after it retires, also every new token but the last (whose K/V are never written)."""
+        return _held_ids(self.records[s])
+
+    def _set_record(self, s, ids, req, images, boxes, sig=None):
+        self.records[s] = dict(ids=ids, req=req, images=images, boxes=boxes,
+                               sig=_image_sig(images) if sig is None else sig)
+
+    def _match(self, rec, ids, images, boxes, sig):
+        """How many leading tokens of the prompt `ids` (host int64 [L]) a row record can give (0: none usable).
+        sig: _image_sig(images), which settles most image mismatches on the host."""
+        if rec is None:
+            return 0
+        held = _held_ids(rec)
+        p = reusable_prefix(self.eng.cfg, ids, held, held.shape[0], rec['boxes'], boxes)
+        # the image last: comparing it waits for the device, and only a usable token prefix needs it
+        if p == 0 or not covers_image_span(self.eng.cfg, ids, p):
+            return 0
+        if sig is not None and rec['sig'] is not None and not torch.equal(sig, rec['sig']):
+            return 0
+        if not same_image(rec['images'], images):
+            return 0
+        return p
+
+    def _free_row(self, free):
+        """The free row a request without an in-place match takes: one that never held anything, else the least
+        recently retired."""
+        fresh = [s for s in free if self.records[s] is None]
+        return fresh[0] if fresh else min(free, key=lambda s: self.retired[s])
+
+    def _plan_round(self):
+        """Pop queued requests while rows are free and plan each against the rows as they will be after the round's full
+        prefills: -> [(req, row, p, donor)] -- p = 0: full prefill; donor None: the row holds the prefix itself."""
+        dev, dt = self.eng.dev, self.eng.dt
+        free = [s for s in range(self.slots) if self.running[s] is None]
+        virtual = list(self.records)
+        plan = []
+        while self.queue and free:
+            req = self.queue.popleft()
+            ids = req.input_ids[0].cpu()
+            images = None if req.images is None else req.images.to(dev, dt)[0]
+            sig = _image_sig(images)
+            boxes = _row_boxes(req.bboxes, 0, host=True)
+            p = {s: self._match(virtual[s], ids, images, boxes, sig) for s in range(self.slots)}
+            pf = max((p[s] for s in free), default=0)
+            pr = max((p[s] for s in range(self.slots) if s not in free), default=0)
+            if pf > 0 and pf >= pr:
+                s = min((s for s in free if p[s] == pf), key=lambda s: self.retired[s])
+                plan.append((req, s, pf, None))
+                n = pf
+            elif pr > pf:
+                donor = next(s for s in range(self.slots) if s not in free and p[s] == pr)
+                s = self._free_row(free)
+                plan.append((req, s, pr, donor))
+                n = pr
+            else:
+                s = self._free_row(free)
+                plan.append((req, s, 0, None))
+                n = ids.shape[0]
+            free.remove(s)
+            # what the row holds once the round's prefills and copies ran: the prompt after a full prefill, the kept
+            # prefix otherwise (the chunk prefill runs last)
+            virtual[s] = dict(ids=ids[:n], req=None, images=images, boxes=boxes, sig=sig)
+        return plan
+
+    def _admit_round(self):
+        """Admit the requests of one round: full prefills (batch 1, as _admit), then the prefix copies, then one chunk
+        prefill over every row that reuses a prefix.  Returns the requests that finished at admission."""
+        plan = self._plan_round()
+        done, error = [], None
+        for i, (req, s, p, donor) in enumerate(plan):
+            if p:
+                continue
+            self.records[s] = None            # the prefill overwrites the row
+            try:
+                r = self._admit(req, s)
+            except Exception as e:
+                req.error, req.done = e, True
+                if req.streamer is not None:
+                    req.streamer.end()
+                # the round's other requests not admitted yet go back to the head of the queue, in order
+                for j in reversed(range(len(plan))):
+                    if j > i or (j < i and plan[j][2]):
+                        self.queue.appendleft(plan[j][0])
+                raise
+            self._set_record(s, req.input_ids[0].cpu(), req, None if req.images is None else
+                             req.images.to(self.eng.dev, self.eng.dt)[0], _row_boxes(req.bboxes, 0, host=True))
+            if r is not None:
+                done.append(r)
+        reuse = [(req, s, p, donor) for req, s, p, donor in plan if p]
+        for req, s, p, donor in reuse:       # truncate each record to its kept prefix, copying it in from the donor
+            src = self.records[s if donor is None else donor]
+            held = self.row_record(s if donor is None else donor)[:p]
+            if donor is not None:
+                for kv in (self.cache.k, self.cache.v):
+                    for t in kv:
+                        t[s, :p].copy_(t[donor, :p])
+            self._set_record(s, held, None, src['images'], src['boxes'], src['sig'])
+        if len(reuse) > 1:
+            try:
+                done += self._extend(reuse)
+                reuse = []
+            except Exception:
+                pass                          # one bad request fails the batch: each one alone, below
+        for one in reuse:
+            try:
+                done += self._extend([one])
+            except Exception as e:
+                req = one[0]
+                req.error, req.done = e, True
+                if req.streamer is not None:
+                    req.streamer.end()
+                error = error or e
+        if error is not None:
+            raise error
+        return done
+
+    def _extend(self, group):
+        """One chunk prefill of the prompts' tails over their rows' held prefixes, then each request's first token."""
+        eng, cfg = self.eng, self.eng.cfg
+        dev = eng.dev
+        k = len(group)
+        slots = [s for _, s, _, _ in group]
+        starts = [p for _, _, p, _ in group]
+        tails = [req.input_ids[0].cpu()[p:] for req, _, p, _ in group]
+        Lc = max(t.shape[0] for t in tails)
+        ids = torch.zeros((k, Lc), dtype=torch.int64)
+        mask = torch.zeros((k, Lc), dtype=torch.int64)
+        tail_boxes, new_box = [], False
+        for i, ((req, s, p, _), t) in enumerate(zip(group, tails)):
+            ids[i, :t.shape[0]], mask[i, :t.shape[0]] = t, 1
+            boxes = _row_boxes(req.bboxes, 0)
+            n_old = int((req.input_ids[0, :p] == cfg.bbox_token).sum())
+            tail_boxes.append(None if boxes is None else boxes[n_old:])
+            new_box = new_box or bool((t == cfg.bbox_token).any())
+        images = None
+        if new_box:   # the tails' region tokens come from a ViT + fuse rerun on the requests' images
+            images = torch.stack([torch.zeros((3, cfg.image_size, cfg.image_size), dtype=eng.dt, device=dev)
+                                  if req.images is None else req.images.to(dev, eng.dt)[0] for req, _, _, _ in group])
+        view = KVCache(cfg, k, self.max_len, dev, kv=(self.cache.k, self.cache.v),
+                       rows=torch.tensor(slots, dtype=torch.int32, device=dev))
+        view.lens = torch.tensor(starts, dtype=torch.int32, device=dev)
+        view.length = max(starts)
+        for (req, s, p, _) in group:          # the rows' device state, as _admit writes it
+            row = slice(s, s + 1)
+            self.cache.lens[row] = p
+            for t, v in ((self.greedy, int(req.greedy)), (self.temperature, req.temperature), (self.top_k, req.top_k),
+                         (self.top_p, req.top_p), (self.seed, req.seed), (self.step_count, 0),
+                         (self.eos_id, req.eos_id), (self.finished, 0), (self.active, 1)):
+                t[row] = v
+            if self.stops is not None:
+                self.stop_state[row] = self.stops.initial_states(req.input_ids, torch.tensor([req.input_ids.shape[1]])
+                                                                 ).to(dev)
+        try:
+            logits = eng.extend(view, ids, images, tail_boxes, attention_mask=mask)
+            first = []
+            for i, (req, s, p, _) in enumerate(group):
+                row = slice(s, s + 1)
+                self._select(logits[i:i + 1], row, None)
+                self.cache.lens[row] = req.input_ids.shape[1]
+                first.append(torch.stack([self.ids[s, 0], self.finished[s].to(torch.int64)]))
+            first = torch.stack(first).tolist()
+        except BaseException:
+            for s in slots:
+                self.active[s] = 0
+            raise
+        done = []
+        for (req, s, p, _), (tok, fin) in zip(group, first):
+            req.reused = p
+            rec = self.records[s]
+            self._set_record(s, req.input_ids[0].cpu(), req, rec['images'], _row_boxes(req.bboxes, 0, host=True),
+                             rec['sig'])
+            if req.streamer is not None:
+                req.streamer.put(req.input_ids.cpu())
+            self.running[s] = req
+            r = self._emit(s, tok, fin)
+            if r is not None:
+                done.append(r)
         return done
 
     def run(self):

@@ -100,14 +100,22 @@ def attention(qkv, B, L, n_heads, head_dim, causal, scale, out=None, seqlens=Non
     return out
 
 
-def attention_cached(qkv, kcache, vcache, B, n_heads, head_dim, Lc, scale, start, qlen=None):
+def attention_cached(qkv, kcache, vcache, B, n_heads, head_dim, Lc, scale, start, qlen=None, cache_rows=None):
     """Chunk attention over the KV cache: qkv packed [B*Lc, 3*HD] (RoPE-rotated at each row's positions), whose k|v were
     already appended to caches [B, Lmax, HD] at start[b]..; start / qlen device int32 [B] (qlen None: all Lc rows valid).
     Query i of row b attends over cache positions 0 .. start[b] + i.  Returns [B*Lc, HD]; rows >= qlen[b] hold finite
-    filler (zeros for 128-row tiles wholly past qlen[b])."""
+    filler (zeros for 128-row tiles wholly past qlen[b]).
+    cache_rows: device int32 [B] -- the caches are [rows, Lmax, HD] (any number of rows) and chunk row b reads cache row
+    cache_rows[b] (g4r_attention_cached_rows_bf16); qlen is then required."""
     act = _bf16(qkv, kcache, vcache)
     hd = n_heads * head_dim
     out = torch.empty((B * Lc, hd), dtype=act, device=qkv.device)
+    if cache_rows is not None:
+        _call('g4r_attention_cached_rows_bf16', qkv.device, _L.ptr(qkv), qkv.stride(0), _L.ptr(kcache), _L.ptr(vcache),
+              kcache.shape[0], kcache.shape[1], _L.ptr(out), out.stride(0), B, n_heads, Lc, head_dim, float(scale),
+              _L.ptr(_L.require_pos_rows(start, B)), _L.ptr(_L.require_pos_rows(qlen, B)),
+              _L.ptr(_L.require_pos_rows(cache_rows, B)), act=act)
+        return out
     _call('g4r_attention_cached_bf16', qkv.device, _L.ptr(qkv), qkv.stride(0), _L.ptr(kcache), _L.ptr(vcache),
           kcache.shape[1], _L.ptr(out), out.stride(0), B, n_heads, Lc, head_dim, float(scale),
           _L.ptr(_L.require_pos_rows(start, B)), None if qlen is None else _L.ptr(_L.require_pos_rows(qlen, B)), act=act)
@@ -389,11 +397,20 @@ def stop_step(ids, table, state, finished):
     return finished
 
 
-def kv_append(qkv, kcache, vcache, B, Ln, pos0, pos_dev=None, pos_rows=None):
+def kv_append(qkv, kcache, vcache, B, Ln, pos0, pos_dev=None, pos_rows=None, cache_rows=None, qlen=None):
     """Copy the k|v parts of packed qkv rows [B*Ln, 3*HD] into caches [B, Lmax, HD] at pos0..pos0+Ln-1.
-    pos_rows: device int32 [B] -- sample b's rows go to pos_rows[b]..pos_rows[b]+Ln-1 instead (pos0 / pos_dev unused)."""
+    pos_rows: device int32 [B] -- sample b's rows go to pos_rows[b]..pos_rows[b]+Ln-1 instead (pos0 / pos_dev unused).
+    cache_rows (with pos_rows and qlen, device int32 [B]): the caches are [rows, Lmax, HD] (any number of rows) and only
+    sample b's first qlen[b] rows are written, to cache row cache_rows[b] at pos_rows[b].. (g4r_kv_append_rows_at_bf16)."""
     HD = kcache.shape[-1]
     act = _bf16(qkv, kcache, vcache)
+    if cache_rows is not None:
+        if pos_rows is None or qlen is None:
+            raise ValueError('kv_append: cache_rows needs pos_rows and qlen')
+        _call('g4r_kv_append_rows_at_bf16', qkv.device, _L.ptr(qkv), qkv.stride(0), _L.ptr(kcache), _L.ptr(vcache), B,
+              Ln, _L.ptr(_L.require_pos_rows(pos_rows, B)), _L.ptr(_L.require_pos_rows(cache_rows, B)),
+              _L.ptr(_L.require_pos_rows(qlen, B)), kcache.shape[1], HD, act=act)
+        return
     if pos_rows is not None:
         _call('g4r_kv_append_rows_bf16', qkv.device, _L.ptr(qkv), qkv.stride(0), _L.ptr(kcache), _L.ptr(vcache), B, Ln,
               _L.ptr(_L.require_pos_rows(pos_rows, B)), kcache.shape[1], HD, act=act)

@@ -58,6 +58,9 @@ SIGNATURES = {
     'g4r_attention_bf16': (_i, [_vp] * 4 + [_ll] * 4 + [_i] * 5 + [_f, _vp, _vp]),
     'g4r_attention_tc_bf16': (_i, [_vp] * 4 + [_ll] * 4 + [_i] * 5 + [_f, _vp, _vp]),
     'g4r_attention_cached_bf16': (_i, [_vp, _ll, _vp, _vp, _i, _vp, _ll, _i, _i, _i, _i, _f, _vp, _vp, _vp]),
+    'g4r_kv_append_rows_at_bf16': (_i, [_vp, _ll, _vp, _vp, _i, _i, _vp, _vp, _vp, _i, _i, _vp]),
+    'g4r_attention_cached_rows_bf16': (_i, [_vp, _ll, _vp, _vp, _i, _i, _vp, _ll, _i, _i, _i, _i, _f, _vp, _vp, _vp,
+                                            _vp]),
     'g4r_layernorm_bf16': (_i, [_vp, _ll, _vp, _vp, _vp, _ll, _i, _i, _f, _vp]),
     'g4r_layernorm_ex': (_i, [_vp, _ll, _i, _vp, _vp, _vp, _ll, _i, _i, _i, _f, _vp]),
     'g4r_cast_f32_bf16': (_i, [_vp, _ll, _ll, _vp, _i, _i, _i, _vp]),
@@ -146,6 +149,8 @@ F16_TWINS = {
     'g4r_kv_append_rows_bf16': 'g4r_kv_append_rows_f16',
     'g4r_decode_attention_rows_bf16': 'g4r_decode_attention_rows_f16',
     'g4r_attention_cached_bf16': 'g4r_attention_cached_f16',
+    'g4r_kv_append_rows_at_bf16': 'g4r_kv_append_rows_at_f16',
+    'g4r_attention_cached_rows_bf16': 'g4r_attention_cached_rows_f16',
     'g4r_sample_tokens_bf16': 'g4r_sample_tokens_f16',
     'g4r_sample_tokens_proc_bf16': 'g4r_sample_tokens_proc_f16',
     'g4r_sample_tokens_out_bf16': 'g4r_sample_tokens_out_f16',

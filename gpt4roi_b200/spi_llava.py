@@ -964,16 +964,19 @@ class SPILlavaMPTForCausalLM(LlamaForCausalLM, _EngineHost):
                            min_new_tokens=procs['min_new_tokens'], length_eos_ids=procs['eos_ids'], **outs)
         return _generate_output(res, outs, pkv) if outs['return_dict_in_generate'] else res
 
-    def continuous_batcher(self, slots=8, max_len=2048, tokenizer=None, stop_strings=None):
+    def continuous_batcher(self, slots=8, max_len=2048, tokenizer=None, stop_strings=None, prefix_reuse=False):
         """A ContinuousBatcher (engine.ContinuousBatcher: requests join and leave the graphed decode step one row at a
         time) on this model's engine, with `slots` rows of up to max_len tokens each.  stop_strings (with tokenizer=;
         resolve_stop_strings, so the model's generation config counts) apply to every request.  Its submit(input_ids,
         images=, bboxes=, max_new_tokens=, **generate_kwargs) resolves each request's sampling rule as the engine loop
-        of generate() does."""
+        of generate() does.  prefix_reuse=True: a request prefills only what no row already holds (a conversation sent
+        again whole each turn, several questions on one image); its tokens are then those of
+        generate(past_key_values=) on the conversation (engine.ContinuousBatcher)."""
         stops = resolve_stop_strings(self, tokenizer, stop_strings)
         eng = self._get_engine(self.device)
         return SeamBatcher(self, ContinuousBatcher(eng, slots, max_len, None if stops is None else
-                                                   stop_strings_from_tokenizer(tokenizer, stops)))
+                                                   stop_strings_from_tokenizer(tokenizer, stops),
+                                                   prefix_reuse=prefix_reuse))
 
     def initialize_vision_tokenizer(self, mm_use_im_start_end, tokenizer, device, tune_mm_mlp_adapter=False,
                                     pretrain_mm_mlp_adapter=None):

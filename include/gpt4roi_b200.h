@@ -280,6 +280,15 @@ int g4r_decode_gemm_rows_bf16(const void* x, long long ldx, const void* W, long 
 /* g4r_kv_append_bf16 with sample b's rows at positions pos_rows[b] .. pos_rows[b]+Ln-1. */
 int g4r_kv_append_rows_bf16(const void* qkv, long long ld, void* kcache, void* vcache,
                             int B, int Ln, const int* pos_rows, int Lmax, int HD, void* stream);
+/* g4r_kv_append_rows_bf16 through a cache-row table (continuous batching with prefix reuse: the chunk prefill of several
+ * admitted requests whose rows of the batcher's cache are not adjacent; transformers' generate(past_key_values=...)
+ * per request, gpt4roi/app.py:242-328 re-submitting the conversation): kcache / vcache are [rows, Lmax, HD]; chunk
+ * row b's first qlen[b] rows go to cache row cache_rows[b] at positions pos_rows[b] .. pos_rows[b]+qlen[b]-1 and its
+ * padding rows are not written.  cache_rows, qlen: device int32 [B].  Caller's contract: cache_rows[b] < rows and
+ * pos_rows[b] + qlen[b] <= Lmax (positions >= Lmax are dropped, never written into the next row). */
+int g4r_kv_append_rows_at_bf16(const void* qkv, long long ld, void* kcache, void* vcache, int B, int Ln,
+                               const int* pos_rows, const int* cache_rows, const int* qlen, int Lmax, int HD,
+                               void* stream);
 /* g4r_decode_attention_bf16 with sample b over its first pos_rows[b] + 1 cached positions; kv_bound (>= every
  * pos_rows[b] + 1, e.g. Lmax in a CUDA graph) sizes the split-KV factor and the shared-memory score buffer. */
 int g4r_decode_attention_rows_bf16(const void* q, long long ldq, const void* kcache, const void* vcache,
@@ -486,6 +495,14 @@ int g4r_attention_tc_bf16(const void* q, const void* k, const void* v, void* out
 int g4r_attention_cached_bf16(const void* q, long long ldq, const void* kcache, const void* vcache, int lmax,
                               void* out, long long ldo, int B, int H, int Lc, int head_dim, float scale,
                               const int* start, const int* qlen, void* stream);
+/* g4r_attention_cached_bf16 through a cache-row table (the same reuse as g4r_kv_append_rows_at_bf16): kcache / vcache
+ * are [rows, lmax, H*head_dim] and chunk row b attends over cache row cache_rows[b] (device int32 [B], each < rows)
+ * instead of row b.  The same CACHED rules: key blocks aligned to position 0, 128-row tiles wholly past qlen[b] zeroed,
+ * the last key block reading cache row positions up to the next multiple of 64 (finite values required; past the last
+ * cache row they read as zeros). */
+int g4r_attention_cached_rows_bf16(const void* q, long long ldq, const void* kcache, const void* vcache, int rows,
+                                   int lmax, void* out, long long ldo, int B, int H, int Lc, int head_dim, float scale,
+                                   const int* start, const int* qlen, const int* cache_rows, void* stream);
 
 /* ---- HBM-bound glue (csrc/elementwise.cu); bf16 rows, fp32 math ------------- */
 /* nn.LayerNorm over the last dim (CLIP layer norms; gpt4roi/models/layers.py:263,266). */
@@ -784,6 +801,12 @@ int g4r_decode_attention_rows_f16(const void* q, long long ldq, const void* kcac
 int g4r_attention_cached_f16(const void* q, long long ldq, const void* kcache, const void* vcache, int lmax,
                              void* out, long long ldo, int B, int H, int Lc, int head_dim, float scale,
                              const int* start, const int* qlen, void* stream);
+int g4r_kv_append_rows_at_f16(const void* qkv, long long ld, void* kcache, void* vcache, int B, int Ln,
+                              const int* pos_rows, const int* cache_rows, const int* qlen, int Lmax, int HD,
+                              void* stream);
+int g4r_attention_cached_rows_f16(const void* q, long long ldq, const void* kcache, const void* vcache, int rows,
+                                  int lmax, void* out, long long ldo, int B, int H, int Lc, int head_dim, float scale,
+                                  const int* start, const int* qlen, const int* cache_rows, void* stream);
 int g4r_sample_tokens_f16(const void* logits, long long ld, int B, int V, float temperature, int top_k, float top_p,
                           int greedy, unsigned long long seed, const long long* rng_step, int eos_id, int pad_id,
                           int* finished, long long* out_ids, void* stream);
