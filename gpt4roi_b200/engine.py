@@ -690,6 +690,19 @@ class KVCache:
         self.ids = big(self.ids, -1)
         self.max_len = max_len
 
+    def crop(self, n):
+        """Keep the first n positions (transformers' DynamicCache.crop, which assisted decoding calls after every verify
+        step): lengths only -- the K/V past n stay in memory but become unreachable, later writes overwrite them, and
+        their recorded ids are cleared so that reusable() stops at n.  The tensors are not replaced, so a CUDA graph
+        captured on the cache stays valid."""
+        n = max(int(n), 0)
+        if n >= self.length and self.lens is None:
+            return
+        self.length = min(self.length, n)
+        if self.lens is not None:
+            self.lens.clamp_(max=n)
+        self.ids[:, n:] = -1
+
     def _same_image(self, b, images):
         return same_image(None if self.images is None else self.images[b], None if images is None else images[b])
 
@@ -775,6 +788,41 @@ def _decode_step_chain(self, token_ids, cache, pos_dev):
     buf = torch.empty((B, self.vocab_pad), dtype=self.dt, device=self.dev)
     dense.linear(x, self.lm_head, out=buf[:, :c.vocab])
     return buf[:, None, :c.vocab]
+
+
+def _verify_step(self, token_ids, cache, st):
+    """The verify step of prompt-lookup decoding: the decode chain over the M <= st.k + 1 rows token_ids (int64 [M, 1])
+    of one sequence held in cache row 0, row i at position st.pos[i] (device int32, consecutive from st.base[0]).
+    Each row's K/V is written at its position (qkv_rope with the per-sample base, then kv_append: the rows are one
+    sample of M rows), and row i attends over positions 0..st.pos[i] (decode_attention_beam with the all-zero ancestry
+    table st.anc[:M] (int32 [>= M, max_len]): a causal M-query attention over cache row 0).  Returns logits [M, 1, V].  M <= 16 runs
+    the weight-streaming decode GEMMs, a larger M the tiled ones.  Every position is read from device memory, so the
+    step can be captured (LookupDecode)."""
+    prev = lib.set_pdl(True)
+    try:
+        c = self.cfg
+        M = token_ids.shape[0]
+        x = splice_region_tokens(token_ids, self.embed, None, None, 0, c.im_patch_token, c.im_start_token,
+                                 c.im_end_token, c.bbox_token, validate=False).view(M, c.hidden)
+        cos, sin = self._rope_span(cache.max_len)
+        scale = c.head_dim ** -0.5
+        swiglu_gemm = dense.decode_gemm if M <= 16 and c.hidden % 256 == 0 else dense.linear
+        for li, w in enumerate(self.layers):
+            h = kernels.rmsnorm(x, w['ln_in'], c.rms_eps)
+            qkv = dense.qkv_rope(h, w['wqkv'], cos, sin, M, 2 * c.hidden, pos_rows=st.base)
+            kernels.kv_append(qkv, cache.k[li], cache.v[li], 1, M, 0, pos_rows=st.base)
+            a = kernels.decode_attention_beam(qkv, cache.k[li], cache.v[li], M, c.n_heads, c.head_dim, cache.max_len,
+                                              scale, st.pos[:M], st.anc[:M])
+            x = dense.linear(a, w['wo'], residual=x)
+            h = kernels.rmsnorm(x, w['ln_post'], c.rms_eps)
+            f = swiglu_gemm(h, w['wgu'], act='swiglu')
+            x = dense.linear(f, w['wdown'], residual=x)
+        x = kernels.rmsnorm(x, self.norm_w, c.rms_eps)
+        buf = torch.empty((M, self.vocab_pad), dtype=self.dt, device=self.dev)
+        dense.linear(x, self.lm_head, out=buf[:, :c.vocab])
+        return buf[:, None, :c.vocab]
+    finally:
+        lib.set_pdl(prev)
 
 
 def _decode_attention(cache, li, qkv, kv_len, scale, pos_dev, rows, anc):
@@ -1080,7 +1128,8 @@ def _generate(self, input_ids, images, bboxes, max_new_tokens=32, do_sample=Fals
               pad_token_id=None, cache=None, top_k=None, top_p=None, num_beams=1, length_penalty=1.0,
               early_stopping=False, num_return_sequences=1, stop_strings=None, repetition_penalty=1.0,
               no_repeat_ngram_size=0, min_length=0, min_new_tokens=0, length_eos_ids=None, output_scores=False,
-              output_logits=False, return_dict_in_generate=False):
+              output_logits=False, return_dict_in_generate=False, prompt_lookup_num_tokens=None,
+              max_matching_ngram_size=None, streamer=None):
     """Prefill + greedy / sampled decode (gpt4roi/app.py:286-300 calls
     model.generate(input_ids, images=..., do_sample=True, temperature=0.2, max_new_tokens=1024,
     stopping_criteria=[...]) with the boxes bound to forward).  Returns ids [B, L + new]: the prompt as given,
@@ -1131,7 +1180,22 @@ def _generate(self, input_ids, images, bboxes, max_new_tokens=32, do_sample=Fals
     [max_new_tokens, R, V], allocated up front: 4 * V bytes (128 KB at V = 32 000) per row, token and output, where HF
     grows its tuples as it goes -- the same peak at full length.  Beam search adds sequences_scores (the returned
     beams' final scores) and beam_indices (int32 [B * num_return_sequences, n], b * num_beams + beam, -1 past a beam's
-    end); its scores are each beam row's log_softmax before the running score is added, as HF stores them."""
+    end); its scores are each beam row's log_softmax before the running score is added, as HF stores them.
+    prompt_lookup_num_tokens = k (with max_matching_ngram_size, default 2): prompt-lookup decoding, transformers'
+    PromptLookupCandidateGenerator and _assisted_decoding -- each step drafts up to k ids by copying what followed the
+    leftmost earlier occurrence of the sequence's last n-gram, and verifies them in one decode chain over k + 1 rows
+    (LookupDecode, one CUDA graph); a step without a draft runs over one row.  It runs for batch 1 with greedy or
+    temperature / top-k / top-p selection, eos_token_id an id or a list, a conversation cache and host stopping_criteria
+    (called on the candidate sequence before each step and on the sequence after it, as HF calls them; streamer:
+    transformers' BaseStreamer contract -- the prompt, then the first token, then each step's accepted tokens); token j
+    is drawn with Philox counter j, so with equal logits the tokens are those of the plain loop with the same seed.
+    Stated deviations from HF's assisted loop: where HF's acceptance would run past max_new_tokens the loop stops
+    there; when sampling, HF's PromptLookupCandidateGenerator also cuts a draft at the first id its warpers mask on
+    constant logits (top_k, top_p < 1: a fixed set of ids), which the draft rule here does not -- the tokens' distribution
+    is the plain loop's either way, but drafts and accept counts can differ from use_hf_loop=True's.  After the call,
+    self.lookup_accepted (a diagnostic, overwritten by the next lookup call) lists the tokens each verify step appended.
+    Every other call (batch > 1, a padded mask, logits processors, stop_strings, outputs, beams,
+    num_return_sequences > 1) ignores the option and runs the plain loop."""
     if length_eos_ids is None:
         length_eos_ids = [] if eos_token_id is None else (
             list(eos_token_id) if isinstance(eos_token_id, (list, tuple)) else [eos_token_id])
@@ -1156,6 +1220,14 @@ def _generate(self, input_ids, images, bboxes, max_new_tokens=32, do_sample=Fals
     B, L = input_ids.shape
     N = int(num_return_sequences)
     greedy = not (do_sample and temperature > 0)
+    if prompt_lookup_num_tokens and B == 1 and N == 1 and neutral and stop_strings is None \
+            and not (output_scores or output_logits or return_dict_in_generate) and self.cfg.head_dim == 128 \
+            and max_new_tokens >= 1 and (attention_mask is None or bool(attention_mask.bool().all())):
+        eos = [] if eos_token_id is None else [int(e) for e in (
+            eos_token_id if isinstance(eos_token_id, (list, tuple)) else [eos_token_id])]
+        return _generate_lookup(self, input_ids, images, bboxes, max_new_tokens, int(prompt_lookup_num_tokens),
+                                int(max_matching_ngram_size or 2), greedy, temperature, top_k, top_p, generator, eos,
+                                stopping_criteria, cache, use_graph, streamer)
     if N != 1:
         if N < 1:
             raise ValueError('num_return_sequences must be >= 1, got %d' % N)
@@ -1297,6 +1369,262 @@ class GraphedDecode:
         if self.sampler is not None:
             self.sampler.advance()
         return self.logits
+
+
+def lookup_candidates(seq, num_output_tokens, max_ngram=2, max_length=None, eos_ids=()):
+    """transformers' PromptLookupCandidateGenerator.get_candidates restated on a host list of ids (one sequence; no
+    logits processors): the draft ids for the next verify step, [] for none.  For n-gram sizes min(max_ngram,
+    len - 1) down to 1, the leftmost window equal to the sequence's last n-gram whose continuation is not empty wins;
+    the draft is up to num_output_tokens ids after it (bounded by the sequence's length and max_length), cut before its
+    first eos id.  No draft when max_length == len + 1.  csrc/lookup.cu computes the same on the device."""
+    seq = [int(t) for t in seq]
+    n = len(seq)
+    max_length = n + num_output_tokens + 1 if max_length is None else int(max_length)
+    if max_length == n + 1:
+        return []
+    eos = {int(e) for e in eos_ids}
+    for g in range(min(max_ngram, n - 1), 0, -1):
+        tail = seq[n - g:]
+        for idx in range(n - g + 1):
+            if seq[idx:idx + g] != tail:
+                continue
+            start = idx + g
+            end = min(start + num_output_tokens, n, max_length)
+            if start < end:
+                draft = seq[start:end]
+                cut = next((i for i, t in enumerate(draft) if t in eos), len(draft))
+                return draft[:cut]      # an eos first: no draft, and the search ends there, as HF's does
+    return []
+
+
+def lookup_accept(drafts, selected, length, max_length, done_candidate=False, eos_ids=()):
+    """The acceptance of transformers' _assisted_decoding (its branch without candidate logits), restated: drafts (d ids)
+    were verified after a sequence of `length` ids and `selected` (d + 1 ids) are the tokens chosen at the d + 1
+    positions.  n = the count of leading drafts equal to the selected tokens; when the candidate sequence is done
+    (done_candidate: the stopping criteria on it, or length + d >= max_length) and all d matched, n -= 1.  Returns (the
+    appended tokens -- the first n + 1 selected, at most max_length - length of them --, whether one is an eos id)."""
+    d = len(drafts)
+    n = 0
+    while n < d and int(drafts[n]) == int(selected[n]):
+        n += 1
+    if (done_candidate or length + d >= max_length) and d > 0 and n == d:
+        n -= 1
+    new = [int(t) for t in selected[:min(n + 1, max_length - length)]]
+    eos = {int(e) for e in eos_ids}
+    return new, any(t in eos for t in new)
+
+
+class LookupDecode:
+    """Prompt-lookup decoding of one sequence (transformers' generate(prompt_lookup_num_tokens=k), batch 1): each step
+    verifies the last accepted token and up to k drafted ids in one decode chain over M = k + 1 rows
+    (PrefillEngine.verify_step), selects a token per row (kernels.sample_tokens_rows, row i with Philox counter j0 + i
+    where j0 is the index of the first new token it decides, so new token j is always drawn with counter j as the plain
+    batch-1 loop draws it), then accepts and drafts the next step on the device (kernels.lookup_step).  A step with no
+    draft (no window matched) runs the same over the one row of the last token, a plain one-token step: the host knows
+    the draft count from the previous readback.  On CUDA each of the two is one graph, captured once (`graph`, M rows;
+    `graph1`, one row); the host replays one per step and reads `readback` once per step.
+    hist: int64 [1, >= prompt_len + max_new_tokens], the prompt then the accepted tokens (the loop's output buffer).
+    The cache must hold prompt_len + max_new_tokens + k positions: rows past the accepted length write K/V there, which
+    nothing reads and later steps overwrite.  On CPU tensors (the loop's host tests) the engine's verify_step is a
+    stand-in and the selection (greedy only), acceptance and draft run as their host restatements."""
+
+    def __init__(self, engine, cache, hist, prompt_len, max_new_tokens, k, max_ngram=2, eos_ids=(), greedy=True,
+                 temperature=1.0, top_k=None, top_p=None, seed=0, use_graph=True):
+        if int(k) < 1 or int(max_ngram) < 1:
+            raise ValueError('prompt lookup needs prompt_lookup_num_tokens >= 1 and max_matching_ngram_size >= 1 (got '
+                             '%r, %r)' % (k, max_ngram))
+        self.eng, self.cache = engine, cache
+        self.k, self.max_ngram = int(k), int(max_ngram)
+        self.prompt_len, self.max_length = int(prompt_len), int(prompt_len) + int(max_new_tokens)
+        self.hist = hist.view(-1)
+        dev = self.hist.device
+        M = self.k + 1
+        self.eos_list = [int(e) for e in eos_ids]
+        self.eos = torch.tensor(self.eos_list, dtype=torch.int32, device=dev) if self.eos_list else None
+        z = dict(device=dev)
+        self.ids = torch.zeros((M, 1), dtype=torch.int64, **z)        # the verify step's input
+        self.sel = torch.zeros(M, dtype=torch.int64, **z)             # its selected tokens
+        self.state = torch.zeros(5, dtype=torch.int32, **z)           # len, d, finished, appended, host_done
+        self.base = torch.zeros(1, dtype=torch.int32, **z)
+        self.pos = torch.zeros(M, dtype=torch.int32, **z)
+        self.step = torch.zeros(M, dtype=torch.int64, **z)
+        self.readback = torch.zeros(4 + M + self.k, dtype=torch.int64, **z)
+        self.greedy = bool(greedy)
+        self.rule = [torch.full((M,), v, dtype=dt, **z) for v, dt in (
+            (int(self.greedy), torch.int32), (float(temperature), torch.float32), (int(top_k or 0), torch.int32),
+            (1.0 if top_p is None else float(top_p), torch.float32), (int(seed), torch.int64))]
+        self.no_eos = torch.full((M,), -1, dtype=torch.int32, **z)    # eos is the lookup kernel's business
+        self.active = torch.ones(M, dtype=torch.int32, **z)
+        self.finished = torch.zeros(M, dtype=torch.int32, **z)        # scratch of the selection
+        self.anc = torch.zeros((M, cache.max_len), dtype=torch.int32, **z) if dev.type == 'cuda' else None
+        self.accepted = []                                            # tokens appended by each verify step
+        self.use_graph = bool(use_graph) and dev.type == 'cuda'
+        self.graph = self.graph1 = None
+        self.rb = None                                                # the last readback, on the host
+
+    def _capture(self, rows):
+        """Capture the verify step over `rows` rows once the first draft is in place: the warm-up runs it at the first
+        step's positions (whose K/V that step rewrites), and its other writes are undone."""
+        mutable = [self.ids, self.sel, self.state, self.base, self.pos, self.step, self.readback, self.finished,
+                   self.hist]
+        saved = [t.clone() for t in mutable]
+        graph, _ = _capture(self.hist.device, lambda: [self._body(rows) for _ in range(2)], lambda: self._body(rows))
+        for t, s in zip(mutable, saved):
+            t.copy_(s)
+        return graph
+
+    def _select(self, logits, rows):
+        """Select rows [0, rows) of logits [rows, 1, V] into self.sel[:rows]."""
+        if logits.is_cuda:
+            g, t, k, p, s = (v[:rows] for v in self.rule)
+            kernels.sample_tokens_rows(logits, self.sel[:rows], g, t, k, p, s, self.step[:rows], self.no_eos[:rows],
+                                       self.active[:rows], self.finished[:rows])
+            return
+        if not self.greedy:
+            raise RuntimeError('token sampling runs on the CUDA device only (csrc/sample.cu): logits are on %s'
+                               % logits.device)
+        self.sel[:rows] = logits.reshape(rows, -1).argmax(-1)
+
+    def _body(self, rows):
+        logits = self.eng.verify_step(self.ids[:rows], self.cache, self)
+        self._select(logits, rows)
+        if logits.is_cuda:
+            kernels.lookup_step(self, self.sel)
+        else:
+            self._host_accept()
+        return logits
+
+    # host restatement of csrc/lookup.cu (CPU tensors)
+    def _host_accept(self):
+        ln, d, done = int(self.state[0]), int(self.state[1]), bool(self.state[4])
+        new, fin = lookup_accept(self.ids[1:1 + d, 0].tolist(), self.sel.tolist(), ln, self.max_length, done,
+                                 self.eos_list)
+        self.hist[ln:ln + len(new)] = torch.tensor(new, dtype=torch.int64)
+        self.readback[4:4 + len(new)] = torch.tensor(new, dtype=torch.int64)
+        self.readback[0] = len(new)
+        self.state[0], self.state[3] = ln + len(new), len(new)
+        self.state[2] = int(bool(self.state[2]) or fin)
+        self._host_draft()
+
+    def _host_draft(self):
+        ln, fin = int(self.state[0]), bool(self.state[2])
+        draft = [] if fin or ln + 1 >= self.max_length else lookup_candidates(
+            self.hist[:ln].tolist(), self.k, self.max_ngram, self.max_length, self.eos_list)
+        d = len(draft)
+        M = self.k + 1
+        last = int(self.hist[ln - 1])
+        row = [last] + draft + [last] * (self.k - d)
+        self.ids[:, 0] = torch.tensor(row, dtype=torch.int64)
+        self.pos.copy_(torch.arange(M, dtype=torch.int32) + ln - 1)
+        self.base[0] = ln - 1
+        self.step.copy_(torch.arange(M, dtype=torch.int64) + ln - self.prompt_len)
+        self.state[1] = d
+        self.readback[1:4] = torch.tensor([int(fin), ln, d])
+        self.readback[4 + M:] = torch.tensor(draft + [-1] * (self.k - d), dtype=torch.int64)
+
+    def first(self, logits):
+        """The first new token, selected from the prefill's logits [1, 1, V] (Philox counter 0), appended to the history;
+        then the first draft.  Returns (the token, whether it is an eos id)."""
+        L = self.prompt_len
+        self.step[0] = 0
+        self._select(logits.reshape(1, 1, -1), 1)
+        tok = int(self.sel[0])
+        fin = tok in self.eos_list
+        self.hist[L] = tok
+        self.state.copy_(torch.tensor([L + 1, 0, int(fin), 1, 0], dtype=torch.int32))
+        if self.hist.is_cuda:
+            kernels.lookup_step(self)
+        else:
+            self._host_draft()
+        if self.use_graph and not fin:
+            self.graph, self.graph1 = self._capture(self.k + 1), self._capture(1)
+        self.rb = self.readback.cpu()
+        return tok, fin
+
+    def run(self, host_done=None):
+        """One verify step: host_done (the host's stopping criteria on the candidate sequence; None without criteria) is
+        written before it.  M rows when the step has drafts, else the one-row step.  Returns the readback on the host
+        (also kept as `rb`): int64 [appended, finished, len, d, the appended tokens (M slots), the next drafts (k
+        slots)]."""
+        if host_done is not None:
+            self.state[4] = int(bool(host_done))
+        rows = self.k + 1 if int(self.rb[3]) else 1
+        graph = self.graph if rows > 1 else self.graph1
+        if graph is not None:
+            graph.replay()
+        else:
+            self._body(rows)
+        self.rb = rb = self.readback.cpu()
+        self.accepted.append(int(rb[0]))
+        return rb
+
+
+def lookup_loop(st, logits, max_new_tokens, stopping_criteria=None, streamer=None):
+    """The host side of prompt-lookup decoding on a LookupDecode `st` from the prefill's logits: the first token, then
+    verify steps until max_new_tokens, an eos id or a stopping criterion.  Host stopping_criteria are called as
+    transformers' _assisted_decoding calls them -- on the candidate sequence (the history plus the drafts) before
+    each verify step, whose acceptance then keeps one draft fewer when all match, and on the history after the
+    accepted tokens are appended -- each with scores None.  The streamer follows transformers' BaseStreamer contract
+    as HF's generate drives it: put(the prompt ids [1, L]) first, then the first token, then each step's accepted
+    tokens, then end().  Returns the count of new tokens in st.hist."""
+    L = st.prompt_len
+    out = st.hist.view(1, -1)
+    if streamer is not None:
+        streamer.put(out[:, :L].cpu())
+    tok, fin = st.first(logits)
+    n = 1
+    if streamer is not None:
+        streamer.put(torch.tensor([tok]))
+
+    def stop(seq):
+        return any(bool(torch.as_tensor(sc(seq, None)).all()) for sc in stopping_criteria)
+    while not fin and n < max_new_tokens:
+        if stopping_criteria is not None and stop(out[:, :L + n]):
+            break
+        rb = st.rb
+        done = None
+        if stopping_criteria is not None:
+            d = int(rb[3])
+            drafts = rb[4 + st.k + 1:4 + st.k + 1 + d].to(out.device)
+            done = stop(torch.cat([out[:, :L + n], drafts[None]], 1))
+        rb = st.run(done)
+        acc = int(rb[0])
+        n += acc
+        fin = bool(rb[1])
+        if streamer is not None:
+            streamer.put(rb[4:4 + acc].clone())
+    if streamer is not None:
+        streamer.end()
+    return n
+
+
+@torch.no_grad()
+def _generate_lookup(self, input_ids, images, bboxes, max_new_tokens, k, max_ngram, greedy, temperature, top_k, top_p,
+                     generator, eos_ids, stopping_criteria, cache, use_graph, streamer):
+    """generate()'s prompt-lookup path (batch 1): the prefill as the plain loop runs it, into a cache with room for k
+    more positions, then lookup_loop on a LookupDecode."""
+    L = input_ids.shape[1]
+    ids = input_ids.to(self.dev)
+    if cache is not None:
+        logits = self.prefill_cached(cache, input_ids, images, bboxes, None, new_tokens=max_new_tokens + k)
+    else:
+        cache = KVCache(self.cfg, 1, L + max_new_tokens + k, self.dev)
+        logits = self.forward_device(ids, None if images is None else images.to(self.dev, self.dt),
+                                     self.plan_boxes(bboxes), validate=True, last_only=True, cache=cache)
+    out = torch.zeros((1, L + max_new_tokens + k), dtype=torch.int64, device=self.dev)
+    out[:, :L] = ids
+    st = LookupDecode(self, cache, out, L, max_new_tokens, k, max_ngram, eos_ids, greedy, temperature, top_k, top_p,
+                      seed=0 if greedy else sampling_seed(generator), use_graph=use_graph)
+    n = lookup_loop(st, logits, max_new_tokens, stopping_criteria, streamer)
+    # the cache holds the prompt and every new token but the last, as after the plain loop
+    cache.length = L + n - 1
+    if cache.lens is not None:
+        cache.lens.fill_(L + n - 1)
+    cache.ids[:, L:] = -1
+    if n > 1:
+        cache.record_ids(out[:, L:L + n - 1], torch.full((1,), L, dtype=torch.int32, device=self.dev))
+    self.lookup_accepted = st.accepted   # diagnostic: tokens appended by each verify step of the engine's last lookup call
+    return out[:, :L + n]
 
 
 class Request:
@@ -1953,6 +2281,7 @@ def _generate_beams(self, input_ids, images, bboxes, max_new_tokens, num_beams, 
 
 
 PrefillEngine.decode_step = _decode_step
+PrefillEngine.verify_step = _verify_step
 PrefillEngine.generate = _generate
 
 

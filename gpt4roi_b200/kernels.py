@@ -397,6 +397,35 @@ def stop_step(ids, table, state, finished):
     return finished
 
 
+def lookup_step(st, sel=None):
+    """Prompt-lookup decoding, one launch (csrc/lookup.cu): with sel (the verify step's selected tokens, int64 [M]) the
+    acceptance of transformers' _assisted_decoding and then the next draft (g4r_lookup_step); without, the draft alone
+    (g4r_lookup_draft, after the prefill's first token).  st: an engine.LookupDecode -- its device buffers ids, hist,
+    state, base, pos, step, eos, readback and its k, max_ngram, prompt_len, max_length."""
+    M = st.k + 1
+    named = [('ids', st.ids, torch.int64, M), ('state', st.state, torch.int32, 5), ('base', st.base, torch.int32, 1),
+             ('pos', st.pos, torch.int32, M), ('step', st.step, torch.int64, M),
+             ('readback', st.readback, torch.int64, 4 + M + st.k)]
+    if sel is not None:
+        named.append(('sel', sel, torch.int64, M))
+    for name, t, dt, n in named:
+        if t.dtype != dt or t.numel() != n or not t.is_contiguous():
+            raise RuntimeError('lookup_step: %s must be a contiguous device %s tensor of %d elements' % (name, dt, n))
+    h = st.hist
+    if h.dtype != torch.int64 or not h.is_contiguous() or h.numel() < st.max_length:
+        raise RuntimeError('lookup_step: hist must be a contiguous int64 tensor of >= %d elements' % st.max_length)
+    n_eos = 0 if st.eos is None else st.eos.numel()
+    _L.require_cuda_same_device([('hist', h), ('eos', st.eos)] + [(n, t) for n, t, _, _ in named])
+    tail = (_L.ptr(st.eos), n_eos, _L.ptr(st.state), _L.ptr(st.base), _L.ptr(st.pos), _L.ptr(st.step),
+            _L.ptr(st.readback))
+    if sel is None:
+        _call('g4r_lookup_draft', h.device, _L.ptr(st.ids), _L.ptr(h), h.numel(), st.k, st.max_ngram, st.prompt_len,
+              st.max_length, *tail)
+    else:
+        _call('g4r_lookup_step', h.device, _L.ptr(sel), _L.ptr(st.ids), _L.ptr(h), h.numel(), st.k, st.max_ngram,
+              st.prompt_len, st.max_length, *tail)
+
+
 def kv_append(qkv, kcache, vcache, B, Ln, pos0, pos_dev=None, pos_rows=None, cache_rows=None, qlen=None):
     """Copy the k|v parts of packed qkv rows [B*Ln, 3*HD] into caches [B, Lmax, HD] at pos0..pos0+Ln-1.
     pos_rows: device int32 [B] -- sample b's rows go to pos_rows[b]..pos_rows[b]+Ln-1 instead (pos0 / pos_dev unused).

@@ -111,6 +111,8 @@ SIGNATURES = {
                                         _vp, _ll, _i, _f, _i, _i, _i, _vp, _i, _i, _vp, _vp, _ll, _vp]),
     'g4r_sample_tokens_rows_bf16': (_i, [_vp, _ll, _i, _i] + [_vp] * 12),
     'g4r_stop_step': (_i, [_vp, _vp, _ll, _i, _i, _i, _vp, _vp, _vp]),
+    'g4r_lookup_step': (_i, [_vp, _vp, _vp, _ll, _i, _i, _i, _i, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
+    'g4r_lookup_draft': (_i, [_vp, _vp, _ll, _i, _i, _i, _i, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
     'g4r_decode_attention_beam_bf16': (_i, [_vp, _ll, _vp, _vp, _vp, _ll, _i, _i, _i, _i, _vp, _vp, _i, _f, _vp]),
     'g4r_beam_step_bf16': (_i, [_vp, _ll] + [_i] * 5 + [_vp] + [_i] * 3 + [_c.c_double] + [_i] * 3 + [_vp] * 13),
     'g4r_beam_step_out_bf16': (_i, [_vp, _ll] + [_i] * 5 + [_vp] + [_i] * 3 + [_c.c_double] + [_i] * 3 + [_vp] * 14

@@ -259,6 +259,13 @@ class G4RCache:
     def __bool__(self):
         return True
 
+    def crop(self, n):
+        """Keep the first n positions (transformers' assisted decoding crops the cache to the accepted length after
+        every verify step): KVCache.crop, and the captured decode step, if any, continues from n."""
+        self.kv.crop(n)
+        if self.stepper is not None:
+            self.stepper.pos.fill_(self.kv.length)
+
     def reorder_cache(self, beam_idx):
         """transformers' beam search (GenerationMixin._beam_search) after every step: row i of the cache becomes row
         beam_idx[i] -- every layer's K/V, the recorded ids, lengths, images and boxes.  In place, so a CUDA graph
@@ -407,14 +414,17 @@ def _stack_images(images):
 
 @torch.no_grad()
 def _run_engine(eng, input_ids, images, bboxes, attention_mask, past_key_values, inputs_embeds, use_cache, want,
-                training=False, max_cache=None, last_only=False, new_prompt=False):
+                training=False, max_cache=None, last_only=False, new_prompt=False, logits_to_keep=0):
     """Inference dispatch shared by both model classes: prefill (ids or embeds, with or without the vision
     branch) or one decode step on our cache.  Mirrors spi_llava.py:44-48: the vision branch runs when images are
     given and (the input is longer than one token or the module is in training mode).
     On a non-empty cache, an input one token longer than what the cache holds is a decode step of its last token; a
     longer one, or any input marked as a generate call's prompt (new_prompt: HF's first iteration), is a later turn of
     the conversation (HF's documented past_key_values reuse): the prefix the cache holds is reused and the rest
-    prefilled (PrefillEngine.prefill_cached)."""
+    prefilled (PrefillEngine.prefill_cached).  A multi-token input with logits_to_keep > 1 that is not a new prompt
+    continues the cached sequence (transformers' assisted decoding feeds the last token and its drafts so): its tokens
+    are prefilled as one chunk after what the cache holds (PrefillEngine.extend) and the last logits_to_keep logits
+    are returned."""
     c = eng.cfg
     cache = _find_cache(past_key_values)
     if cache is not None and cache.kv.length > 0:
@@ -428,6 +438,10 @@ def _run_engine(eng, input_ids, images, bboxes, attention_mask, past_key_values,
             out = eng.prefill_cached(cache.kv, input_ids, _stack_images(images), bboxes, attention_mask,
                                      new_tokens=max(budget, 1))
             return out, cache
+        if input_ids.shape[1] > 1 and logits_to_keep > 1:
+            out = eng.extend(cache.kv, input_ids.to(eng.dev), None, None, last_only=False)
+            cache.stepper = None          # the chunk moved the lengths (and may have grown the cache)
+            return out[:, -int(logits_to_keep):], cache
         if input_ids.shape[1] != 1:
             input_ids = input_ids[:, -1:]
         ids = input_ids.to(eng.dev).contiguous()
@@ -640,6 +654,16 @@ def resolve_outputs(model, do_sample=None, temperature=None, **kwargs):
                 output_logits=rd and bool(gc.output_logits))
 
 
+def resolve_prompt_lookup(model, **kwargs):
+    """prompt_lookup_num_tokens and max_matching_ngram_size of a generate call, resolved as transformers resolves them
+    (the explicit kwargs, then `generation_config=`, then model.generation_config): (k, n-gram size), k None when
+    prompt lookup is off; the n-gram size defaults to 2, as HF's PromptLookupCandidateGenerator takes it."""
+    given = {k: v for k, v in kwargs.items() if v is not None}
+    gc = _generation_config(model, given)
+    k = gc.prompt_lookup_num_tokens
+    return (None if not k else int(k)), int(gc.max_matching_ngram_size or 2)
+
+
 def _generate_output(res, outs, past_key_values):
     """The engine loop's result as transformers' own generate output class (GenerateDecoderOnlyOutput, or
     GenerateBeamDecoderOnlyOutput for beam search).  past_key_values: the caller's cache, else None (the engine's own
@@ -816,7 +840,7 @@ class SPILlavaMPTForCausalLM(LlamaForCausalLM, _EngineHost):
         logits, cache = _run_engine(eng, input_ids, images, bboxes, attention_mask, past_key_values, inputs_embeds,
                                     use_cache, want='logits', training=self.training,
                                     last_only=(logits_to_keep == 1 and labels is None),
-                                    new_prompt=bool(kwargs.get('is_first_iteration')))
+                                    new_prompt=bool(kwargs.get('is_first_iteration')), logits_to_keep=logits_to_keep)
         loss = None
         if labels is not None:  # llava.py:238-249
             shift_logits = logits[..., :-1, :].float().reshape(-1, self.config.vocab_size)
@@ -832,13 +856,16 @@ class SPILlavaMPTForCausalLM(LlamaForCausalLM, _EngineHost):
         forward skips the vision branch for one-token inputs, spi_llava.py:47-48).  A generate call's prompt on a
         non-empty cache (a later turn of a conversation, a regenerated or a shorter one) is passed whole, with its mask:
         the forward reuses the prefix the cache holds and prefills the rest.  The prompt is HF's first iteration
-        (`is_first_iteration`); without that flag, an input longer than the cache plus one token is taken as one."""
+        (`is_first_iteration`); without that flag, an input longer than the cache plus one token is taken as one.
+        After the first iteration the tokens the cache does not hold yet are passed: the last one, or with assisted
+        decoding (prompt_lookup_num_tokens) the last one and the candidate tokens, whose logits the forward keeps as
+        HF's logits_to_keep asks."""
         cache = _find_cache(past_key_values)
         first = kwargs.get('is_first_iteration')
         if cache is not None and cache.kv.length > 0:
             decode = (input_ids.shape[1] == cache.kv.length + 1) if first is None else not first
             if decode:
-                input_ids = input_ids[:, -1:]
+                input_ids = input_ids[:, min(cache.kv.length, input_ids.shape[1] - 1):]
         if inputs_embeds is not None and (cache is None or cache.kv.length == 0):
             model_inputs = {'inputs_embeds': inputs_embeds}
         else:
@@ -898,7 +925,19 @@ class SPILlavaMPTForCausalLM(LlamaForCausalLM, _EngineHost):
         transformers' GenerateDecoderOnlyOutput (GenerateBeamDecoderOnlyOutput with beam search: sequences_scores,
         beam_indices) with HF's scores / logits, written by the selection and beam kernels inside the graphed step;
         model.compute_transition_scores takes them.  Its past_key_values is the caller's cache when one was passed,
-        else None.  output_attentions / output_hidden_states raise NotImplementedError on both loops."""
+        else None.  output_attentions / output_hidden_states raise NotImplementedError on both loops.
+        prompt_lookup_num_tokens = k (resolve_prompt_lookup; max_matching_ngram_size, default 2), transformers' prompt
+        lookup decoding: on the engine loop each step drafts up to k tokens by copying what followed the earliest
+        earlier occurrence of the sequence's last n-gram in the prompt or the answer, and verifies them in one graphed
+        decode step over k + 1 rows (engine.LookupDecode), so a repetitive answer takes fewer weight passes.  It runs
+        for batch 1 with greedy or temperature / top_k / top_p selection, one eos id or a list, past_key_values and
+        host stopping_criteria (called as HF's assisted decoding calls them); the tokens are the plain loop's, up to the
+        attention's summation order, and a streamer= gets the prompt, then each step's accepted tokens (transformers'
+        BaseStreamer contract, as HF's generate drives it).  When sampling with top_k / top_p, HF's own assisted loop
+        also drops draft ids its warpers mask on constant logits; the engine's draft rule does not, so drafts and accept
+        counts (not the tokens' distribution) can differ from use_hf_loop=True's.  Any other call (batch > 1,
+        logits processors, stop_strings, outputs, beams, num_return_sequences > 1) ignores the option and runs the plain
+        loop.  With use_hf_loop=True transformers' own assisted decoding runs over this model's cache (G4RCache.crop)."""
         if bboxes is None:
             bboxes = getattr(getattr(self, 'forward', None), 'keywords', {}).get('bboxes')
         if use_hf_loop:
@@ -945,6 +984,9 @@ class SPILlavaMPTForCausalLM(LlamaForCausalLM, _EngineHost):
         if nrs > 1 and pkv is not None:
             raise NotImplementedError('several sampled answers per prompt (num_return_sequences=%d) on a conversation '
                                       'cache (past_key_values) run on the HF loop only: pass use_hf_loop=True' % nrs)
+        lookup, ngram = resolve_prompt_lookup(self, do_sample=do_sample, temperature=temperature, **gen)
+        lk = {} if lookup is None else dict(prompt_lookup_num_tokens=lookup, max_matching_ngram_size=ngram,
+                                            streamer=kwargs.get('streamer'))
         eng = self._get_engine(input_ids.device)
         kv = None
         if pkv is not None:   # a conversation's cache: reused and left holding this turn too
@@ -961,7 +1003,7 @@ class SPILlavaMPTForCausalLM(LlamaForCausalLM, _EngineHost):
                            stop_strings=None if stops is None else stop_strings_from_tokenizer(kwargs['tokenizer'], stops),
                            num_return_sequences=nrs, repetition_penalty=procs['repetition_penalty'],
                            no_repeat_ngram_size=procs['no_repeat_ngram_size'], min_length=procs['min_length'],
-                           min_new_tokens=procs['min_new_tokens'], length_eos_ids=procs['eos_ids'], **outs)
+                           min_new_tokens=procs['min_new_tokens'], length_eos_ids=procs['eos_ids'], **outs, **lk)
         return _generate_output(res, outs, pkv) if outs['return_dict_in_generate'] else res
 
     def continuous_batcher(self, slots=8, max_len=2048, tokenizer=None, stop_strings=None, prefix_reuse=False):

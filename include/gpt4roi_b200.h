@@ -436,6 +436,31 @@ int g4r_sample_tokens_rows_bf16(const void* logits, long long ld, int S, int V, 
 int g4r_stop_step(const long long* ids, const short* step, long long ld, int V_tok, int S, int B, int* state,
                   int* finished, void* stream);
 
+/* ---- prompt-lookup decoding (batch 1; the last launch of each verify step) ---------------------
+ * Replaces transformers' PromptLookupCandidateGenerator.get_candidates and the acceptance of
+ * GenerationMixin._assisted_decoding (greedy / non-speculative-sampling branch) for generate(prompt_lookup_num_tokens=k).
+ * The verify step feeds M = k + 1 rows: ids[0] the last accepted token, ids[1..d] the d drafts (rows past d repeat
+ * ids[0]), at positions pos[i] = base[0] + i, and selects sel[i] per row.
+ * hist: int64 [ld_h], the prompt then the accepted tokens; state: int32 [5] = {len, d, finished, appended, host_done};
+ * base: int32 [1]; pos: int32 [M]; step: int64 [M] (row i's Philox counter, the index of the new token it decides);
+ * eos: int32 [n_eos]; readback: int64 [4 + M + k] = {appended, finished, len, d, the appended tokens [M], the next
+ * drafts [k] (-1 past d)}.
+ * g4r_lookup_step: n = the count of leading drafts ids[1 + i] equal to sel[i]; if the candidate sequence was done
+ * (len + d >= max_length, or host_done != 0: the host's stopping criteria on it) and n == d > 0, n -= 1; then
+ * min(n + 1, max_length - len) tokens sel[0..] are appended to hist, len advances by as many, and finished is set when
+ * one of them is an eos id.  Then, as g4r_lookup_draft, the next draft from hist[0..len): for g = min(max_ngram,
+ * len - 1) down to 1, the smallest idx with hist[idx..idx+g) == hist[len-g..len) and idx + g < min(len, max_length)
+ * wins; the draft is hist[idx+g .. min(idx+g+k, len, max_length)) cut before its first eos id (no draft when
+ * finished, when len + 1 >= max_length, or when no window matches).  Writes ids, pos, base, step (= len - prompt_len
+ * + i), state and readback.  max_length: prompt_len + max_new_tokens (<= ld_h).
+ * Capturable: every per-step value is read from device memory. */
+int g4r_lookup_step(const long long* sel, long long* ids, long long* hist, long long ld_h, int k, int max_ngram,
+                    int prompt_len, int max_length, const int* eos, int n_eos, int* state, int* base, int* pos,
+                    long long* step, long long* readback, void* stream);
+int g4r_lookup_draft(long long* ids, long long* hist, long long ld_h, int k, int max_ngram, int prompt_len,
+                     int max_length, const int* eos, int n_eos, int* state, int* base, int* pos, long long* step,
+                     long long* readback, void* stream);
+
 /*
  * NHWC convolution as an implicit GEMM (stride 1, pad (ksize-1)/2, ksize 1 or 3):
  *   Y[n,y,x,co] = act( sum_{ky,kx,ci} X[n,y+ky-1,x+kx-1,ci] * Wt[co,(ky*ks+kx)*Cin+ci] + bias[co] )
