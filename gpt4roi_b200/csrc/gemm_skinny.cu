@@ -330,8 +330,16 @@ static int decode_gemm(const void* x, long long ldx, const void* W, long long ld
                        int cache_lmax, int cache_hd, void* stream) {
   G4R_REQUIRE(x && W && out && M > 0 && M <= 16 && N > 0 && K > 0, "decode_gemm: M must be 1..16 (got %d)", M);
   G4R_REQUIRE(ldx % 8 == 0 && ldw % 8 == 0 && K % 32 == 0, "decode_gemm: K %% 32 == 0 and 16-byte-aligned rows required");
+  // the kernel reads both operands with 16-byte vector loads along rows of ldx / ldw elements
+  G4R_REQUIRE(((uintptr_t)x & 15) == 0 && ((uintptr_t)W & 15) == 0, "decode_gemm: x and W must be 16-byte aligned");
+  G4R_REQUIRE(ldx >= K && ldw >= K, "decode_gemm: ldx (%lld) and ldw (%lld) must be >= K (%d)", ldx, ldw, K);
   G4R_REQUIRE(act == SK_ACT_NONE || act == SK_ACT_SWIGLU, "decode_gemm: act must be none or swiglu");
   G4R_REQUIRE((rope_cos == nullptr) == (rope_sin == nullptr), "decode_gemm: both RoPE tables or none");
+  // the RoPE epilogue stores the rotated (or v) columns and returns; the SwiGLU epilogue writes out[:, n / 2]: neither
+  // applies the other epilogues, so a combination is refused rather than silently dropped
+  G4R_REQUIRE(!(residual && rope_cos), "decode_gemm: a residual cannot be combined with RoPE");
+  G4R_REQUIRE(!(residual && act == SK_ACT_SWIGLU), "decode_gemm: a residual cannot be combined with SwiGLU");
+  G4R_REQUIRE(!(act != SK_ACT_NONE && rope_cos), "decode_gemm: an activation cannot be combined with RoPE");
   G4R_REQUIRE(!(kcache || vcache) || (rope_cos && kcache && vcache && cache_lmax > 0 && cache_hd > 0 && N == 3 * cache_hd),
               "decode_gemm: the KV-cache write needs the fused q|k|v projection with RoPE (N == 3 * cache_hd)");
   SkinnyParams p{};

@@ -203,19 +203,32 @@ def decode_gemm(x, weight, act=None, residual=None, rope=None, kv=None, pos_rows
     pos_rows: device int32 [M] -- sample m is rotated at (and cached at) pos_rows[m] instead of pos0 / pos_dev."""
     M, K = x.shape
     N = weight.shape[0]
-    dev = _L.require_cuda_same_device([('x', x), ('weight', weight), ('residual', residual)])
-    a16 = _act16('decode_gemm', x, weight)
-    n_out = N // 2 if act == 'swiglu' else N
-    out = torch.empty((M, n_out), dtype=a16, device=dev)
     cos = sin = pos_dev = None
     rope_cols = pos0 = 0
     if rope is not None:
         cos, sin, rope_cols, pos0, pos_dev = rope
     kc = vc = None
-    lmax = hd = 0
     if kv is not None:
         kc, vc = kv
+    dev = _L.require_cuda_same_device([('x', x), ('weight', weight), ('residual', residual), ('cos', cos), ('sin', sin),
+                                       ('pos_dev', pos_dev), ('pos_rows', pos_rows), ('kcache', kc), ('vcache', vc)])
+    a16 = _act16('decode_gemm', x, weight)
+    n_out = N // 2 if act == 'swiglu' else N
+    lmax = hd = 0
+    if kv is not None:
+        if kc.dtype != a16 or vc.dtype != a16:
+            raise RuntimeError('decode_gemm: the KV caches must be %s, got %s / %s' % (a16, kc.dtype, vc.dtype))
+        _L.require_contiguous([('kcache', kc), ('vcache', vc)])
+        if kc.dim() != 3 or kc.shape != vc.shape or kc.shape[0] < M or 3 * kc.shape[2] != N:
+            raise RuntimeError('decode_gemm: the KV caches must both be [>= %d, Lmax, %d], got %s / %s'
+                               % (M, N // 3, tuple(kc.shape), tuple(vc.shape)))
         lmax, hd = kc.shape[1], kc.shape[2]
+    if rope is not None and pos_dev is None and pos_rows is None:
+        # the host position is the one position source: it must name a row of the tables and of the caches
+        if not 0 <= pos0 < cos.shape[0] or (kv is not None and pos0 >= lmax):
+            raise RuntimeError('decode_gemm: pos0 = %d outside the RoPE tables (%d rows)%s'
+                               % (pos0, cos.shape[0], ' or the KV cache (Lmax %d)' % lmax if kv is not None else ''))
+    out = torch.empty((M, n_out), dtype=a16, device=dev)
     with torch.cuda.device(dev):
         _ps = _prof_begin(dev)
         if pos_rows is not None:
