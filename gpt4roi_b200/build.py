@@ -17,9 +17,11 @@ LIB = os.path.join(PKG, 'libgpt4roi_b200.so')
 ARCH = ['-gencode', 'arch=compute_90a,code=sm_90a']
 COMMON = ['-O3', '-std=c++17', '-lineinfo', '-Xcompiler', '-fPIC', '--expt-relaxed-constexpr',
           '-Xptxas', '-v']
-# per-file extra flags.  roi_align.cu: no FMA contraction (bit-exact bin/weight arithmetic).
+# per-file extra flags.  roi_align.cu, clip_preprocess.cu: no FMA contraction (bit-exact bin/weight arithmetic; the
+# FMAs clip_preprocess.cu needs to match torch's CPU bilinear are explicit __fmaf_rn).
 EXTRA = {
     'roi_align.cu': ['-fmad=false'],
+    'clip_preprocess.cu': ['-fmad=false'],
 }
 # The inference kernels are built twice: bf16 as written, and an fp16 twin (-DG4R_ACT_HALF, csrc/act_type.cuh) for the
 # demo's dtype (gpt4roi/app.py:74-98: model.half()).  Both land in the one shared library.

@@ -102,6 +102,7 @@ SIGNATURES = {
     'g4r_sumsq': (_i, [_vp, _i, _ll, _vp, _vp]),
     'g4r_grad_clip_coef': (_i, [_vp, _ll, _f, _f, _vp, _vp]),
     'g4r_preprocess_images': (_i, [_vp] * 6 + [_i, _i, _vp, _vp, _i, _i, _vp]),
+    'g4r_clip_preprocess': (_i, [_vp] * 4 + [_i, _i, _ll, _vp, _vp, _i, _vp]),
     'g4r_affine_relu_nhwc_bf16': (_i, [_vp, _vp, _vp, _vp, _i, _ll, _i, _vp]),
     'g4r_add_bias_pos_cast': (_i, [_vp, _i, _vp, _vp, _vp, _i, _i, _vp]),
     'g4r_sample_tokens_bf16': (_i, [_vp, _ll, _i, _i, _f, _i, _f, _i, _c.c_ulonglong, _vp, _i, _i, _vp, _vp, _vp]),

@@ -699,6 +699,18 @@ int g4r_preprocess_images(const void* src_packed, const long long* offsets, cons
                           const int* flip, void* out, int B, int S, const float* mean3, const float* std3, int to_rgb,
                           int out_dtype, void* stream);
 
+/* CLIPImageProcessor image path of the demo and the VCR datasets (gpt4roi/app.py:125-136, gpt4roi/datasets/vcr.py:
+ * 181-189): CLIPImageProcessor.preprocess(image, do_center_crop=False) [PIL BICUBIC resize of the short side,
+ * integer-exact; float32(u8 * (1/255) in double); (x - mean) / std in float32] -> F.interpolate((S, S), 'bilinear',
+ * align_corners=False) [torch's CPU arithmetic] for a ragged batch of uint8 HWC RGB images, in two launches.
+ * meta: device int64 [B][13] per-image fields (source address, width, offsets into `tables` and `tmp`, counts; see
+ * csrc/clip_preprocess.cu); tables: device int32 tap windows, fixed-point weights and bilinear tables built by
+ * gpt4roi_b200.input_pipeline.ClipPreprocessor; tmp: device uint8 intermediate; max_work1 = the largest per-image
+ * rows x columns of the first resize pass.  out [B,3,S,S] fp32 (bit-identical to that path), bf16 or fp16.
+ * mean3 / std3: HOST float[3]. */
+int g4r_clip_preprocess(const long long* meta, const int* tables, void* tmp, void* out, int B, int S,
+                        long long max_work1, const float* mean3, const float* std3, int out_dtype, void* stream);
+
 /* Apply a pending GroupNorm affine + ReLU to an NHWC bf16 map: out = relu(z * scale[b,c] + shift[b,c]) with the
  * fp32 [B,C] scale / shift of g4r_gn_finalize.  The activated map is what MLVLFuseModule.forward returns
  * (gpt4roi/models/layers.py:182-195; mmcv ConvModule conv -> GN -> ReLU, conv_module.py:196-208); inside the fused
