@@ -29,7 +29,7 @@ Anything outside this (output_attentions, left padding, list-of-images) raises i
 """
 import collections
 import weakref
-from typing import List, Optional
+from typing import List, NamedTuple, Optional
 
 import torch
 import torch.nn as nn
@@ -518,25 +518,78 @@ def _generation_config(model, given):
     return gc
 
 
-def _resolve_selection(model, input_len, do_sample, temperature, kwargs):
-    """-> (do_sample, temperature, top_k, top_p), the history-dependent processors' parameters, the names of every
-    processor beyond the three warpers in HF's order, the names of those that are not history-dependent."""
+class ResolvedGenerate(NamedTuple):
+    """A generate call's configuration, as resolve_generate reads it off transformers' resolution."""
+    do_sample: bool
+    temperature: float
+    top_k: int              # 0: off
+    top_p: float            # 1: off
+    processors: dict        # repetition_penalty, no_repeat_ngram_size, min_length, min_new_tokens, eos_ids
+    names: tuple            # every processor beyond the three warpers HF would build, in HF's order
+    other: tuple            # those of `names` the engine loop does not run
+    num_return_sequences: int
+    beam: Optional[dict]    # None when num_beams is 1
+    outputs: dict           # return_dict_in_generate, output_scores, output_logits
+    layer_outputs: bool     # output_attentions / output_hidden_states asked for
+    lookup: tuple           # (prompt_lookup_num_tokens or None, max_matching_ngram_size)
+    stop_strings: Optional[tuple]
+
+
+_LAYER_OUTPUTS = ('output_attentions / output_hidden_states: attention maps and per-layer hidden states are not '
+                  'materialised by the fused engine')
+_STOP_STRINGS_NEED_TOKENIZER = (
+    "There are one or more stop strings, either in the arguments to `generate` or in the model's generation config, "
+    "but we could not locate a tokenizer. When generating with stop strings, you must pass the model's tokenizer to "
+    "the `tokenizer` argument of `generate`.")
+
+
+def resolve_generate(model, input_len, max_new_tokens, do_sample=None, temperature=None, eos_token_id=None,
+                     **kwargs):
+    """A generate call's configuration, resolved once as transformers resolves it (GenerationMixin.
+    _prepare_generation_config: explicit kwargs, then `generation_config=`, then model.generation_config, then HF's
+    defaults; `do_sample=True` alone therefore samples with top_k=50), for an input of `input_len` tokens.  Values
+    HF's config validation or its processors refuse raise HF's ValueError here (greedy with num_return_sequences > 1,
+    num_return_sequences > num_beams, max_new_tokens < 1, ...); what the engine loop or the batcher does not run is
+    left to their callers to refuse.
+
+    The selection rule is (False, 1.0, 0, 1.0) for greedy.  The processors are read off HF's own _get_logits_processor:
+    without beam search after HF's length preparation (GenerationMixin._prepare_generated_length: a given
+    min_new_tokens sets min_length to min_new_tokens + input_len); `processors` holds the history-dependent ones with
+    neutral values for those HF does not build or that can never suppress anything (min_length at most input_len,
+    min_new_tokens 0), and eos_ids, the resolved eos list (generation_config._eos_token_tensor: the eos_token_id kwarg,
+    else the model's) that the minimum lengths suppress.  `other` lists the rest (min_p, typical_p, epsilon / eta
+    cutoffs, bad_words_ids, suppress_tokens, sequence_bias, a caller's logits_processor, ...).  With num_beams > 1 the
+    list is built as HF builds it for beam search, and `names` and `other` both hold every processor in it, the
+    neutral ones included: the engine loop runs none with beams.  `beam` is a dict of num_beams, length_penalty,
+    early_stopping, num_return_sequences, eos_token_id (a list), pad_token_id and max_length.  output_scores and
+    output_logits count only with return_dict_in_generate, as in HF.  The n-gram size of prompt lookup defaults to 2,
+    as HF's PromptLookupCandidateGenerator takes it."""
     from transformers.generation import logits_process as lp
-    given = {k: v for k, v in dict(kwargs, do_sample=do_sample, temperature=temperature).items() if v is not None}
-    gc = _generation_config(model, given)
+    given = dict(kwargs, do_sample=do_sample, temperature=temperature, eos_token_id=eos_token_id,
+                 max_new_tokens=max_new_tokens)
+    gc = _generation_config(model, {k: v for k, v in given.items() if v is not None})
+    beam = None
     if (gc.num_beams or 1) > 1:
-        raise NotImplementedError('beam search (num_beams=%d) runs on the HF loop only: pass use_hf_loop=True'
-                                  % gc.num_beams)
-    if gc.min_new_tokens is not None:   # GenerationMixin._prepare_generated_length: min_new_tokens takes precedence
+        eos, pad = gc._eos_token_tensor, gc._pad_token_tensor
+        beam = dict(num_beams=int(gc.num_beams),
+                    length_penalty=float(gc.length_penalty if gc.length_penalty is not None else 1.0),
+                    early_stopping=gc.early_stopping if gc.early_stopping is not None else False,
+                    num_return_sequences=int(gc.num_return_sequences or 1),
+                    eos_token_id=None if eos is None else eos.flatten().tolist(),
+                    pad_token_id=None if pad is None else int(pad),
+                    max_length=int(input_len + gc.max_new_tokens if gc.max_new_tokens is not None else gc.max_length))
+    elif gc.min_new_tokens is not None:
         gc.min_length = gc.min_new_tokens + input_len
     procs = model._get_logits_processor(gc, input_ids_seq_length=input_len, device='cpu', model_kwargs={},
                                         logits_processor=kwargs.get('logits_processor'))
     found = dict(repetition_penalty=1.0, no_repeat_ngram_size=0, min_length=0, min_new_tokens=0, eos_ids=[])
     names, other = [], []
     for p in procs:
-        if isinstance(p, (lp.TemperatureLogitsWarper, lp.TopKLogitsWarper, lp.TopPLogitsWarper)):
+        if beam is not None:
+            other.append(type(p).__name__)
+        elif isinstance(p, (lp.TemperatureLogitsWarper, lp.TopKLogitsWarper, lp.TopPLogitsWarper)):
             continue
-        if type(p) is lp.RepetitionPenaltyLogitsProcessor and not p.prompt_ignore_length:
+        elif type(p) is lp.RepetitionPenaltyLogitsProcessor and not p.prompt_ignore_length:
             found['repetition_penalty'] = float(p.penalty)
         elif type(p) is lp.NoRepeatNGramLogitsProcessor:
             found['no_repeat_ngram_size'] = int(p.ngram_size)
@@ -556,112 +609,17 @@ def _resolve_selection(model, input_len, do_sample, temperature, kwargs):
     else:
         rule = (True, float(gc.temperature if gc.temperature is not None else 1.0), int(gc.top_k or 0),
                 float(gc.top_p if gc.top_p is not None else 1.0))
-    return rule, found, names, other
-
-
-def resolve_processors(model, input_len, do_sample=None, temperature=None, **kwargs):
-    """The engine loop's selection rule for a generate call, resolved as transformers resolves it: explicit kwargs, then
-    `generation_config=`, then model.generation_config, then HF's global defaults (GenerationMixin.
-    _prepare_generation_config; `do_sample=True` alone therefore samples with top_k=50), and read off the processors
-    HF's _get_logits_processor builds from it, after HF's length preparation (GenerationMixin.
-    _prepare_generated_length: a given min_new_tokens sets min_length to min_new_tokens + the input length).  Returns (do_sample, temperature, top_k, top_p, processors) with top_k 0 /
-    top_p 1 meaning off; processors: dict(repetition_penalty, no_repeat_ngram_size, min_length, min_new_tokens,
-    eos_ids) -- the history-dependent processors HF would apply (neutral values for those it does not build or that
-    can never suppress anything: min_length at most the input length, min_new_tokens 0), eos_ids
-    the resolved eos list (generation_config._eos_token_tensor: the eos_token_id kwarg, else the model's config) that
-    the minimum lengths suppress.  A call whose resolved config would make HF apply any other logits processor (min_p,
-    typical_p, epsilon / eta cutoffs, bad_words_ids, suppress_tokens, sequence_bias, a caller's logits_processor, ...),
-    or run beam search, raises NotImplementedError: the engine loop does not implement it, the HF loop
-    (use_hf_loop=True) does."""
-    rule, found, _, other = _resolve_selection(model, input_len, do_sample, temperature, kwargs)
-    if other:
-        raise NotImplementedError('the engine loop applies temperature, top_k, top_p, repetition_penalty, '
-                                  'no_repeat_ngram_size, min_length and min_new_tokens only; %s run on the HF loop: '
-                                  'pass use_hf_loop=True' % ', '.join(other))
-    return rule + (found,)
-
-
-def resolve_sampling(model, input_len, do_sample=None, temperature=None, **kwargs):
-    """resolve_processors for a selection without logits processors: returns (do_sample, temperature, top_k, top_p).
-    A call whose resolved config would make HF apply any logits processor beyond TemperatureLogitsWarper,
-    TopKLogitsWarper and TopPLogitsWarper (repetition_penalty, min_p, typical_p, no_repeat_ngram_size, a caller's
-    logits_processor, ...), or run beam search, raises NotImplementedError naming use_hf_loop=True."""
-    rule, _, names, _ = _resolve_selection(model, input_len, do_sample, temperature, kwargs)
-    if names:
-        raise NotImplementedError('the engine loop applies temperature, top_k and top_p only; %s run on the HF loop: '
-                                  'pass use_hf_loop=True' % ', '.join(names))
-    return rule
-
-
-def resolve_num_return_sequences(model, do_sample=None, temperature=None, **kwargs):
-    """How many answers per prompt a generate call without beam search returns, resolved as transformers resolves it:
-    the explicit kwarg, then `generation_config=`, then model.generation_config (GenerationMixin.
-    _prepare_generation_config).  Greedy selection with more than one raises HF's own ValueError from the config's
-    validation."""
-    given = {k: v for k, v in dict(kwargs, do_sample=do_sample, temperature=temperature).items() if v is not None}
-    return int(_generation_config(model, given).num_return_sequences or 1)
-
-
-def resolve_beam_search(model, input_len, max_new_tokens, do_sample=None, **kwargs):
-    """The engine loop's beam search for a generate call, resolved as transformers resolves it (explicit kwargs, then
-    `generation_config=`, then model.generation_config, then HF's defaults: GenerationMixin._prepare_generation_config).
-    Returns None when the resolved num_beams is 1, else a dict of num_beams, length_penalty, early_stopping,
-    num_return_sequences, eos_token_id (a list), pad_token_id and max_length.  Beam search with do_sample or with any
-    logits processor raises NotImplementedError: the HF loop (use_hf_loop=True) runs those.  This resolves the search
-    alone: a call whose resolved config asks for outputs (output_scores / output_logits / return_dict_in_generate)
-    raises NotImplementedError too; generate() resolves those with resolve_outputs and calls this with them off."""
-    given = {k: v for k, v in dict(kwargs, do_sample=do_sample, max_new_tokens=max_new_tokens).items() if v is not None}
-    gc = _generation_config(model, given)
-    N = gc.num_beams or 1
-    if N <= 1:
-        return None
-    hf = 'runs on the HF loop only: pass use_hf_loop=True'
-    if gc.do_sample:
-        raise NotImplementedError('beam search with do_sample (beam sampling) ' + hf)
-    if gc.output_scores or gc.output_logits or gc.return_dict_in_generate:
-        raise NotImplementedError('resolve_beam_search resolves the search alone: resolve output_scores / output_logits '
-                                  '/ return_dict_in_generate with resolve_outputs and pass them off here, as generate() '
-                                  'does (or generate with use_hf_loop=True)')
-    procs = model._get_logits_processor(gc, input_ids_seq_length=input_len, device='cpu', model_kwargs={},
-                                        logits_processor=kwargs.get('logits_processor'))
-    if len(procs):
-        raise NotImplementedError('the engine loop applies no logits processor to beam search; %s %s'
-                                  % (', '.join(type(p).__name__ for p in procs), hf))
-    nrs = gc.num_return_sequences or 1
-    if nrs > N:
-        raise ValueError('num_return_sequences (%d) must be <= num_beams (%d)' % (nrs, N))
-    eos = gc._eos_token_tensor
-    pad = gc._pad_token_tensor
-    return dict(num_beams=int(N), length_penalty=float(gc.length_penalty if gc.length_penalty is not None else 1.0),
-                early_stopping=gc.early_stopping if gc.early_stopping is not None else False,
-                num_return_sequences=int(nrs), eos_token_id=None if eos is None else eos.flatten().tolist(),
-                pad_token_id=None if pad is None else int(pad),
-                max_length=int(input_len + gc.max_new_tokens if gc.max_new_tokens is not None else gc.max_length))
-
-
-def resolve_outputs(model, do_sample=None, temperature=None, **kwargs):
-    """What a generate call returns besides the ids, resolved as transformers resolves it (the explicit kwargs, then
-    `generation_config=`, then model.generation_config): a dict of return_dict_in_generate, output_scores and
-    output_logits (the last two only count with the first, as in HF).  output_attentions / output_hidden_states raise
-    NotImplementedError: the fused engine materialises neither, on either loop."""
-    given = {k: v for k, v in dict(kwargs, do_sample=do_sample, temperature=temperature).items() if v is not None}
-    gc = _generation_config(model, given)
-    if gc.output_attentions or gc.output_hidden_states:
-        raise NotImplementedError('output_attentions / output_hidden_states: attention maps and per-layer hidden states '
-                                  'are not materialised by the fused engine')
     rd = bool(gc.return_dict_in_generate)
-    return dict(return_dict_in_generate=rd, output_scores=rd and bool(gc.output_scores),
-                output_logits=rd and bool(gc.output_logits))
-
-
-def resolve_prompt_lookup(model, **kwargs):
-    """prompt_lookup_num_tokens and max_matching_ngram_size of a generate call, resolved as transformers resolves them
-    (the explicit kwargs, then `generation_config=`, then model.generation_config): (k, n-gram size), k None when
-    prompt lookup is off; the n-gram size defaults to 2, as HF's PromptLookupCandidateGenerator takes it."""
-    given = {k: v for k, v in kwargs.items() if v is not None}
-    gc = _generation_config(model, given)
-    k = gc.prompt_lookup_num_tokens
-    return (None if not k else int(k)), int(gc.max_matching_ngram_size or 2)
+    stops = gc.stop_strings
+    return ResolvedGenerate(
+        *rule, processors=found, names=tuple(names), other=tuple(other),
+        num_return_sequences=int(gc.num_return_sequences or 1), beam=beam,
+        outputs=dict(return_dict_in_generate=rd, output_scores=rd and bool(gc.output_scores),
+                     output_logits=rd and bool(gc.output_logits)),
+        layer_outputs=bool(gc.output_attentions or gc.output_hidden_states),
+        lookup=(int(gc.prompt_lookup_num_tokens) if gc.prompt_lookup_num_tokens else None,
+                int(gc.max_matching_ngram_size or 2)),
+        stop_strings=None if stops is None else (stops,) if isinstance(stops, str) else tuple(stops))
 
 
 def _generate_output(res, outs, past_key_values):
@@ -696,23 +654,6 @@ def stop_strings_from_tokenizer(tokenizer, stop_strings):
             _STOP_STRINGS.popitem(last=False)
     _STOP_STRINGS.move_to_end(key)
     return _STOP_STRINGS[key]
-
-
-def resolve_stop_strings(model, tokenizer=None, stop_strings=None, generation_config=None):
-    """The stop strings of a generate call, resolved as transformers resolves them (the explicit kwarg, then
-    `generation_config=`, then model.generation_config): a tuple, or None when there are none.  Stop strings without a
-    tokenizer raise the ValueError transformers raises (GenerationMixin._get_stopping_criteria)."""
-    given = dict(generation_config=generation_config)
-    if stop_strings is not None:
-        given['stop_strings'] = stop_strings
-    stops = _generation_config(model, given).stop_strings
-    if stops is None:
-        return None
-    if tokenizer is None:
-        raise ValueError("There are one or more stop strings, either in the arguments to `generate` or in the model's "
-                         "generation config, but we could not locate a tokenizer. When generating with stop strings, "
-                         "you must pass the model's tokenizer to the `tokenizer` argument of `generate`.")
-    return (stops,) if isinstance(stops, str) else tuple(stops)
 
 
 class SPILlavaMPTForCausalLM(LlamaForCausalLM, _EngineHost):
@@ -903,32 +844,32 @@ class SPILlavaMPTForCausalLM(LlamaForCausalLM, _EngineHost):
         prepare_inputs_for_generation / past_key_values instead of the engine's loop.
         attention_mask (right- or left-padded) and pad_token_id reach either loop: prompts of different lengths in one
         batch each continue from their own last token, and finished rows are filled with pad_token_id.
-        Sampling on the engine loop follows HF's resolution of do_sample / temperature / top_k / top_p /
-        generation_config (resolve_sampling: the demo's call samples from the top 50 at T = 0.2, as on the HF loop);
-        the draws are keyed by torch's default generator (or `generator=`), so torch.manual_seed makes them
-        reproducible.  repetition_penalty, no_repeat_ngram_size, min_length and min_new_tokens (resolve_processors, with
-        HF's resolved eos list) run there too, on the device inside the decode step, greedy or sampled; other logits
-        processors raise NotImplementedError there.
-        stop_strings (with tokenizer=, as transformers' generate takes them; resolve_stop_strings) are matched on the
-        device, per row, inside the decode step (engine.StopStrings): a row that has produced a stop string is finished
+        The engine loop resolves the call's keywords, generation_config= and the model's generation config once, as
+        transformers resolves them (resolve_generate), and refuses what it does not run before it builds an engine.
+        Sampling there follows HF's resolution of do_sample / temperature / top_k / top_p (the demo's call samples
+        from the top 50 at T = 0.2, as on the HF loop); the draws are keyed by torch's default generator (or
+        `generator=`), so torch.manual_seed makes them reproducible.  repetition_penalty, no_repeat_ngram_size,
+        min_length and min_new_tokens (with HF's resolved eos list) run there too, on the device inside the decode
+        step, greedy or sampled; other logits processors raise NotImplementedError there.
+        stop_strings (with tokenizer=, as transformers' generate takes them) are matched on the device, per row,
+        inside the decode step (engine.StopStrings): a row that has produced a stop string is finished
         and, when eos_token_id and pad_token_id are given, filled with pad_token_id, as on the HF loop.  Host
         stopping_criteria (KeywordsStoppingCriteria) keep running as callbacks after every token.
-        num_beams > 1 (do_sample false) runs beam search on the engine loop (resolve_beam_search: length_penalty,
-        early_stopping, num_return_sequences, eos / max length as HF resolves them): the prompt is prefilled once per
-        sample and the beams share its KV cache; beam sampling, logits processors, stopping_criteria, stop_strings and
+        num_beams > 1 (do_sample false) runs beam search on the engine loop (length_penalty, early_stopping,
+        num_return_sequences, eos / max length as HF resolves them): the prompt is prefilled once per sample and the
+        beams share its KV cache; beam sampling, logits processors, stopping_criteria, stop_strings and
         past_key_values raise NotImplementedError there, and run with use_hf_loop=True.
-        do_sample with num_return_sequences = N > 1 (resolve_num_return_sequences) returns N independent samples per
-        prompt, [B * N, L + new] with row b*N + i sample i of prompt b, as HF does; the engine loop prefills each prompt
-        once and its N rows share the prompt's KV cache.  With past_key_values it raises NotImplementedError (run it
-        with use_hf_loop=True).
-        return_dict_in_generate with output_scores / output_logits (resolve_outputs) returns, on the engine loop too,
-        transformers' GenerateDecoderOnlyOutput (GenerateBeamDecoderOnlyOutput with beam search: sequences_scores,
+        do_sample with num_return_sequences = N > 1 returns N independent samples per prompt, [B * N, L + new] with row
+        b*N + i sample i of prompt b, as HF does; the engine loop prefills each prompt once and its N rows share the
+        prompt's KV cache.  With past_key_values it raises NotImplementedError (run it with use_hf_loop=True).
+        return_dict_in_generate with output_scores / output_logits returns, on the engine loop too, transformers'
+        GenerateDecoderOnlyOutput (GenerateBeamDecoderOnlyOutput with beam search: sequences_scores,
         beam_indices) with HF's scores / logits, written by the selection and beam kernels inside the graphed step;
         model.compute_transition_scores takes them.  Its past_key_values is the caller's cache when one was passed,
         else None.  output_attentions / output_hidden_states raise NotImplementedError on both loops.
-        prompt_lookup_num_tokens = k (resolve_prompt_lookup; max_matching_ngram_size, default 2), transformers' prompt
-        lookup decoding: on the engine loop each step drafts up to k tokens by copying what followed the earliest
-        earlier occurrence of the sequence's last n-gram in the prompt or the answer, and verifies them in one graphed
+        prompt_lookup_num_tokens = k (max_matching_ngram_size, default 2), transformers' prompt lookup decoding: on
+        the engine loop each step drafts up to k tokens by copying what followed the earliest earlier occurrence of
+        the sequence's last n-gram in the prompt or the answer, and verifies them in one graphed
         decode step over k + 1 rows (engine.LookupDecode), so a repetitive answer takes fewer weight passes.  It runs
         for batch 1 with greedy or temperature / top_k / top_p selection, one eos id or a list, past_key_values and
         host stopping_criteria (called as HF's assisted decoding calls them); the tokens are the plain loop's, up to the
@@ -952,56 +893,63 @@ class SPILlavaMPTForCausalLM(LlamaForCausalLM, _EngineHost):
                 kw['temperature'] = temperature
             return super().generate(input_ids, images=images, bboxes=bboxes, max_new_tokens=max_new_tokens,
                                     do_sample=bool(do_sample), use_cache=True, **kw)
-        gen = {k: v for k, v in kwargs.items() if k not in ('attention_mask', 'pad_token_id', 'past_key_values',
-                                                             'generator', 'tokenizer')}
-        outs = resolve_outputs(self, do_sample, temperature, **gen)
-        stops = resolve_stop_strings(self, kwargs.get('tokenizer'), kwargs.get('stop_strings'),
-                                     kwargs.get('generation_config'))
-        no_outs = dict(return_dict_in_generate=False, output_scores=False, output_logits=False)   # resolved above
-        beam = resolve_beam_search(self, input_ids.shape[1], max_new_tokens, do_sample, eos_token_id=eos_token_id,
-                                   pad_token_id=kwargs.get('pad_token_id'), **dict(gen, **no_outs))
-        if beam is not None:
-            if stopping_criteria is not None:
-                raise NotImplementedError('beam search with stopping_criteria runs on the HF loop only: pass '
-                                          'use_hf_loop=True')
-            if stops is not None:
-                raise NotImplementedError('beam search with stop_strings runs on the HF loop only: pass '
-                                          'use_hf_loop=True')
-            if kwargs.get('past_key_values') is not None:
-                raise NotImplementedError('beam search on a conversation cache (past_key_values) runs on the HF loop '
-                                          'only: pass use_hf_loop=True')
-            eng = self._get_engine(input_ids.device)
-            res = eng.generate(input_ids, images, bboxes, max_new_tokens=beam['max_length'] - input_ids.shape[1],
-                               num_beams=beam['num_beams'], length_penalty=beam['length_penalty'],
-                               early_stopping=beam['early_stopping'], num_return_sequences=beam['num_return_sequences'],
-                               eos_token_id=beam['eos_token_id'], pad_token_id=beam['pad_token_id'],
-                               attention_mask=kwargs.get('attention_mask'), **outs)
-            return _generate_output(res, outs, None) if outs['return_dict_in_generate'] else res
-        nrs = resolve_num_return_sequences(self, do_sample, temperature, **gen)
-        do_sample, temperature, top_k, top_p, procs = resolve_processors(self, input_ids.shape[1], do_sample,
-                                                                         temperature, eos_token_id=eos_token_id, **gen)
+        L = input_ids.shape[1]
+        gen = {k: v for k, v in kwargs.items()
+               if k not in ('attention_mask', 'past_key_values', 'generator', 'tokenizer')}
+        r = resolve_generate(self, L, max_new_tokens, do_sample, temperature, eos_token_id, **gen)
         pkv = kwargs.get('past_key_values')
-        if nrs > 1 and pkv is not None:
+        # refusals, in the order a caller meets them, before an engine is built
+        hf = 'runs on the HF loop only: pass use_hf_loop=True'
+        if r.layer_outputs:
+            raise NotImplementedError(_LAYER_OUTPUTS)
+        if r.stop_strings is not None and kwargs.get('tokenizer') is None:
+            raise ValueError(_STOP_STRINGS_NEED_TOKENIZER)
+        if r.beam is not None:
+            if r.do_sample:
+                raise NotImplementedError('beam search with do_sample (beam sampling) ' + hf)
+            if r.names:
+                raise NotImplementedError('the engine loop applies no logits processor to beam search; %s %s'
+                                          % (', '.join(r.names), hf))
+            if stopping_criteria is not None:
+                raise NotImplementedError('beam search with stopping_criteria ' + hf)
+            if r.stop_strings is not None:
+                raise NotImplementedError('beam search with stop_strings ' + hf)
+            if pkv is not None:
+                raise NotImplementedError('beam search on a conversation cache (past_key_values) ' + hf)
+        elif r.other:
+            raise NotImplementedError('the engine loop applies temperature, top_k, top_p, repetition_penalty, '
+                                      'no_repeat_ngram_size, min_length and min_new_tokens only; %s run on the HF '
+                                      'loop: pass use_hf_loop=True' % ', '.join(r.other))
+        elif r.num_return_sequences > 1 and pkv is not None:
             raise NotImplementedError('several sampled answers per prompt (num_return_sequences=%d) on a conversation '
-                                      'cache (past_key_values) run on the HF loop only: pass use_hf_loop=True' % nrs)
-        lookup, ngram = resolve_prompt_lookup(self, do_sample=do_sample, temperature=temperature, **gen)
+                                      'cache (past_key_values) run on the HF loop only: pass use_hf_loop=True'
+                                      % r.num_return_sequences)
+        outs = r.outputs
+        eng = self._get_engine(input_ids.device)
+        if r.beam is not None:
+            beam = dict(r.beam)
+            res = eng.generate(input_ids, images, bboxes, max_new_tokens=beam.pop('max_length') - L,
+                               attention_mask=kwargs.get('attention_mask'), **beam, **outs)
+            return _generate_output(res, outs, None) if outs['return_dict_in_generate'] else res
+        lookup, ngram = r.lookup
         lk = {} if lookup is None else dict(prompt_lookup_num_tokens=lookup, max_matching_ngram_size=ngram,
                                             streamer=kwargs.get('streamer'))
-        eng = self._get_engine(input_ids.device)
         kv = None
         if pkv is not None:   # a conversation's cache: reused and left holding this turn too
             cache = _find_cache(pkv)
             if cache is None:
-                cache = G4RCache(KVCache(eng.cfg, input_ids.shape[0], input_ids.shape[1] + max_new_tokens, eng.dev))
+                cache = G4RCache(KVCache(eng.cfg, input_ids.shape[0], L + max_new_tokens, eng.dev))
                 pkv._g4r_cache = cache      # ride on HF's Cache object, as the HF loop's prefill does
             cache.stepper = None
             kv = cache.kv
-        res = eng.generate(input_ids, images, bboxes, max_new_tokens=max_new_tokens, do_sample=do_sample,
-                           temperature=temperature, top_k=top_k, top_p=top_p, stopping_criteria=stopping_criteria,
+        procs = r.processors
+        res = eng.generate(input_ids, images, bboxes, max_new_tokens=max_new_tokens, do_sample=r.do_sample,
+                           temperature=r.temperature, top_k=r.top_k, top_p=r.top_p, stopping_criteria=stopping_criteria,
                            eos_token_id=eos_token_id, attention_mask=kwargs.get('attention_mask'),
                            pad_token_id=kwargs.get('pad_token_id'), cache=kv, generator=kwargs.get('generator'),
-                           stop_strings=None if stops is None else stop_strings_from_tokenizer(kwargs['tokenizer'], stops),
-                           num_return_sequences=nrs, repetition_penalty=procs['repetition_penalty'],
+                           stop_strings=None if r.stop_strings is None else
+                           stop_strings_from_tokenizer(kwargs['tokenizer'], r.stop_strings),
+                           num_return_sequences=r.num_return_sequences, repetition_penalty=procs['repetition_penalty'],
                            no_repeat_ngram_size=procs['no_repeat_ngram_size'], min_length=procs['min_length'],
                            min_new_tokens=procs['min_new_tokens'], length_eos_ids=procs['eos_ids'], **outs, **lk)
         return _generate_output(res, outs, pkv) if outs['return_dict_in_generate'] else res
@@ -1009,12 +957,14 @@ class SPILlavaMPTForCausalLM(LlamaForCausalLM, _EngineHost):
     def continuous_batcher(self, slots=8, max_len=2048, tokenizer=None, stop_strings=None, prefix_reuse=False):
         """A ContinuousBatcher (engine.ContinuousBatcher: requests join and leave the graphed decode step one row at a
         time) on this model's engine, with `slots` rows of up to max_len tokens each.  stop_strings (with tokenizer=;
-        resolve_stop_strings, so the model's generation config counts) apply to every request.  Its submit(input_ids,
+        the model's generation config counts, as in generate()) apply to every request.  Its submit(input_ids,
         images=, bboxes=, max_new_tokens=, **generate_kwargs) resolves each request's sampling rule as the engine loop
         of generate() does.  prefix_reuse=True: a request prefills only what no row already holds (a conversation sent
         again whole each turn, several questions on one image); its tokens are then those of
         generate(past_key_values=) on the conversation (engine.ContinuousBatcher)."""
-        stops = resolve_stop_strings(self, tokenizer, stop_strings)
+        stops = resolve_generate(self, 0, None, stop_strings=stop_strings).stop_strings
+        if stops is not None and tokenizer is None:
+            raise ValueError(_STOP_STRINGS_NEED_TOKENIZER)
         eng = self._get_engine(self.device)
         return SeamBatcher(self, ContinuousBatcher(eng, slots, max_len, None if stops is None else
                                                    stop_strings_from_tokenizer(tokenizer, stops),
@@ -1074,7 +1024,7 @@ class SeamBatcher:
     def submit(self, input_ids, images=None, bboxes=None, max_new_tokens=32, do_sample=None, temperature=None,
                eos_token_id=None, generator=None, streamer=None, **generate_kwargs):
         """Queue one request ([1, L] or [L] ids) and return its engine.Request.  do_sample / temperature / top_k /
-        top_p / generation_config resolve as on generate()'s engine loop (resolve_sampling: `do_sample=True` alone
+        top_p / generation_config resolve as on generate()'s engine loop (resolve_generate: `do_sample=True` alone
         samples from the top 50); eos_token_id stops the request as it stops that loop.  As on that loop, only the
         sampling rule (and what is refused below) is read from generation_config: max_new_tokens and eos_token_id are
         this call's arguments.  What the batcher does not run -- logits processors, beam search, several answers per
@@ -1092,19 +1042,26 @@ class SeamBatcher:
         mask = generate_kwargs.get('attention_mask')
         if mask is not None and not bool(torch.as_tensor(mask).bool().all()):
             raise NotImplementedError('a padded prompt: submit its tokens alone, or run it with model.generate')
-        L = torch.as_tensor(input_ids).shape[-1]
-        try:
-            if resolve_num_return_sequences(self.model, do_sample, temperature, **gen) > 1:
-                raise NotImplementedError('num_return_sequences > 1')
-            if resolve_outputs(self.model, do_sample, temperature, **gen)['return_dict_in_generate']:
-                raise NotImplementedError('return_dict_in_generate / output_scores / output_logits')
-            do_sample, temperature, top_k, top_p = resolve_sampling(self.model, L, do_sample, temperature,
-                                                                    eos_token_id=eos_token_id, **gen)
-        except NotImplementedError as e:
+        r = resolve_generate(self.model, torch.as_tensor(input_ids).shape[-1], None, do_sample, temperature,
+                             eos_token_id, **gen)
+        if r.num_return_sequences > 1:
+            why = 'num_return_sequences > 1'
+        elif r.layer_outputs:
+            why = _LAYER_OUTPUTS
+        elif r.outputs['return_dict_in_generate']:
+            why = 'return_dict_in_generate / output_scores / output_logits'
+        elif r.beam is not None:
+            why = 'beam search (num_beams=%d) runs on the HF loop only: pass use_hf_loop=True' % r.beam['num_beams']
+        elif r.names:
+            why = ('the engine loop applies temperature, top_k and top_p only; %s run on the HF loop: pass '
+                   'use_hf_loop=True' % ', '.join(r.names))
+        else:
+            why = None
+        if why is not None:
             raise NotImplementedError('the continuous batcher selects with temperature, top_k and top_p only (%s): run '
-                                      'this request with model.generate' % e) from None
-        return self.batcher.submit(input_ids, images, bboxes, max_new_tokens, do_sample, temperature, top_k, top_p,
-                                   generator, eos_token_id, streamer)
+                                      'this request with model.generate' % why)
+        return self.batcher.submit(input_ids, images, bboxes, max_new_tokens, r.do_sample, r.temperature, r.top_k,
+                                   r.top_p, generator, eos_token_id, streamer)
 
     def step(self):
         return self.batcher.step()

@@ -226,32 +226,37 @@ def test_tie_rule_prefers_lower_flat_index():
 # seam
 # ---------------------------------------------------------------------------------------------
 def test_resolve_beam_search_and_refusals():
-    from gpt4roi_b200.spi_llava import resolve_beam_search, resolve_sampling
-    m = _tiny_model()
+    from transformers import GenerationConfig
+    from gpt4roi_b200.spi_llava import resolve_generate
+    from tests.test_serve_cpu import _seam, _StubEngine
+    m = _seam(_StubEngine())
     m.generation_config.eos_token_id = 2
-    assert resolve_beam_search(m, 10, 8) is None
-    r = resolve_beam_search(m, 10, 8, num_beams=4)
+    assert resolve_generate(m, 10, 8).beam is None
+    r = resolve_generate(m, 10, 8, num_beams=4).beam
     assert r == dict(num_beams=4, length_penalty=1.0, early_stopping=False, num_return_sequences=1, eos_token_id=[2],
                      pad_token_id=2, max_length=18)
-    r = resolve_beam_search(m, 10, 8, num_beams=3, length_penalty=-0.5, early_stopping='never', num_return_sequences=3,
-                            eos_token_id=[5, 6], pad_token_id=0)
+    r = resolve_generate(m, 10, 8, num_beams=3, length_penalty=-0.5, early_stopping='never', num_return_sequences=3,
+                         eos_token_id=[5, 6], pad_token_id=0).beam
     assert (r['length_penalty'], r['early_stopping'], r['num_return_sequences'], r['eos_token_id'], r['pad_token_id']) \
         == (-0.5, 'never', 3, [5, 6], 0)
-    from transformers import GenerationConfig
-    r = resolve_beam_search(m, 10, 8, generation_config=GenerationConfig(num_beams=2, early_stopping=True))
+    r = resolve_generate(m, 10, 8, generation_config=GenerationConfig(num_beams=2, early_stopping=True)).beam
     assert r['num_beams'] == 2 and r['early_stopping'] is True
-    with pytest.raises(NotImplementedError, match='use_hf_loop'):
-        resolve_beam_search(m, 10, 8, num_beams=2, do_sample=True)
-    with pytest.raises(NotImplementedError, match='use_hf_loop'):
-        resolve_beam_search(m, 10, 8, num_beams=2, repetition_penalty=1.3)
-    with pytest.raises(NotImplementedError, match='use_hf_loop'):
-        resolve_beam_search(m, 10, 8, num_beams=2, output_scores=True, return_dict_in_generate=True)
-    with pytest.raises(NotImplementedError, match='use_hf_loop'):
-        resolve_beam_search(m, 10, 8, num_beams=2, no_repeat_ngram_size=2)
+    # the search does not depend on the output flags
+    assert resolve_generate(m, 10, 8, num_beams=2, output_scores=True, return_dict_in_generate=True).beam == \
+        resolve_generate(m, 10, 8, num_beams=2).beam
     with pytest.raises(ValueError):
-        resolve_beam_search(m, 10, 8, num_beams=2, num_return_sequences=3)
+        resolve_generate(m, 10, 8, num_beams=2, num_return_sequences=3)
+    ids = torch.arange(1, 11)[None]
+    m._get_engine = lambda device: pytest.fail('no engine should be built')
+    for bad in (dict(do_sample=True), dict(repetition_penalty=1.3), dict(no_repeat_ngram_size=2)):
+        with pytest.raises(NotImplementedError, match='use_hf_loop'):
+            m.generate(ids, images=torch.zeros(1, 3, 28, 28), max_new_tokens=8, num_beams=2, **bad)
+    # any processor, even a min_length at most the prompt's length
+    with pytest.raises(NotImplementedError, match='MinLengthLogitsProcessor'):
+        m.generate(ids, images=torch.zeros(1, 3, 28, 28), max_new_tokens=8, num_beams=2, min_length=5)
+    m._get_engine = lambda device: _StubEngine()
     with pytest.raises(NotImplementedError, match='num_beams=2'):
-        resolve_sampling(m, 10, num_beams=2)        # unchanged
+        m.continuous_batcher(slots=1, max_len=32).submit(ids, max_new_tokens=2, num_beams=2)
 
 
 def test_engine_loop_refusals():

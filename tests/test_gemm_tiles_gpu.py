@@ -15,6 +15,7 @@ the next.  Each case checks
     (the last two must take the scalar path)."""
 import contextlib
 import re
+import time
 
 import pytest
 import torch
@@ -53,8 +54,10 @@ _KERNEL = re.compile(r'g4r(?:_h)?::gemm_bf16_wgmma<(false|true), (\d), (\d), (\d
 def launched_widths(fn):
     """fn() under the CUDA profiler: returns its result and the set of (CONV, TA, TB, BN) template arguments of the
     gemm_bf16_wgmma kernels it launched (bf16 namespace g4r, fp16 g4r_h).  fn must be repeatable: a trace that
-    comes back without any GEMM kernel is taken once more, because the profiler now and then returns an empty one."""
-    for _ in range(2):
+    comes back without any GEMM kernel is taken again, up to five times in all, because the profiler now and then
+    returns an empty one, sometimes several in a row."""
+    for attempt in range(5):
+        time.sleep(0.05 * attempt)
         with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
             out = fn()
             torch.cuda.synchronize()

@@ -14,35 +14,38 @@ IMG = torch.zeros(3, 3, 4, 4)
 
 def test_resolve_outputs_like_transformers():
     from transformers import GenerationConfig
-    from gpt4roi_b200.spi_llava import resolve_outputs
+    from gpt4roi_b200.spi_llava import resolve_generate
     m = _tiny_model()
+
+    def outputs(**kw):
+        return resolve_generate(m, 3, None, **kw).outputs
     off = dict(return_dict_in_generate=False, output_scores=False, output_logits=False)
-    assert resolve_outputs(m) == off
-    assert resolve_outputs(m, output_scores=True) == off                   # HF: scores only with return_dict_in_generate
-    assert resolve_outputs(m, return_dict_in_generate=True) == dict(off, return_dict_in_generate=True)
-    assert resolve_outputs(m, return_dict_in_generate=True, output_scores=True, output_logits=True) == \
+    assert outputs() == off
+    assert outputs(output_scores=True) == off                   # HF: scores only with return_dict_in_generate
+    assert outputs(return_dict_in_generate=True) == dict(off, return_dict_in_generate=True)
+    assert outputs(return_dict_in_generate=True, output_scores=True, output_logits=True) == \
         dict(return_dict_in_generate=True, output_scores=True, output_logits=True)
     gc = GenerationConfig(return_dict_in_generate=True, output_logits=True)
-    assert resolve_outputs(m, generation_config=gc) == dict(off, return_dict_in_generate=True, output_logits=True)
-    assert resolve_outputs(m, generation_config=gc, return_dict_in_generate=False) == off      # the kwarg first
+    assert outputs(generation_config=gc) == dict(off, return_dict_in_generate=True, output_logits=True)
+    assert outputs(generation_config=gc, return_dict_in_generate=False) == off      # the kwarg first
     m.generation_config.return_dict_in_generate, m.generation_config.output_scores = True, True   # then the model's
-    assert resolve_outputs(m) == dict(off, return_dict_in_generate=True, output_scores=True)
+    assert outputs() == dict(off, return_dict_in_generate=True, output_scores=True)
+    assert not resolve_generate(m, 3, None).layer_outputs
+    m._get_engine = lambda device: pytest.fail('no engine should be built')
     for bad in (dict(output_attentions=True), dict(output_hidden_states=True)):
+        assert resolve_generate(m, 3, None, return_dict_in_generate=True, **bad).layer_outputs
         with pytest.raises(NotImplementedError, match='not materialised'):
-            resolve_outputs(m, return_dict_in_generate=True, **bad)
+            m.generate(torch.tensor([[1, 5, 9]]), images=IMG[:1], max_new_tokens=4, return_dict_in_generate=True, **bad)
 
 
 def test_beam_search_outputs_resolve_at_generate_only():
-    """resolve_beam_search resolves the search alone and still refuses output flags; generate() resolves them with
-    resolve_outputs and gets the same search, whether the flags come as kwargs, in generation_config= or in the
+    """generate() gets the same search whether the output flags come as kwargs, in generation_config= or in the
     model's config."""
     from transformers import GenerationConfig
-    from gpt4roi_b200.spi_llava import resolve_beam_search
+    from gpt4roi_b200.spi_llava import resolve_generate
     m = _tiny_model().eval()
     m.generation_config.eos_token_id = 2
-    base = resolve_beam_search(m, 3, 4, num_beams=2)
-    with pytest.raises(NotImplementedError, match='resolve_outputs'):
-        resolve_beam_search(m, 3, 4, num_beams=2, return_dict_in_generate=True, output_scores=True)
+    base = resolve_generate(m, 3, 4, num_beams=2).beam
     calls = []
 
     class _Engine:

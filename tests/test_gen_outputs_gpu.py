@@ -1,6 +1,8 @@
 """GPU tests of generate()'s return_dict_in_generate outputs: the scores and logits the selection kernel
 (csrc/sample.cu, g4r_sample_tokens_out_*) and the beam kernels (csrc/beam.cu, g4r_beam_step_out_*) write inside the
 graphed step, against transformers' own processors and loops."""
+import time
+
 import numpy as np
 import pytest
 import torch
@@ -127,12 +129,20 @@ def test_no_output_launches_the_same_kernels(rows):
     hist = _history(4, 48, seed=1).to(DEV)
 
     def names(fn):
-        torch.cuda.synchronize()
-        with profile(activities=[ProfilerActivity.CUDA]) as prof:
-            for _ in range(3):
-                fn()
+        """The selection kernels fn launches.  Every fn here launches one, so an empty trace is the profiler's (it now
+        and then returns one, sometimes several in a row): it is taken again, up to five times in all."""
+        for attempt in range(5):
+            time.sleep(0.05 * attempt)
             torch.cuda.synchronize()
-        return sorted({e.name for e in prof.events() if e.device_type.name == 'CUDA' and 'sample_tokens' in e.name})
+            with profile(activities=[ProfilerActivity.CUDA]) as prof:
+                for _ in range(3):
+                    fn()
+                torch.cuda.synchronize()
+            found = sorted({e.name for e in prof.events()
+                            if e.device_type.name == 'CUDA' and 'sample_tokens' in e.name})
+            if found:
+                break
+        return found
     out = torch.empty(4, 1, dtype=torch.int64, device=DEV)
     rng = torch.zeros(1, dtype=torch.int64, device=DEV)
     names(lambda: kernels.sample_tokens(lg, out, True))     # the profiler's first session starts its tracer

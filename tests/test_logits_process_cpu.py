@@ -232,8 +232,11 @@ def _hf_history_processors(m, L, **kw):
 
 def test_seam_resolves_the_processors_like_transformers():
     from transformers import GenerationConfig
-    from gpt4roi_b200.spi_llava import resolve_processors
+    from gpt4roi_b200.spi_llava import resolve_generate
     m = _tiny_model()
+
+    def resolved(**kw):
+        return resolve_generate(m, 7, None, **kw)
     eos_model = m.generation_config.eos_token_id
     assert eos_model is not None
     cases = [dict(), dict(repetition_penalty=1.3), dict(no_repeat_ngram_size=3, min_new_tokens=8),
@@ -241,44 +244,48 @@ def test_seam_resolves_the_processors_like_transformers():
              dict(generation_config=GenerationConfig(repetition_penalty=1.1, no_repeat_ngram_size=2, min_length=4)),
              dict(generation_config=GenerationConfig(repetition_penalty=1.1), repetition_penalty=1.4)]
     for kw in cases:
-        got = resolve_processors(m, 7, **kw)[4]
+        got = resolved(**kw).processors
         assert got == _hf_history_processors(m, 7, **kw), kw
     # min_new_tokens takes precedence over min_length, as in HF's generate: min_length = min_new_tokens + L
-    both = resolve_processors(m, 7, min_length=30, min_new_tokens=3)[4]
+    both = resolved(min_length=30, min_new_tokens=3).processors
     assert both['min_length'] == 10 and both['min_new_tokens'] == 3
     assert both == _hf_history_processors(m, 7, min_length=30, min_new_tokens=3)
     # min_new_tokens=0 (HF: min_length = L) and min_length <= L suppress nothing: neutral, no processed kernel
     for kw in (dict(min_new_tokens=0), dict(min_length=7), dict(min_length=30, min_new_tokens=0)):
-        got = resolve_processors(m, 7, **kw)[4]
+        got = resolved(**kw).processors
         assert got['min_length'] == 0 and got['min_new_tokens'] == 0 and got == _hf_history_processors(m, 7, **kw), kw
     # the eos list from the model's config when the caller gives none
-    assert resolve_processors(m, 7, min_new_tokens=3)[4]['eos_ids'] == [eos_model]
-    assert resolve_processors(m, 7, min_new_tokens=3, eos_token_id=9)[4]['eos_ids'] == [9]
+    assert resolved(min_new_tokens=3).processors['eos_ids'] == [eos_model]
+    assert resolved(min_new_tokens=3, eos_token_id=9).processors['eos_ids'] == [9]
     # then the model's generation config
     m.generation_config.repetition_penalty, m.generation_config.no_repeat_ngram_size = 1.2, 4
-    got = resolve_processors(m, 7, do_sample=True, temperature=0.5)
-    assert got[:4] == (True, 0.5, 50, 1.0) and got[4]['repetition_penalty'] == pytest.approx(1.2)
-    assert got[4]['no_repeat_ngram_size'] == 4
-    assert resolve_processors(m, 7, repetition_penalty=1.0)[4]['repetition_penalty'] == 1.0
+    got = resolved(do_sample=True, temperature=0.5)
+    assert got[:4] == (True, 0.5, 50, 1.0) and got.processors['repetition_penalty'] == pytest.approx(1.2)
+    assert got.processors['no_repeat_ngram_size'] == 4
+    assert resolved(repetition_penalty=1.0).processors['repetition_penalty'] == 1.0
 
 
 def test_seam_refusals():
     from transformers.generation.logits_process import LogitsProcessor, LogitsProcessorList
-    from gpt4roi_b200.spi_llava import resolve_processors, resolve_sampling
+    from tests.test_serve_cpu import _seam, _StubEngine
 
     class Mine(LogitsProcessor):
         def __call__(self, input_ids, scores):
             return scores
-    m = _tiny_model()
+    m = _seam(_StubEngine())
+    sb = m.continuous_batcher(slots=1, max_len=16)
+    m._get_engine = lambda device: pytest.fail('no engine should be built')
+    ids = torch.tensor([[1, 2, 3, 4, 5]])
     for bad in (dict(min_p=0.1), dict(typical_p=0.5), dict(epsilon_cutoff=1e-3), dict(eta_cutoff=1e-3),
                 dict(bad_words_ids=[[5]]), dict(suppress_tokens=[5]), dict(sequence_bias={(5,): 1.0}),
                 dict(logits_processor=LogitsProcessorList([Mine()])), dict(num_beams=2)):
         with pytest.raises(NotImplementedError, match='use_hf_loop=True'):
-            resolve_processors(m, 5, do_sample=True, temperature=0.7, repetition_penalty=1.2, **bad)
-    # resolve_sampling keeps refusing the history-dependent ones
+            m.generate(ids, images=torch.zeros(1, 3, 28, 28), max_new_tokens=4, do_sample=True, temperature=0.7,
+                       repetition_penalty=1.2, **bad)
+    # the continuous batcher refuses the history-dependent ones too
     for bad in (dict(repetition_penalty=1.1), dict(no_repeat_ngram_size=3), dict(min_new_tokens=2)):
         with pytest.raises(NotImplementedError, match='use_hf_loop=True'):
-            resolve_sampling(m, 5, do_sample=True, **bad)
+            sb.submit(ids, max_new_tokens=2, do_sample=True, **bad)
 
 
 def test_seam_routes_the_processors_to_the_engine_loop():

@@ -115,6 +115,47 @@ def test_hf_generate_loop_drives_the_seam_with_our_cache():
     assert [c[2] for c in stub.calls[1:]] == [3, 4, 5]           # cache length seen by each decode step
 
 
+def test_engine_loop_resolves_each_call_once():
+    """The engine loop's generate() and the batcher's submit() resolve a call's generation config once and build HF's
+    processor list at most once, whatever the call asks for."""
+    from tests.stop_tokenizer import seeded_tokenizer
+    from tests.test_serve_cpu import _seam, _StubEngine as _ServeStub
+    m = _seam(_ServeStub())
+    sb = m.continuous_batcher(slots=1, max_len=16)
+    calls = []
+
+    class _Engine:
+        def generate(self, input_ids, images, bboxes, **kw):
+            calls.append(kw)
+            res = dict(sequences=input_ids, scores=None, logits=None, sequences_scores=None,
+                       beam_indices=torch.zeros(1, 1, dtype=torch.int32))
+            return res if kw['return_dict_in_generate'] else input_ids
+    m._get_engine = lambda device: _Engine()
+    counts = dict(config=0, processors=0)
+
+    def counted(name, key):
+        orig = getattr(m, name)
+
+        def f(*a, **kw):
+            counts[key] += 1
+            return orig(*a, **kw)
+        setattr(m, name, f)
+    counted('_prepare_generation_config', 'config')
+    counted('_get_logits_processor', 'processors')
+    ids = torch.tensor([[1, 5, 9]])
+    tok = seeded_tokenizer(140, seed=1)
+    for kw in (dict(), dict(do_sample=True, temperature=0.7), dict(num_beams=2), dict(prompt_lookup_num_tokens=3),
+               dict(stop_strings='###', tokenizer=tok), dict(return_dict_in_generate=True, output_scores=True)):
+        counts.update(config=0, processors=0)
+        m.generate(ids, images=torch.zeros(1, 3, 28, 28), max_new_tokens=4, **kw)
+        assert counts['config'] == 1 and counts['processors'] <= 1, (kw, counts)
+    assert len(calls) == 6
+    for kw in (dict(), dict(do_sample=True, top_k=5)):
+        counts.update(config=0, processors=0)
+        sb.submit(ids, max_new_tokens=2, **kw)
+        assert counts['config'] == 1 and counts['processors'] <= 1, (kw, counts)
+
+
 def test_prepare_inputs_for_generation_follows_reference():
     from gpt4roi_b200.engine import EngineConfig, KVCache
     from gpt4roi_b200.spi_llava import G4RCache

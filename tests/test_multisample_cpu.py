@@ -119,24 +119,28 @@ def test_engine_refusals():
 
 def test_seam_resolves_num_return_sequences_like_transformers():
     from transformers import GenerationConfig
-    from gpt4roi_b200.spi_llava import resolve_num_return_sequences, resolve_sampling
+    from gpt4roi_b200.spi_llava import resolve_generate
     m = _tiny_model()
-    assert resolve_num_return_sequences(m) == 1
-    assert resolve_num_return_sequences(m, do_sample=True, num_return_sequences=3) == 3
+
+    def nrs(**kw):
+        return resolve_generate(m, 5, None, **kw).num_return_sequences
+    assert nrs() == 1
+    assert nrs(do_sample=True, num_return_sequences=3) == 3
     gc = GenerationConfig(do_sample=True, num_return_sequences=4)
-    assert resolve_num_return_sequences(m, generation_config=gc) == 4
-    assert resolve_num_return_sequences(m, generation_config=gc, num_return_sequences=2) == 2     # explicit kwarg first
+    assert nrs(generation_config=gc) == 4
+    assert nrs(generation_config=gc, num_return_sequences=2) == 2     # explicit kwarg first
     m.generation_config.do_sample, m.generation_config.num_return_sequences = True, 5            # then the model's config
-    assert resolve_num_return_sequences(m) == 5
-    assert resolve_num_return_sequences(m, generation_config=gc) == 4
+    assert nrs() == 5
+    assert nrs(generation_config=gc) == 4
     m.generation_config.do_sample, m.generation_config.num_return_sequences = False, 1
     # sampling parameters resolve as before
-    assert resolve_sampling(m, 5, do_sample=True, temperature=0.7, num_return_sequences=3) == (True, 0.7, 50, 1.0)
-    # greedy with N > 1: HF's own ValueError, at both resolvers and through generate
+    assert resolve_generate(m, 5, None, do_sample=True, temperature=0.7, num_return_sequences=3)[:4] == \
+        (True, 0.7, 50, 1.0)
+    # greedy with N > 1: HF's own ValueError, at the resolution and through generate
     with pytest.raises(ValueError, match='num_return_sequences'):
-        resolve_num_return_sequences(m, do_sample=False, num_return_sequences=2)
+        nrs(do_sample=False, num_return_sequences=2)
     with pytest.raises(ValueError, match='num_return_sequences'):
-        resolve_sampling(m, 5, num_return_sequences=2)
+        nrs(num_return_sequences=2)
     m._get_engine = lambda device: pytest.fail('no engine should be built')
     with pytest.raises(ValueError, match='num_return_sequences'):
         m.generate(torch.tensor([[1, 5, 9]]), images=torch.zeros(1, 3, 28, 28), num_return_sequences=2)
@@ -159,7 +163,7 @@ def test_seam_routes_samples_to_the_engine_and_beams_unchanged():
     assert calls[-1]['temperature'] == 0.7 and calls[-1]['top_k'] == 50 and calls[-1]['cache'] is None
     m.generate(ids, images=img, max_new_tokens=4, do_sample=True)
     assert calls[-1]['num_return_sequences'] == 1
-    # num_beams > 1 still goes to beam search, its num_return_sequences from resolve_beam_search
+    # num_beams > 1 still goes to beam search, its num_return_sequences from the beam resolution
     m.generate(ids, images=img, max_new_tokens=4, num_beams=3, num_return_sequences=2)
     assert calls[-1]['num_beams'] == 3 and calls[-1]['num_return_sequences'] == 2 and 'do_sample' not in calls[-1]
     n = len(calls)

@@ -128,22 +128,29 @@ def test_kept_set_restatement_equals_transformers(dtype):
 
 def test_seam_resolves_sampling_like_transformers():
     from transformers import GenerationConfig
-    from gpt4roi_b200.spi_llava import resolve_sampling
-    m = _tiny_model()
+    from gpt4roi_b200.spi_llava import resolve_generate
+    from tests.test_serve_cpu import _seam, _StubEngine
+    m = _seam(_StubEngine())
+
+    def rule(**kw):
+        return resolve_generate(m, 5, kw.pop('max_new_tokens', None), **kw)[:4]
     # gpt4roi/app.py:293-300: do_sample=True, temperature=0.2 and no top_k -> HF's global default top_k=50
-    assert resolve_sampling(m, 5, do_sample=True, temperature=0.2, max_new_tokens=1024) == (True, 0.2, 50, 1.0)
-    assert resolve_sampling(m, 5, do_sample=True, temperature=0.2, top_k=0, top_p=0.9) == (True, 0.2, 0, 0.9)
+    assert rule(do_sample=True, temperature=0.2, max_new_tokens=1024) == (True, 0.2, 50, 1.0)
+    assert rule(do_sample=True, temperature=0.2, top_k=0, top_p=0.9) == (True, 0.2, 0, 0.9)
     gc = GenerationConfig(do_sample=True, temperature=0.7, top_k=20, top_p=0.8)
-    assert resolve_sampling(m, 5, generation_config=gc) == (True, 0.7, 20, 0.8)
-    assert resolve_sampling(m, 5, generation_config=gc, top_k=5) == (True, 0.7, 5, 0.8)     # explicit kwargs first
-    m.generation_config.top_p = 0.95                                                           # then the model's config
-    assert resolve_sampling(m, 5, do_sample=True) == (True, 1.0, 50, 0.95)
-    assert resolve_sampling(m, 5, generation_config=gc) == (True, 0.7, 20, 0.8)
-    assert resolve_sampling(m, 5, do_sample=False, temperature=0.2, top_k=3) == (False, 1.0, 0, 1.0)
-    assert resolve_sampling(m, 5) == (False, 1.0, 0, 1.0)
+    assert rule(generation_config=gc) == (True, 0.7, 20, 0.8)
+    assert rule(generation_config=gc, top_k=5) == (True, 0.7, 5, 0.8)     # explicit kwargs first
+    m.generation_config.top_p = 0.95                                        # then the model's config
+    assert rule(do_sample=True) == (True, 1.0, 50, 0.95)
+    assert rule(generation_config=gc) == (True, 0.7, 20, 0.8)
+    assert rule(do_sample=False, temperature=0.2, top_k=3) == (False, 1.0, 0, 1.0)
+    assert rule() == (False, 1.0, 0, 1.0)
+    # the batcher runs the three warpers only
+    sb = m.continuous_batcher(slots=1, max_len=16)
+    ids = torch.tensor([[1, 2, 3, 4, 5]])
     for bad in (dict(repetition_penalty=1.1), dict(min_p=0.1), dict(num_beams=2), dict(typical_p=0.5),
                 dict(no_repeat_ngram_size=3)):
         with pytest.raises(NotImplementedError, match='use_hf_loop=True'):
-            resolve_sampling(m, 5, do_sample=True, temperature=0.2, **bad)
+            sb.submit(ids, max_new_tokens=2, do_sample=True, temperature=0.2, **bad)
     with pytest.raises(NotImplementedError, match='use_hf_loop=True'):
-        resolve_sampling(m, 5, do_sample=False, repetition_penalty=1.1)
+        sb.submit(ids, max_new_tokens=2, do_sample=False, repetition_penalty=1.1)

@@ -167,19 +167,23 @@ def test_host_stopping_criteria_still_fire_beside_stop_strings():
 
 def test_seam_resolves_stop_strings_like_transformers():
     from transformers import GenerationConfig
-    from gpt4roi_b200.spi_llava import resolve_stop_strings, stop_strings_from_tokenizer
+    from gpt4roi_b200.spi_llava import resolve_generate, stop_strings_from_tokenizer
     m = _tiny_model()
     tok = seeded_tokenizer(120, seed=1)
-    assert resolve_stop_strings(m) is None and resolve_stop_strings(m, tok) is None
-    assert resolve_stop_strings(m, tok, stop_strings='###') == ('###',)
+
+    def stops(**kw):
+        return resolve_generate(m, 3, None, **kw).stop_strings
+    assert stops() is None
+    assert stops(stop_strings='###') == ('###',)
     gc = GenerationConfig(stop_strings=['ab', '#'])
-    assert resolve_stop_strings(m, tok, generation_config=gc) == ('ab', '#')
-    assert resolve_stop_strings(m, tok, stop_strings=['y.'], generation_config=gc) == ('y.',)     # explicit kwarg first
-    m.generation_config.stop_strings = ['abab']                                                  # then the model's config
-    assert resolve_stop_strings(m, tok) == ('abab',)
-    assert resolve_stop_strings(m, tok, generation_config=gc) == ('ab', '#')
+    assert stops(generation_config=gc) == ('ab', '#')
+    assert stops(stop_strings=['y.'], generation_config=gc) == ('y.',)     # explicit kwarg first
+    m.generation_config.stop_strings = ['abab']                           # then the model's config
+    assert stops() == ('abab',)
+    assert stops(generation_config=gc) == ('ab', '#')
+    m._get_engine = lambda device: pytest.fail('no engine should be built')
     with pytest.raises(ValueError, match='could not locate a tokenizer'):
-        resolve_stop_strings(m)
+        m.generate(torch.tensor([[1, 5, 9]]), images=torch.zeros(1, 3, 28, 28), max_new_tokens=4)
     built = stop_strings_from_tokenizer(tok, ['###'])
     assert built is stop_strings_from_tokenizer(tok, '###') and built.V_tok == 120
     assert built.table is StopStrings(clean_strings(tok), ['###']).table
