@@ -63,6 +63,7 @@
 #define g4r_sample_tokens_proc_bf16 g4r_sample_tokens_proc_f16
 #define g4r_sample_tokens_out_bf16 g4r_sample_tokens_out_f16
 #define g4r_sample_tokens_rows_bf16 g4r_sample_tokens_rows_f16
+#define g4r_sample_tokens_rows_proc_bf16 g4r_sample_tokens_rows_proc_f16
 #define g4r_decode_attention_beam_bf16 g4r_decode_attention_beam_f16
 #define g4r_decode_attention_group_bf16 g4r_decode_attention_group_f16
 #define g4r_beam_step_bf16 g4r_beam_step_f16

@@ -194,7 +194,8 @@ __device__ __forceinline__ int list_owner(unsigned long long e) {
 template <bool OUT>
 __device__ void select_processed(const unsigned short* __restrict__ row, int V, float temperature, int top_k,
                                  float top_p, int greedy, unsigned long long seed, const long long* __restrict__ rng_step,
-                                 const SampleProc& pr, const SampleOut& out, unsigned* smem, int& s_tok) {
+                                 const SampleProc& pr, const SampleOut& out, unsigned* smem, int& s_tok,
+                                 unsigned rng_row) {
   __shared__ unsigned long long s_best[32];
   __shared__ int s_int[32];
   __shared__ float s_flt[32];
@@ -416,7 +417,7 @@ __device__ void select_processed(const unsigned short* __restrict__ row, int V, 
   __syncthreads();
   // ---- inverse CDF over the kept groups, from the top; a thread with kept groups takes it when rounding leaves the
   // target past every thread's inclusive mass
-  const uint4 r = philox4x32_10(make_uint4((unsigned)step, (unsigned)((unsigned long long)step >> 32), (unsigned)b, 0u),
+  const uint4 r = philox4x32_10(make_uint4((unsigned)step, (unsigned)((unsigned long long)step >> 32), rng_row, 0u),
                                 make_uint2((unsigned)seed, (unsigned)(seed >> 32)));
   const float target = (float)(r.x >> 8) * 0x1p-24f * s_zk;
   if (tid == 0) {
@@ -485,8 +486,8 @@ __device__ void select_processed(const unsigned short* __restrict__ row, int V, 
     });
 }
 
-// rng_row: the row word of the plain selection's Philox counter -- blockIdx.x for a batch, 0 for the per-row kernel,
-// whose rows each draw as a batch of one would.
+// rng_row: the row word of the Philox counter -- blockIdx.x for a batch, 0 for the per-row kernels, whose rows each
+// draw as a batch of one would.
 template <bool PROC, bool OUT>
 __device__ __forceinline__ void sample_row(const unsigned short* __restrict__ logits, long long ld, int V,
                                            float temperature, int top_k, float top_p, int greedy,
@@ -503,7 +504,7 @@ __device__ __forceinline__ void sample_row(const unsigned short* __restrict__ lo
   const unsigned short* row = logits + (long long)b * ld;
 
   if constexpr (PROC) {
-    select_processed<OUT>(row, V, temperature, top_k, top_p, greedy, seed, rng_step, proc, out, hist, s_tok);
+    select_processed<OUT>(row, V, temperature, top_k, top_p, greedy, seed, rng_step, proc, out, hist, s_tok, rng_row);
   } else if (greedy) {
     // arg-max, first index among equals (torch.argmax)
     unsigned long long best = 0;
@@ -708,20 +709,51 @@ sample_tokens_out_kernel(const unsigned short* __restrict__ logits, long long ld
                          out_ids, proc, out, blockIdx.x);
 }
 
+// The per-row processors of g4r_sample_tokens_rows_proc_*: row r's SampleProc comes from entry r of each array.
+struct SampleProcRows {
+  long long* hist;              // int64 [S, ld_h]: row r's submitted prompt, then its new tokens
+  long long ld_h;
+  const int* prompt_len;        // [S]
+  const float* penalty;         // [S], 1: off
+  const int* ngram;             // [S], 0: off
+  const int* min_length;        // [S]
+  const int* min_new_tokens;    // [S]
+  const int* eos_ids;           // [S, PROC_ROW_EOS]: the ids min_length / min_new_tokens suppress
+  const int* n_eos;             // [S]
+};
+constexpr int PROC_ROW_EOS = 4;
+
 // The per-row kernel (g4r_sample_tokens_rows_*): the decode step of a continuous batch, whose rows are independent
 // requests.  Row r runs the plain selection on its own rule, seed and counter step[r]; an inactive row returns before
 // any work.  `lens` is the step's last write: the decode kernels of the same step have read it already.
+// PROC (g4r_sample_tokens_rows_proc_*): a row whose processors are not all neutral runs the processed selection on its
+// history h[r, 0 .. prompt_len[r] + step[r]) and appends its token there; a neutral row runs the plain body, so it
+// selects bitwise as the PROC = false instance does.
+template <bool PROC>
 __global__ void __launch_bounds__(SAMPLE_THREADS, 1)
 sample_tokens_rows_kernel(const unsigned short* __restrict__ logits, long long ld, int V, const int* __restrict__ greedy,
                           const float* __restrict__ temperature, const int* __restrict__ top_k,
                           const float* __restrict__ top_p, const unsigned long long* __restrict__ seed,
                           long long* __restrict__ step, const int* __restrict__ eos_id, const int* __restrict__ active,
-                          int* __restrict__ finished, long long* __restrict__ out_ids, int* __restrict__ lens) {
+                          int* __restrict__ finished, long long* __restrict__ out_ids, int* __restrict__ lens,
+                          SampleProcRows rp) {
   const int r = blockIdx.x;
   if (!active[r]) return;   // uniform over the CTA
-  sample_row<false, false>(logits, ld, V, temperature[r], top_k[r], top_p[r], greedy[r], seed[r], step + r, -1, -1,
-                           nullptr, out_ids, SampleProc{}, SampleOut{}, 0u);
-  if (threadIdx.x == 0) {   // the thread that wrote out_ids[r]
+  if constexpr (PROC) {
+    const SampleProc pr{rp.hist, rp.ld_h, rp.prompt_len[r], rp.penalty[r], rp.ngram[r], rp.min_length[r],
+                        rp.min_new_tokens[r], rp.eos_ids + (long long)r * PROC_ROW_EOS, rp.n_eos[r], 1};
+    const bool neutral = pr.penalty == 1.f && pr.ngram == 0 && !((pr.min_length || pr.min_new_tokens) && pr.n_eos);
+    if (neutral)   // uniform over the CTA
+      sample_row<false, false>(logits, ld, V, temperature[r], top_k[r], top_p[r], greedy[r], seed[r], step + r, -1, -1,
+                               nullptr, out_ids, SampleProc{}, SampleOut{}, 0u);
+    else
+      sample_row<true, false>(logits, ld, V, temperature[r], top_k[r], top_p[r], greedy[r], seed[r], step + r, -1, -1,
+                              nullptr, out_ids, pr, SampleOut{}, 0u);
+  } else {
+    sample_row<false, false>(logits, ld, V, temperature[r], top_k[r], top_p[r], greedy[r], seed[r], step + r, -1, -1,
+                             nullptr, out_ids, SampleProc{}, SampleOut{}, 0u);
+  }
+  if (threadIdx.x == 0) {   // the thread that wrote out_ids[r] (and appended it to the history)
     const long long tok = out_ids[r];
     if (eos_id[r] >= 0 && tok == eos_id[r]) finished[r] = 1;
     step[r] += 1;
@@ -832,15 +864,53 @@ extern "C" int g4r_sample_tokens_rows_bf16(const void* logits, long long ld, int
   cudaStream_t st = (cudaStream_t)stream;
   static bool set = false;
   if (!set) {
-    G4R_CUDA(cudaFuncSetAttribute(sample_tokens_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    G4R_CUDA(cudaFuncSetAttribute(sample_tokens_rows_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                   (int)SAMPLE_SMEM));
     set = true;
   }
   // the sampling amount always: which rows sample is device data, and a captured launch serves every later admission
-  sample_tokens_rows_kernel<<<S, SAMPLE_THREADS, SAMPLE_SMEM, st>>>(
+  sample_tokens_rows_kernel<false><<<S, SAMPLE_THREADS, SAMPLE_SMEM, st>>>(
       (const unsigned short*)logits, ld, V, greedy, temperature, top_k, top_p, seed, step, eos_id, active, finished,
-      out_ids, lens);
+      out_ids, lens, SampleProcRows{});
   G4R_LAUNCH_CHECK("sample_tokens_rows");
+  return G4R_OK;
+}
+
+extern "C" int g4r_sample_tokens_rows_proc_bf16(const void* logits, long long ld, int S, int V, const int* greedy,
+                                                const float* temperature, const int* top_k, const float* top_p,
+                                                const unsigned long long* seed, long long* step, const int* eos_id,
+                                                const int* active, int* finished, long long* out_ids, int* lens,
+                                                long long* history, long long ld_h, const int* prompt_len,
+                                                const float* repetition_penalty, const int* no_repeat_ngram_size,
+                                                const int* min_length, const int* min_new_tokens, const int* eos_ids,
+                                                const int* n_eos, void* stream) {
+  G4R_REQUIRE(logits && out_ids && S > 0 && V > 0 && V < 65536 && ld >= V,
+              "sample_tokens_rows_proc: bad arguments (S=%d V=%d ld=%lld; V < 65536)", S, V, ld);
+  G4R_REQUIRE(greedy && temperature && top_k && top_p && seed && step && eos_id && active && finished,
+              "sample_tokens_rows_proc: every per-row array but lens is required");
+  G4R_REQUIRE(history && ld_h >= 1 && prompt_len && repetition_penalty && no_repeat_ngram_size && min_length &&
+                  min_new_tokens && eos_ids && n_eos,
+              "sample_tokens_rows_proc: the history (ld_h=%lld >= 1) and every per-row processor array are required",
+              ld_h);
+  const long long listed = ld_h < PROC_LIST_MAX ? ld_h : PROC_LIST_MAX;
+  long long list_n = 1;
+  while (list_n < listed) list_n <<= 1;
+  // the largest amount always: which rows sample, and which carry a penalty, is device data
+  const size_t smem = SAMPLE_SMEM + 2 * sizeof(unsigned) * ((V + 31) / 32) + list_n * sizeof(unsigned long long);
+  cudaStream_t st = (cudaStream_t)stream;
+  static bool set = false;
+  if (!set) {
+    const size_t most = SAMPLE_SMEM + 2 * sizeof(unsigned) * 2048 + PROC_LIST_MAX * sizeof(unsigned long long);
+    G4R_CUDA(cudaFuncSetAttribute(sample_tokens_rows_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                  (int)most));
+    set = true;
+  }
+  const SampleProcRows rp{history, ld_h, prompt_len, repetition_penalty, no_repeat_ngram_size, min_length,
+                          min_new_tokens, eos_ids, n_eos};
+  sample_tokens_rows_kernel<true><<<S, SAMPLE_THREADS, smem, st>>>(
+      (const unsigned short*)logits, ld, V, greedy, temperature, top_k, top_p, seed, step, eos_id, active, finished,
+      out_ids, lens, rp);
+  G4R_LAUNCH_CHECK("sample_tokens_rows_proc");
   return G4R_OK;
 }
 

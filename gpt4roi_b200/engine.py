@@ -1632,14 +1632,17 @@ class Request:
     HF's layout) grows by one token per step while it runs; `done` turns True when it retires -- it emitted its eos id,
     ended a stop string, or has max_new_tokens new tokens -- or when its admission failed: `error` is then the exception,
     which ContinuousBatcher.step() raised, and the request has no new tokens.  `reused`: how many prompt tokens its
-    admission took from K/V a batcher row already held (ContinuousBatcher(prefix_reuse=True)); 0 for a full prefill."""
+    admission took from K/V a batcher row already held (ContinuousBatcher(prefix_reuse=True)); 0 for a full prefill.
+    `processors` (ContinuousBatcher(request_options=True)): the request's repetition_penalty, no_repeat_ngram_size,
+    min_length, min_new_tokens and length_eos_ids, None when all are neutral; `stops`: its own StopStrings or None."""
 
     def __init__(self, input_ids, images, bboxes, max_new_tokens, greedy, temperature, top_k, top_p, seed, eos_id,
-                 streamer):
+                 streamer, processors=None, stops=None):
         self.input_ids, self.images, self.bboxes = input_ids, images, bboxes
         self.max_new_tokens = max_new_tokens
         self.greedy, self.temperature, self.top_k, self.top_p, self.seed = greedy, temperature, top_k, top_p, seed
         self.eos_id, self.streamer = eos_id, streamer
+        self.processors, self.stops = processors, stops
         self.tokens = []
         self.done = False
         self.error = None
@@ -1688,9 +1691,18 @@ class ContinuousBatcher:
     taken never-used first, then least recently retired, so held conversations live as long as they can.  The requests
     of a step that reuse a prefix are prefilled together by one chunk prefill (PrefillEngine.extend on a row view of
     the cache).  A reused request's tokens are those of that chunk prefill -- generate(cache=) on the conversation --
-    not those of a full prefill, and may depend on what the row held: the caller opts into that."""
+    not those of a full prefill, and may depend on what the row held: the caller opts into that.
 
-    def __init__(self, engine, slots, max_len, stop_strings=None, prefix_reuse=False):
+    request_options=True: each request may also carry transformers' history-dependent logits processors
+    (repetition_penalty, no_repeat_ngram_size, min_length, min_new_tokens) and its own stop strings, as generate() runs
+    them for a batch of one.  The graph then ends with kernels.sample_tokens_rows_processed, reading each row's
+    processors and its history -- int64 [slots, max_len], row s the whole submitted prompt (under prefix reuse too,
+    the part taken from the cache included), then the request's new tokens -- and kernels.stop_step_rows, reading each
+    row's own stop table.  A request's StopStrings replaces the batcher's for its row; every table must have the
+    batcher's V_tok (that of `stop_strings`, else the engine's vocabulary).  A row whose processors are all neutral
+    selects exactly as on a batcher without the option.  The choice is made once, here: one graph per batcher."""
+
+    def __init__(self, engine, slots, max_len, stop_strings=None, prefix_reuse=False, request_options=False):
         if slots < 1 or max_len < 2:
             raise ValueError('ContinuousBatcher needs slots >= 1 and max_len >= 2 (got %d, %d)' % (slots, max_len))
         if prefix_reuse and engine.cfg.head_dim != 128:
@@ -1718,6 +1730,18 @@ class ContinuousBatcher:
         self.stops = stop_strings
         self.stop_table = None if stop_strings is None else stop_strings.on(dev)
         self.stop_state = vec(0, torch.int32)
+        self.request_options = bool(request_options)
+        if self.request_options:
+            # the per-row processors and stop tables that kernels.sample_tokens_rows_processed / stop_step_rows read
+            self.history = torch.zeros((S, self.max_len), dtype=torch.int64, device=dev)
+            self.prompt_len, self.penalty = vec(0, torch.int32), vec(1.0, torch.float32)
+            self.ngram, self.min_length, self.min_new_tokens = (vec(0, torch.int32) for _ in range(3))
+            self.length_eos = torch.zeros((S, kernels.PROC_ROW_EOS), dtype=torch.int32, device=dev)
+            self.n_length_eos = vec(0, torch.int32)
+            self.V_tok = engine.cfg.vocab if stop_strings is None else stop_strings.V_tok
+            self.row_tables, self.row_states = vec(0, torch.int64), vec(1, torch.int32)
+            self.row_stops = [None] * S     # each running row's table: the graph reads it through row_tables
+            self.row_procs = [None] * S     # each running row's processors (the host stand-in restates them)
         self.ids = torch.zeros((S, 1), dtype=torch.int64, device=dev)     # the decode step's input: each row's last token
         self.pos = torch.zeros(1, dtype=torch.int32, device=dev)          # pos_dev: positions come from cache.lens
         self.readback = torch.zeros((S, 2), dtype=torch.int64, device=dev)   # (token, finished) per row: one copy out
@@ -1730,6 +1754,15 @@ class ContinuousBatcher:
     def _select(self, logits, rows, lens):
         """The selection of rows `rows` (a slice) from logits [n, 1, V] into self.ids[rows], then the stop strings."""
         ids, fin = self.ids[rows], self.finished[rows]
+        if logits.is_cuda and self.request_options:
+            kernels.sample_tokens_rows_processed(
+                logits, ids, self.greedy[rows], self.temperature[rows], self.top_k[rows], self.top_p[rows],
+                self.seed[rows], self.step_count[rows], self.eos_id[rows], self.active[rows], fin, lens,
+                self.history[rows], self.prompt_len[rows], self.penalty[rows], self.ngram[rows], self.min_length[rows],
+                self.min_new_tokens[rows], self.length_eos[rows], self.n_length_eos[rows])
+            kernels.stop_step_rows(ids, self.row_tables[rows], self.row_states[rows], self.V_tok, self.active[rows],
+                                   self.stop_state[rows], fin)
+            return
         if logits.is_cuda:
             kernels.sample_tokens_rows(logits, ids, self.greedy[rows], self.temperature[rows], self.top_k[rows],
                                        self.top_p[rows], self.seed[rows], self.step_count[rows], self.eos_id[rows],
@@ -1742,14 +1775,33 @@ class ContinuousBatcher:
         if bool((live & (self.greedy[rows] == 0)).any()):
             raise RuntimeError('token sampling runs on the CUDA device only (csrc/sample.cu): logits are on %s'
                                % logits.device)
-        tok = torch.where(live, logits.reshape(live.shape[0], -1).argmax(-1), ids[:, 0])
+        scores = logits.reshape(live.shape[0], -1)
+        if self.request_options:
+            scores = scores.float().clone()
+            for i, s in enumerate(range(self.slots)[rows]):
+                if live[i] and self.row_procs[s] is not None:
+                    scores[i:i + 1] = LogitsProcessors(self.history[s:s + 1], int(self.prompt_len[s]),
+                                                       **self.row_procs[s]).apply(scores[i:i + 1],
+                                                                                  int(self.step_count[s]))
+        tok = torch.where(live, scores.argmax(-1), ids[:, 0])
         ids[:, 0] = tok
         eos = self.eos_id[rows]
         fin |= (live & (eos >= 0) & (tok == eos)).to(torch.int32)
+        if self.request_options:
+            for i, s in enumerate(range(self.slots)[rows]):
+                at = int(self.prompt_len[s] + self.step_count[s])
+                if live[i] and at < self.max_len:
+                    self.history[s, at] = tok[i]
         self.step_count[rows] += live.to(torch.int64)
         if lens is not None:
             lens += live.to(torch.int32)
-        if self.stop_table is not None:
+        if self.request_options:
+            for i, s in enumerate(range(self.slots)[rows]):
+                if live[i] and not fin[i] and self.row_stops[s] is not None:
+                    new, hit = _stop_lookup(self.row_stops[s], tok[i:i + 1], self.stop_state[s:s + 1].to(torch.int64))
+                    self.stop_state[s] = int(new[0])
+                    fin[i] |= int(hit[0])
+        elif self.stop_table is not None:
             state = self.stop_state[rows]
             new, hit = _stop_lookup(self.stop_table, tok, state.to(torch.int64))
             open_ = fin == 0
@@ -1767,12 +1819,18 @@ class ContinuousBatcher:
         return logits
 
     def submit(self, input_ids, images=None, bboxes=None, max_new_tokens=32, do_sample=False, temperature=1.0,
-               top_k=None, top_p=None, generator=None, eos_token_id=None, streamer=None):
+               top_k=None, top_p=None, generator=None, eos_token_id=None, streamer=None, repetition_penalty=1.0,
+               no_repeat_ngram_size=0, min_length=0, min_new_tokens=0, length_eos_ids=None, stop_strings=None):
         """Queue one request and return its Request.  input_ids: int64 [1, L] or [L]; images [1, 3, S, S] or None;
         bboxes: a list of one [K, 4] box tensor, or None.  Sampling as generate(): do_sample with temperature > 0 draws
         from the temperature / top_k / top_p processed softmax with a seed taken from `generator` (default: torch's
         default generator) now, at submission; otherwise the arg-max.  eos_token_id: an id, or a list of one.
-        streamer: transformers' BaseStreamer contract -- put(prompt ids) at admission, put(token) per new token, end()."""
+        streamer: transformers' BaseStreamer contract -- put(prompt ids) at admission, put(token) per new token, end().
+        repetition_penalty, no_repeat_ngram_size, min_length, min_new_tokens, length_eos_ids (1..4 ids; None:
+        [eos_token_id] when one is given) as generate() takes them, and stop_strings (a StopStrings, which replaces the
+        batcher's for this request) need a batcher built with request_options=True; otherwise a value that would
+        change a token raises NotImplementedError.  The request's stop table is built here, before any decode step
+        needs it."""
         ids = torch.as_tensor(input_ids)
         if ids.dim() == 1:
             ids = ids[None]
@@ -1784,6 +1842,16 @@ class ContinuousBatcher:
         if L + n > self.max_len:
             raise ValueError('prompt (%d) + max_new_tokens (%d) exceed the batcher\'s max_len %d'
                              % (L, n, self.max_len))
+        if length_eos_ids is None:
+            length_eos_ids = [] if eos_token_id is None else (
+                list(eos_token_id) if isinstance(eos_token_id, (list, tuple)) else [eos_token_id])
+        neutral = LogitsProcessors.neutral(repetition_penalty, no_repeat_ngram_size, min_length, min_new_tokens,
+                                           length_eos_ids)
+        if not self.request_options and (not neutral or stop_strings is not None):
+            raise NotImplementedError('%s per request: run it with model.generate, or build the batcher with '
+                                      '`request_options=True`' % ('stop_strings' if neutral else
+                                                                  'a logits processor (repetition_penalty, '
+                                                                  'no_repeat_ngram_size, min_length, min_new_tokens)'))
         if isinstance(eos_token_id, (list, tuple)):
             if len(eos_token_id) > 1:
                 raise NotImplementedError('the continuous batcher stops a request on one eos id, got %r: run it with '
@@ -1792,9 +1860,31 @@ class ContinuousBatcher:
         greedy = not (do_sample and temperature > 0)
         if not greedy and top_p is not None and top_p < 0:
             raise ValueError('top_p must be >= 0, got %r' % (top_p,))
+        procs = None
+        if not neutral:
+            procs = dict(repetition_penalty=1.0 if repetition_penalty is None else float(repetition_penalty),
+                         no_repeat_ngram_size=int(no_repeat_ngram_size or 0), min_length=int(min_length or 0),
+                         min_new_tokens=int(min_new_tokens or 0), eos_ids=[int(e) for e in length_eos_ids])
+            if not procs['repetition_penalty'] > 0 or min(procs['no_repeat_ngram_size'], procs['min_length'],
+                                                           procs['min_new_tokens']) < 0:
+                raise ValueError('repetition_penalty must be > 0 and no_repeat_ngram_size, min_length, min_new_tokens '
+                                 '>= 0 (got %r)' % (procs,))
+            if (procs['min_length'] or procs['min_new_tokens']) and len(procs['eos_ids']) > kernels.PROC_ROW_EOS:
+                raise NotImplementedError('the continuous batcher suppresses at most %d eos ids below a minimum length, '
+                                          'got %r: run it with model.generate' % (kernels.PROC_ROW_EOS,
+                                                                                  procs['eos_ids']))
+            if not greedy and procs['repetition_penalty'] != 1.0 and L + n > kernels.PROC_LIST_MAX:
+                raise NotImplementedError('sampling with repetition_penalty holds at most %d prompt + new tokens per '
+                                          'row (%d asked): run it with model.generate and use_hf_loop=True'
+                                          % (kernels.PROC_LIST_MAX, L + n))
+        if stop_strings is not None:
+            if stop_strings.V_tok != self.V_tok:
+                raise ValueError('stop_strings: the table covers %d token ids, the batcher\'s %d (one tokenizer per '
+                                 'batcher)' % (stop_strings.V_tok, self.V_tok))
+            stop_strings.on(self.eng.dev)
         req = Request(ids.to(torch.int64), images, bboxes, n, greedy, float(temperature), int(top_k or 0),
                       1.0 if top_p is None else float(top_p), 0 if greedy else sampling_seed(generator),
-                      -1 if eos_token_id is None else int(eos_token_id), streamer)
+                      -1 if eos_token_id is None else int(eos_token_id), streamer, procs, stop_strings)
         self.queue.append(req)
         return req
 
@@ -1809,11 +1899,45 @@ class ContinuousBatcher:
         req.done = True
         self.running[s] = None
         self.active[s] = 0
+        if self.request_options:          # inactive now: the graph no longer reads its table
+            self.row_stops[s] = self.row_procs[s] = None
         self.clock += 1
         self.retired[s] = self.clock
         if req.streamer is not None:
             req.streamer.end()
         return req
+
+    def _set_row(self, req, s):
+        """Write slot s's device state for `req`: its rule, counters and flags, its stop state and, with
+        request_options, its history (the whole submitted prompt), processors and stop table."""
+        dev, row = self.eng.dev, slice(s, s + 1)
+        L = req.input_ids.shape[1]
+        for t, v in ((self.greedy, int(req.greedy)), (self.temperature, req.temperature), (self.top_k, req.top_k),
+                     (self.top_p, req.top_p), (self.seed, req.seed), (self.step_count, 0),
+                     (self.eos_id, req.eos_id), (self.finished, 0), (self.active, 1)):
+            t[row] = v
+        if not self.request_options:
+            if self.stops is not None:
+                self.stop_state[row] = self.stops.initial_states(req.input_ids, torch.tensor([L])).to(dev)
+            return
+        self.history[s, :L] = req.input_ids[0].to(dev)
+        self.prompt_len[row] = L
+        pr = req.processors or dict(repetition_penalty=1.0, no_repeat_ngram_size=0, min_length=0, min_new_tokens=0,
+                                    eos_ids=[])
+        eos = pr['eos_ids'] if pr['min_length'] or pr['min_new_tokens'] else []
+        for t, v in ((self.penalty, pr['repetition_penalty']), (self.ngram, pr['no_repeat_ngram_size']),
+                     (self.min_length, pr['min_length']), (self.min_new_tokens, pr['min_new_tokens']),
+                     (self.n_length_eos, len(eos))):
+            t[row] = v
+        if eos:
+            self.length_eos[s, :len(eos)] = torch.tensor(eos, dtype=torch.int32).to(dev)
+        self.row_procs[s] = req.processors
+        stops = req.stops if req.stops is not None else self.stops
+        self.row_stops[s] = None if stops is None else stops.on(dev)
+        if stops is not None:
+            self.stop_state[row] = stops.initial_states(req.input_ids, torch.tensor([L])).to(dev)
+            self.row_states[row] = stops.S
+        self.row_tables[row] = 0 if stops is None else self.row_stops[s].data_ptr()
 
     def _admit(self, req, s):
         """Prefill `req` into slot s (batch 1, straight into the slot's rows of the cache) and select its first token.
@@ -1828,12 +1952,7 @@ class ContinuousBatcher:
         images = None if req.images is None else req.images.to(dev, eng.dt)
         logits = eng.forward_device(ids, images, eng.plan_boxes(req.bboxes), validate=True, last_only=True, cache=one)
         try:
-            for t, v in ((self.greedy, int(req.greedy)), (self.temperature, req.temperature), (self.top_k, req.top_k),
-                         (self.top_p, req.top_p), (self.seed, req.seed), (self.step_count, 0),
-                         (self.eos_id, req.eos_id), (self.finished, 0), (self.active, 1)):
-                t[row] = v
-            if self.stops is not None:
-                self.stop_state[row] = self.stops.initial_states(req.input_ids, torch.tensor([L])).to(dev)
+            self._set_row(req, s)
             self._select(logits, row, None)
             self.cache.lens[row] = L
             tok, fin = torch.stack([self.ids[s, 0], self.finished[s].to(torch.int64)]).tolist()
@@ -2026,15 +2145,8 @@ class ContinuousBatcher:
         view.lens = torch.tensor(starts, dtype=torch.int32, device=dev)
         view.length = max(starts)
         for (req, s, p, _) in group:          # the rows' device state, as _admit writes it
-            row = slice(s, s + 1)
-            self.cache.lens[row] = p
-            for t, v in ((self.greedy, int(req.greedy)), (self.temperature, req.temperature), (self.top_k, req.top_k),
-                         (self.top_p, req.top_p), (self.seed, req.seed), (self.step_count, 0),
-                         (self.eos_id, req.eos_id), (self.finished, 0), (self.active, 1)):
-                t[row] = v
-            if self.stops is not None:
-                self.stop_state[row] = self.stops.initial_states(req.input_ids, torch.tensor([req.input_ids.shape[1]])
-                                                                 ).to(dev)
+            self.cache.lens[s:s + 1] = p
+            self._set_row(req, s)
         try:
             logits = eng.extend(view, ids, images, tail_boxes, attention_mask=mask)
             first = []

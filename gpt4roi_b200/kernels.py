@@ -270,6 +270,52 @@ def sample_tokens_rows(logits, out, greedy, temperature, top_k, top_p, seed, ste
 
 
 PROC_LIST_MAX = 8192   # history ids per row that sampling with a repetition penalty holds (csrc/sample.cu)
+PROC_ROW_EOS = 4       # ids a row's minimum lengths suppress in sample_tokens_rows_processed (csrc/sample.cu)
+
+
+def sample_tokens_rows_processed(logits, out, greedy, temperature, top_k, top_p, seed, step, eos_id, active, finished,
+                                 lens, history, prompt_len, repetition_penalty, no_repeat_ngram_size, min_length,
+                                 min_new_tokens, eos_ids, n_eos):
+    """sample_tokens_rows with transformers' history-dependent logits processors per row (include/gpt4roi_b200.h:
+    g4r_sample_tokens_rows_proc_bf16): an active row whose four processors are neutral selects as sample_tokens_rows
+    does; any other selects as sample_tokens_processed on that row alone with L = prompt_len[r] and rng_step = step[r],
+    and writes its token to history[r, prompt_len[r] + step[r]].  The arguments of sample_tokens_rows (lens may be
+    None), then: history, a contiguous device int64 [S, ld_h] tensor; per-row contiguous device vectors of S entries:
+    prompt_len, no_repeat_ngram_size, min_length, min_new_tokens, n_eos (int32), repetition_penalty (fp32); eos_ids, a
+    contiguous device int32 [S, 4] tensor whose row r holds the n_eos[r] ids row r's minimum lengths suppress.  The
+    values are device data: the caller checks them (penalty > 0, lengths >= 0, n_eos <= 4, and a sampled row with a
+    penalty holding at most min(ld_h, PROC_LIST_MAX) history ids)."""
+    rows, act = _logit_rows('sample_tokens_rows_processed', logits)
+    S, V = rows.shape
+    if out.dtype != torch.int64 or out.numel() != S or not out.is_contiguous():
+        raise RuntimeError('sample_tokens_rows_processed: out must be a contiguous int64 tensor of %d elements' % S)
+    named = [('greedy', greedy, torch.int32), ('temperature', temperature, torch.float32),
+             ('top_k', top_k, torch.int32), ('top_p', top_p, torch.float32), ('seed', seed, torch.int64),
+             ('step', step, torch.int64), ('eos_id', eos_id, torch.int32), ('active', active, torch.int32),
+             ('finished', finished, torch.int32), ('lens', lens, torch.int32)]
+    procs = [('prompt_len', prompt_len, torch.int32), ('repetition_penalty', repetition_penalty, torch.float32),
+             ('no_repeat_ngram_size', no_repeat_ngram_size, torch.int32), ('min_length', min_length, torch.int32),
+             ('min_new_tokens', min_new_tokens, torch.int32), ('n_eos', n_eos, torch.int32)]
+    for name, t, dt in named + procs:
+        if t is None and name == 'lens':
+            continue
+        if t is None or t.dtype != dt or t.numel() != S or not t.is_contiguous():
+            raise RuntimeError('sample_tokens_rows_processed: %s must be a contiguous device %s [%d] vector'
+                               % (name, dt, S))
+    if history is None or history.dtype != torch.int64 or history.dim() != 2 or history.shape[0] != S \
+            or history.shape[1] < 1 or not history.is_contiguous():
+        raise RuntimeError('sample_tokens_rows_processed: history must be a contiguous int64 [%d, ld_h] tensor' % S)
+    if eos_ids is None or eos_ids.dtype != torch.int32 or tuple(eos_ids.shape) != (S, PROC_ROW_EOS) \
+            or not eos_ids.is_contiguous():
+        raise RuntimeError('sample_tokens_rows_processed: eos_ids must be a contiguous int32 [%d, %d] tensor'
+                           % (S, PROC_ROW_EOS))
+    _L.require_cuda_same_device([('logits', rows), ('out', out), ('history', history), ('eos_ids', eos_ids)]
+                                + [(n, t) for n, t, _ in named + procs])
+    p = [_L.ptr(t) for _, t, _ in procs]
+    _call('g4r_sample_tokens_rows_proc_bf16', rows.device, _L.ptr(rows), rows.stride(0), S, V,
+          *[_L.ptr(t) for _, t, _ in named[:8]], _L.ptr(finished), _L.ptr(out), _L.ptr(lens), _L.ptr(history),
+          history.shape[1], *p[:5], _L.ptr(eos_ids), p[5], act=act)
+    return out
 
 
 def sample_tokens_processed(logits, out, greedy, temperature=1.0, top_k=0, top_p=1.0, seed=0, rng_step=None, eos_id=-1,
@@ -394,6 +440,28 @@ def stop_step(ids, table, state, finished):
     _L.require_cuda_same_device([('ids', ids), ('table', table), ('state', state), ('finished', finished)])
     _call('g4r_stop_step', ids.device, _L.ptr(ids), _L.ptr(table), table.stride(0), table.shape[0] - 1, table.shape[1],
           B, _L.ptr(state), _L.ptr(finished))
+    return finished
+
+
+def stop_step_rows(ids, tables, n_states, V_tok, active, state, finished):
+    """stop_step with a table per row (include/gpt4roi_b200.h: g4r_stop_step_rows): every row b with active[b] != 0,
+    finished[b] == 0 and a table advances its matcher state by the token ids[b] through its table and sets finished[b]
+    on a hit.  tables: a contiguous device int64 [B] vector of table addresses (0: the row has no stop strings), row b's
+    an int16 [V_tok + 1, n_states[b]] contiguous tensor (engine.StopStrings) the caller keeps alive; V_tok is shared.
+    ids: int64, B contiguous elements; n_states, active, state, finished: contiguous device int32 [B]."""
+    B = ids.numel()
+    if ids.dtype != torch.int64 or not ids.is_contiguous():
+        raise RuntimeError('stop_step_rows: ids must be a contiguous int64 tensor')
+    if int(V_tok) < 1:
+        raise RuntimeError('stop_step_rows: V_tok must be >= 1, got %d' % V_tok)
+    named = [('tables', tables, torch.int64), ('n_states', n_states, torch.int32), ('active', active, torch.int32),
+             ('state', state, torch.int32), ('finished', finished, torch.int32)]
+    for name, t, dt in named:
+        if t is None or t.dtype != dt or t.numel() != B or not t.is_contiguous():
+            raise RuntimeError('stop_step_rows: %s must be a contiguous device %s [%d] vector' % (name, dt, B))
+    _L.require_cuda_same_device([('ids', ids)] + [(n, t) for n, t, _ in named])
+    _call('g4r_stop_step_rows', ids.device, _L.ptr(ids), _L.ptr(tables), _L.ptr(n_states), int(V_tok), B,
+          _L.ptr(active), _L.ptr(state), _L.ptr(finished))
     return finished
 
 

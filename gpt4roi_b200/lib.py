@@ -111,7 +111,9 @@ SIGNATURES = {
     'g4r_sample_tokens_out_bf16': (_i, [_vp, _ll, _i, _i, _f, _i, _f, _i, _c.c_ulonglong, _vp, _i, _i, _vp, _vp,
                                         _vp, _ll, _i, _f, _i, _i, _i, _vp, _i, _i, _vp, _vp, _ll, _vp]),
     'g4r_sample_tokens_rows_bf16': (_i, [_vp, _ll, _i, _i] + [_vp] * 12),
+    'g4r_sample_tokens_rows_proc_bf16': (_i, [_vp, _ll, _i, _i] + [_vp] * 12 + [_ll] + [_vp] * 8),
     'g4r_stop_step': (_i, [_vp, _vp, _ll, _i, _i, _i, _vp, _vp, _vp]),
+    'g4r_stop_step_rows': (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp]),
     'g4r_lookup_step': (_i, [_vp, _vp, _vp, _ll, _i, _i, _i, _i, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
     'g4r_lookup_draft': (_i, [_vp, _vp, _ll, _i, _i, _i, _i, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
     'g4r_decode_attention_beam_bf16': (_i, [_vp, _ll, _vp, _vp, _vp, _ll, _i, _i, _i, _i, _vp, _vp, _i, _f, _vp]),
@@ -158,6 +160,7 @@ F16_TWINS = {
     'g4r_sample_tokens_proc_bf16': 'g4r_sample_tokens_proc_f16',
     'g4r_sample_tokens_out_bf16': 'g4r_sample_tokens_out_f16',
     'g4r_sample_tokens_rows_bf16': 'g4r_sample_tokens_rows_f16',
+    'g4r_sample_tokens_rows_proc_bf16': 'g4r_sample_tokens_rows_proc_f16',
     'g4r_decode_attention_beam_bf16': 'g4r_decode_attention_beam_f16',
     'g4r_beam_step_bf16': 'g4r_beam_step_f16',
     'g4r_beam_step_out_bf16': 'g4r_beam_step_out_f16',

@@ -638,18 +638,24 @@ def _generate_output(res, outs, past_key_values):
 _STOP_STRINGS = collections.OrderedDict()   # (vocabulary, stop strings) -> StopStrings; the last 8 used
 
 
+def _token_strings(tokenizer):
+    """The string of every token id as transformers' matcher sees it (StopStringCriteria.clean_tokenizer_vocab), a list
+    indexed by id, None for ids the vocabulary does not hold."""
+    from transformers.generation.stopping_criteria import StopStringCriteria
+    strings, ids = StopStringCriteria.clean_tokenizer_vocab(tokenizer)
+    by_id = [None] * (max(ids) + 1)
+    for s, i in zip(strings, ids):
+        by_id[i] = s
+    return by_id
+
+
 def stop_strings_from_tokenizer(tokenizer, stop_strings):
     """The engine's StopStrings table for `tokenizer`: its token strings are what transformers' matcher uses
     (StopStringCriteria.clean_tokenizer_vocab).  Kept per (vocabulary, stop strings), as HF keeps its own tables."""
-    from transformers.generation.stopping_criteria import StopStringCriteria
     stops = (stop_strings,) if isinstance(stop_strings, str) else tuple(stop_strings)
     key = (tuple(sorted(tokenizer.get_vocab().items())), stops)     # sorted: a fast tokenizer lists it in no fixed order
     if key not in _STOP_STRINGS:
-        strings, ids = StopStringCriteria.clean_tokenizer_vocab(tokenizer)
-        by_id = [None] * (max(ids) + 1)
-        for s, i in zip(strings, ids):
-            by_id[i] = s
-        _STOP_STRINGS[key] = StopStrings(by_id, stops)
+        _STOP_STRINGS[key] = StopStrings(_token_strings(tokenizer), stops)
         if len(_STOP_STRINGS) > 8:
             _STOP_STRINGS.popitem(last=False)
     _STOP_STRINGS.move_to_end(key)
@@ -954,21 +960,25 @@ class SPILlavaMPTForCausalLM(LlamaForCausalLM, _EngineHost):
                            min_new_tokens=procs['min_new_tokens'], length_eos_ids=procs['eos_ids'], **outs, **lk)
         return _generate_output(res, outs, pkv) if outs['return_dict_in_generate'] else res
 
-    def continuous_batcher(self, slots=8, max_len=2048, tokenizer=None, stop_strings=None, prefix_reuse=False):
+    def continuous_batcher(self, slots=8, max_len=2048, tokenizer=None, stop_strings=None, prefix_reuse=False,
+                           request_options=False):
         """A ContinuousBatcher (engine.ContinuousBatcher: requests join and leave the graphed decode step one row at a
         time) on this model's engine, with `slots` rows of up to max_len tokens each.  stop_strings (with tokenizer=;
         the model's generation config counts, as in generate()) apply to every request.  Its submit(input_ids,
         images=, bboxes=, max_new_tokens=, **generate_kwargs) resolves each request's sampling rule as the engine loop
         of generate() does.  prefix_reuse=True: a request prefills only what no row already holds (a conversation sent
         again whole each turn, several questions on one image); its tokens are then those of
-        generate(past_key_values=) on the conversation (engine.ContinuousBatcher)."""
+        generate(past_key_values=) on the conversation (engine.ContinuousBatcher).  request_options=True: each
+        request may also carry repetition_penalty, no_repeat_ngram_size, min_length, min_new_tokens and its own stop
+        strings, which end it alongside the batcher's (SeamBatcher.submit)."""
         stops = resolve_generate(self, 0, None, stop_strings=stop_strings).stop_strings
         if stops is not None and tokenizer is None:
             raise ValueError(_STOP_STRINGS_NEED_TOKENIZER)
         eng = self._get_engine(self.device)
         return SeamBatcher(self, ContinuousBatcher(eng, slots, max_len, None if stops is None else
                                                    stop_strings_from_tokenizer(tokenizer, stops),
-                                                   prefix_reuse=prefix_reuse))
+                                                   prefix_reuse=prefix_reuse, request_options=request_options),
+                           tokenizer, stops)
 
     def initialize_vision_tokenizer(self, mm_use_im_start_end, tokenizer, device, tune_mm_mlp_adapter=False,
                                     pretrain_mm_mlp_adapter=None):
@@ -1016,10 +1026,32 @@ class SPILlavaMPTForCausalLM(LlamaForCausalLM, _EngineHost):
 
 
 class SeamBatcher:
-    """model.continuous_batcher(): the engine's ContinuousBatcher (`batcher`) with generate()'s keyword resolution."""
+    """model.continuous_batcher(): the engine's ContinuousBatcher (`batcher`) with generate()'s keyword resolution.
+    tokenizer, stop_strings: the batcher's own (continuous_batcher(tokenizer=, stop_strings=)), which a batcher built
+    with request_options=True unites with each request's stop strings."""
 
-    def __init__(self, model, batcher):
+    def __init__(self, model, batcher, tokenizer=None, stop_strings=None):
         self.model, self.batcher = model, batcher
+        self.tokenizer, self.stop_strings = tokenizer, tuple(stop_strings or ())
+        self._vocab = {}                            # id(tokenizer) -> (tokenizer, token strings): cleaned once
+        self._tables = collections.OrderedDict()    # (id(tokenizer), stop strings) -> (tokenizer, StopStrings)
+
+    def _stop_table(self, tokenizer, stops):
+        """The StopStrings of `stops` over `tokenizer`'s vocabulary, padded with ids it does not hold to the
+        batcher's V_tok.  The vocabulary is cleaned once per tokenizer and a table built once per stop set, so a
+        repeated set costs a dictionary lookup."""
+        key = (id(tokenizer), stops)
+        if key in self._tables:
+            self._tables.move_to_end(key)
+            return self._tables[key][1]
+        if id(tokenizer) not in self._vocab:
+            strings = _token_strings(tokenizer)
+            strings += [None] * (self.batcher.V_tok - len(strings))
+            self._vocab[id(tokenizer)] = (tokenizer, strings)
+        self._tables[key] = (tokenizer, StopStrings(self._vocab[id(tokenizer)][1], stops))
+        if len(self._tables) > 64:
+            self._tables.popitem(last=False)
+        return self._tables[key][1]
 
     def submit(self, input_ids, images=None, bboxes=None, max_new_tokens=32, do_sample=None, temperature=None,
                eos_token_id=None, generator=None, streamer=None, **generate_kwargs):
@@ -1030,7 +1062,16 @@ class SeamBatcher:
         this call's arguments.  What the batcher does not run -- logits processors, beam search, several answers per
         prompt, generate outputs, stop strings per request (stop_strings=, or in generation_config) -- raises
         NotImplementedError naming model.generate.  tokenizer= is accepted and unused: the batcher's stop strings, if
-        any, were resolved with its own tokenizer."""
+        any, were resolved with its own tokenizer.
+        On a batcher built with request_options=True, repetition_penalty, no_repeat_ngram_size, min_length and
+        min_new_tokens resolve and run as on generate()'s engine loop, and stop strings (stop_strings=, else
+        generation_config's, else the model's) are matched with the batcher's own: the request ends at the first
+        string of either set.  They are matched over tokenizer=, else the batcher's tokenizer; with neither, HF's
+        ValueError.  Other logits processors, beam search, several answers per prompt, generate outputs and
+        past_key_values still raise NotImplementedError naming model.generate."""
+        if self.batcher.request_options:
+            return self._submit_options(input_ids, images, bboxes, max_new_tokens, do_sample, temperature,
+                                        eos_token_id, generator, streamer, generate_kwargs)
         gen = {k: v for k, v in generate_kwargs.items() if k not in ('pad_token_id', 'attention_mask', 'tokenizer')}
         gc = gen.get('generation_config')
         for k, v in (('stop_strings', gen.pop('stop_strings', None)), ('past_key_values', gen.pop('past_key_values', None)),
@@ -1062,6 +1103,49 @@ class SeamBatcher:
                                       'this request with model.generate' % why)
         return self.batcher.submit(input_ids, images, bboxes, max_new_tokens, r.do_sample, r.temperature, r.top_k,
                                    r.top_p, generator, eos_token_id, streamer)
+
+    def _submit_options(self, input_ids, images, bboxes, max_new_tokens, do_sample, temperature, eos_token_id,
+                        generator, streamer, generate_kwargs):
+        gen = {k: v for k, v in generate_kwargs.items() if k not in ('pad_token_id', 'attention_mask', 'tokenizer')}
+        if gen.pop('past_key_values', None) is not None:
+            raise NotImplementedError('past_key_values per request: the batcher has no conversation cache (build it '
+                                      'with prefix_reuse=True and send the whole conversation); run the request with '
+                                      'model.generate')
+        mask = generate_kwargs.get('attention_mask')
+        if mask is not None and not bool(torch.as_tensor(mask).bool().all()):
+            raise NotImplementedError('a padded prompt: submit its tokens alone, or run it with model.generate')
+        r = resolve_generate(self.model, torch.as_tensor(input_ids).shape[-1], None, do_sample, temperature,
+                             eos_token_id, **gen)
+        if r.num_return_sequences > 1:
+            why = 'num_return_sequences > 1'
+        elif r.layer_outputs:
+            why = _LAYER_OUTPUTS
+        elif r.outputs['return_dict_in_generate']:
+            why = 'return_dict_in_generate / output_scores / output_logits'
+        elif r.beam is not None:
+            why = 'beam search (num_beams=%d) runs on the HF loop only: pass use_hf_loop=True' % r.beam['num_beams']
+        elif r.other:
+            why = '%s run on the HF loop: pass use_hf_loop=True' % ', '.join(r.other)
+        else:
+            why = None
+        if why is not None:
+            raise NotImplementedError('the continuous batcher selects with temperature, top_k, top_p, '
+                                      'repetition_penalty, no_repeat_ngram_size, min_length and min_new_tokens only '
+                                      '(%s): run this request with model.generate' % why)
+        stops = None
+        if r.stop_strings is not None:
+            tok = generate_kwargs.get('tokenizer') or self.tokenizer
+            if tok is None:
+                raise ValueError(_STOP_STRINGS_NEED_TOKENIZER)
+            union = tuple(dict.fromkeys(self.stop_strings + r.stop_strings))
+            stops = self._stop_table(tok, union)
+        procs = r.processors
+        return self.batcher.submit(input_ids, images, bboxes, max_new_tokens, r.do_sample, r.temperature, r.top_k,
+                                   r.top_p, generator, eos_token_id, streamer,
+                                   repetition_penalty=procs['repetition_penalty'],
+                                   no_repeat_ngram_size=procs['no_repeat_ngram_size'], min_length=procs['min_length'],
+                                   min_new_tokens=procs['min_new_tokens'], length_eos_ids=procs['eos_ids'],
+                                   stop_strings=stops)
 
     def step(self):
         return self.batcher.step()

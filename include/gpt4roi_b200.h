@@ -423,6 +423,30 @@ int g4r_sample_tokens_rows_bf16(const void* logits, long long ld, int S, int V, 
                                 const unsigned long long* seed, long long* step, const int* eos_id, const int* active,
                                 int* finished, long long* out_ids, int* lens, void* stream);
 
+/* ---- next-token selection with a rule and history-dependent processors per row -------------------
+ * Replaces, per request of a continuous batch, the logits processors transformers' GenerationMixin._sample runs before
+ * TemperatureLogitsWarper (RepetitionPenaltyLogitsProcessor, NoRepeatNGramLogitsProcessor, MinLengthLogitsProcessor,
+ * MinNewTokensLengthLogitsProcessor), with each request's own values.
+ * g4r_sample_tokens_rows_bf16 (same arguments, same per-row rule, Philox counter (step[r], 0, 0), finished / step /
+ * lens updates) where row r's processors are g4r_sample_tokens_proc_bf16's with
+ *   history: int64 [S, ld_h], row pitch ld_h: row r's history is history[r, 0 .. prompt_len[r] + step[r]);
+ *   repetition_penalty (fp32, 1: off), no_repeat_ngram_size, min_length, min_new_tokens (int32): entry r;
+ *   eos_ids: int32 [S, 4], the first n_eos[r] of row r are the ids the minimum lengths suppress.
+ * An active row whose four processors are neutral (penalty 1, n-gram size 0, and no minimum length or n_eos[r] == 0)
+ * selects exactly as g4r_sample_tokens_rows_bf16; any other active row selects as a B = 1 g4r_sample_tokens_proc_bf16
+ * call on its logits with L = prompt_len[r] and *rng_step = step[r], and writes its token to
+ * history[r, prompt_len[r] + step[r]] (when that is < ld_h).  Inactive rows are left alone.  Sampling with a
+ * repetition penalty lists at most min(ld_h, 8192) penalised ids per row (the caller's check).  V < 65536.
+ * Capturable: every per-step value is read from device memory. */
+int g4r_sample_tokens_rows_proc_bf16(const void* logits, long long ld, int S, int V, const int* greedy,
+                                     const float* temperature, const int* top_k, const float* top_p,
+                                     const unsigned long long* seed, long long* step, const int* eos_id,
+                                     const int* active, int* finished, long long* out_ids, int* lens,
+                                     long long* history, long long ld_h, const int* prompt_len,
+                                     const float* repetition_penalty, const int* no_repeat_ngram_size,
+                                     const int* min_length, const int* min_new_tokens, const int* eos_ids,
+                                     const int* n_eos, void* stream);
+
 /* ---- stop strings (after the next-token selection, once per decode step) ---------------------
  * Replaces transformers.generation.stopping_criteria.StopStringCriteria.__call__ (and, per row, the reference's
  * KeywordsStoppingCriteria, llava/model/utils.py:26-46) for the decode loop: a row stops at the first generated token
@@ -435,6 +459,15 @@ int g4r_sample_tokens_rows_bf16(const void* logits, long long ld, int S, int V, 
  * Capturable: every per-step value is read from device memory. */
 int g4r_stop_step(const long long* ids, const short* step, long long ld, int V_tok, int S, int B, int* state,
                   int* finished, void* stream);
+
+/* g4r_stop_step with a table per row (transformers' StopStringCriteria of each request of a continuous batch):
+ * tables: B device pointers, row b's table int16 [V_tok + 1, S[b]] (row pitch S[b]) or NULL (no stop strings); one
+ * V_tok for every table.  For every row b with active[b] != 0, finished[b] == 0 and a table:
+ * e = tables[b][t][state[b]], t = ids[b] if 0 <= ids[b] < V_tok else V_tok; state[b] = e & 0x7FFF; finished[b] = 1 if
+ * e < 0.  Other rows are left untouched.  ids: int64 [B]; S, active, state, finished: int32 [B].
+ * Capturable: every per-step value is read from device memory. */
+int g4r_stop_step_rows(const long long* ids, const short* const* tables, const int* S, int V_tok, int B,
+                       const int* active, int* state, int* finished, void* stream);
 
 /* ---- prompt-lookup decoding (batch 1; the last launch of each verify step) ---------------------
  * Replaces transformers' PromptLookupCandidateGenerator.get_candidates and the acceptance of
@@ -880,6 +913,14 @@ int g4r_sample_tokens_rows_f16(const void* logits, long long ld, int S, int V, c
                                const float* temperature, const int* top_k, const float* top_p,
                                const unsigned long long* seed, long long* step, const int* eos_id, const int* active,
                                int* finished, long long* out_ids, int* lens, void* stream);
+int g4r_sample_tokens_rows_proc_f16(const void* logits, long long ld, int S, int V, const int* greedy,
+                                    const float* temperature, const int* top_k, const float* top_p,
+                                    const unsigned long long* seed, long long* step, const int* eos_id,
+                                    const int* active, int* finished, long long* out_ids, int* lens,
+                                    long long* history, long long ld_h, const int* prompt_len,
+                                    const float* repetition_penalty, const int* no_repeat_ngram_size,
+                                    const int* min_length, const int* min_new_tokens, const int* eos_ids,
+                                    const int* n_eos, void* stream);
 
 #ifdef __cplusplus
 }
